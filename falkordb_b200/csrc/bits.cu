@@ -73,8 +73,8 @@ void bits_from_csr(const DevCSR &F, DevBits &X) {
 // bit-matrix.  A warp owns 32 consecutive vertices; a 5-stage shuffle butterfly transposes their 32x32 bit
 // block so lane b holds "which of my 32 vertices are in frontier row b" (and row 32+b for the high half).
 // Count pass: popcounts per (tile, row), laid out row-major-by-tile so ONE global exclusive scan yields final
-// CSR positions.  Fill pass: each lane expands its rows' masks into a shared-memory list (u16 tile-local ids),
-// then every row segment is copied out with coalesced stores -- ascending vertex id within each row.
+// CSR positions.  Fill pass: a warp expands one row's masks into a shared-memory list (u16 tile-local ids),
+// then the row segment is copied out with coalesced stores -- ascending vertex id within each row.
 static const u32 TILE_V = 1024;          // vertices per CTA tile
 static const u32 TILE_THREADS = 512;     // 16 warps x 2 groups of 32 vertices
 
@@ -194,341 +194,140 @@ k_bits_count_csa(const u64 *__restrict__ X, u64 n, u64 ntiles, u32 *__restrict__
     }
 }
 
-// Row-per-warp materialise (fill_kernel = 1, default).  Phase A transposes the tile exactly like k_bits_count and parks
-// the 64 x 32 row masks in shared memory; phase B gives each warp whole rows: lane l owns the 32 vertices of mask word l
-// (all lanes see the same row, so their populations are alike and the expansion loop barely diverges), a warp scan places
-// the lanes, the ids go to a warp-private list aligned with the destination modulo 4 entries, and the list leaves as
-// 16-byte stores.  One block barrier per word column (the masks are double-buffered); no block-wide prefix.
-static const u32 FILL2_TSTRIDE = 33;                       // padded row stride of the mask tile (bank-conflict free)
-static const u32 FILL2_LIST = TILE_V + 4;                  // entries per warp list (+3 alignment slack, rounded)
-static const size_t FILL2_SMEM = 2 * 64 * FILL2_TSTRIDE * sizeof(u32) + (TILE_THREADS / 32) * FILL2_LIST * sizeof(unsigned short);
-__global__ void __launch_bounds__(TILE_THREADS)
-k_bits_fill_rows(const u64 *__restrict__ X, u64 n, u32 W, u64 ntiles, const u64 *__restrict__ off, u32 *__restrict__ Cj) {
-    extern __shared__ __align__(16) unsigned char fill2_smem[];
-    u32 *T = reinterpret_cast<u32 *>(fill2_smem);                                   // [2][64][33]
+// Materialise fill.  A CTA owns a 1024-vertex tile (the count pass's tile) and reads each vertex record once: a pass loads
+// G = min(W, 4) word columns of the tile's records -- 32 contiguous bytes per lane and vertex, one whole sector at W >= 4 --
+// transposes them into a 64G x 32 mask tile in shared memory, and the warps then emit whole rows of that tile: lane l owns the
+// 32 vertices of mask word l, a warp scan places the lanes (two rows per shuffle), the ids go to a warp-private u16 list aligned
+// with the destination modulo 4 entries, and the list leaves as 16-byte stores with the tile's high id bits merged by PRMT.
+// The mask tile is double-buffered and the next pass's records are loaded into registers before the rows are expanded, so one
+// block barrier per pass separates the passes and the loads are in flight while the stores drain.  Loading one 8-byte word
+// column per pass instead fetches every 32-byte sector up to four times and leaves loads and stores in separate phases: that is
+// what bounded the fill (the id expansion itself is under 3 % of its time).  64 registers and ~98 KB of shared memory: 2 CTAs per SM.
+template <int W> struct FillCfg {
+    static constexpr u32 G = W < 4 ? W : 4;       // word columns per pass
+    static constexpr u32 NP = W / G;              // passes per tile
+    static constexpr u32 ROWS = 64 * G;           // mask rows per pass
+};
+static const u32 FILL_STRIDE = 33;                          // padded row stride of the mask tile (bank-conflict free)
+static const u32 FILL_LIST = TILE_V + 8;                    // entries per warp list (+3 alignment slack, rounded)
+template <int W> constexpr size_t fill_smem() {
+    return 2 * FillCfg<W>::ROWS * FILL_STRIDE * sizeof(u32) + (TILE_THREADS / 32) * FILL_LIST * sizeof(unsigned short);
+}
+template <int G> __device__ __forceinline__ void ld_words(u64 (&x)[G], const u64 *p) {
+    if constexpr (G == 1) { x[0] = __ldg(p); }
+    else {
+#pragma unroll
+        for (int k = 0; k < G; k += 2) { ulonglong2 q = __ldg(reinterpret_cast<const ulonglong2 *>(p) + k / 2); x[k] = q.x; x[k + 1] = q.y; }
+    }
+}
+template <int W>
+__global__ void __launch_bounds__(TILE_THREADS, 2)
+k_bits_fill(const u64 *__restrict__ X, u64 n, u64 ntiles, const u64 *__restrict__ off, u32 *__restrict__ Cj) {
+    using Cfg = FillCfg<W>;
+    constexpr u32 G = Cfg::G, NP = Cfg::NP, ROWS = Cfg::ROWS, NW = TILE_THREADS / 32, RPW = ROWS / NW;
+    static_assert(RPW % 4 == 0, "rows are scanned in groups of four");
+    extern __shared__ __align__(16) unsigned char fill_smem_raw[];
+    u32 *T = reinterpret_cast<u32 *>(fill_smem_raw);                                // [2][ROWS][FILL_STRIDE]
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    unsigned short *L = reinterpret_cast<unsigned short *>(fill2_smem + 2 * 64 * FILL2_TSTRIDE * sizeof(u32)) + warp * FILL2_LIST;
-    const u32 NW = TILE_THREADS / 32;
+    unsigned short *L = reinterpret_cast<unsigned short *>(fill_smem_raw + 2 * ROWS * FILL_STRIDE * sizeof(u32)) + warp * FILL_LIST;
     const u64 strm = policy_stream();
     const u64 tile = blockIdx.x;
     const u64 vbase = tile * TILE_V;
-    const u32 vb = (u32)vbase;
-    for (u32 w = 0; w < W; w++) {
-        u32 *Tw = T + (w & 1) * 64 * FILL2_TSTRIDE;
+    const u32 lo16base = (u32)(vbase & 0xFFFFu), vbhi = (u32)(vbase >> 16);     // a 1024-aligned tile never crosses 2^16
+    u64 x[2][G];
+#pragma unroll
+    for (u32 g = 0; g < 2; g++) {
+        const u64 v = vbase + (u64)warp * 64 + g * 32 + lane;
+        if (v < n) ld_words<G>(x[g], X + v * W);
+        else {
+#pragma unroll
+            for (u32 k = 0; k < G; k++) x[g][k] = 0;
+        }
+    }
+    for (u32 p = 0; p < NP; p++) {
+        u32 *Tp = T + (p & 1) * ROWS * FILL_STRIDE;
 #pragma unroll
         for (u32 g = 0; g < 2; g++) {
-            u64 v = vbase + (u64)warp * 64 + g * 32 + lane;
-            u64 word = (v < n) ? X[v * W + w] : 0ULL;
-            u32 tl = 0, th = 0;
-            if (__ballot_sync(0xffffffffu, word != 0ULL)) {
-                tl = transpose32((u32)word, lane);
-                th = transpose32((u32)(word >> 32), lane);
+#pragma unroll
+            for (u32 k = 0; k < G; k++) {
+                u32 tl = 0, th = 0;
+                if (__ballot_sync(0xffffffffu, x[g][k] != 0ULL)) {
+                    tl = transpose32((u32)x[g][k], lane);
+                    th = transpose32((u32)(x[g][k] >> 32), lane);
+                }
+                Tp[(k * 64 + lane) * FILL_STRIDE + 2 * warp + g] = tl;
+                Tp[(k * 64 + 32 + lane) * FILL_STRIDE + 2 * warp + g] = th;
             }
-            Tw[lane * FILL2_TSTRIDE + 2 * warp + g] = tl;
-            Tw[(lane + 32) * FILL2_TSTRIDE + 2 * warp + g] = th;
         }
-        __syncthreads();
-        for (u32 r = warp; r < 64; r += NW) {
-            u32 m = Tw[r * FILL2_TSTRIDE + lane];
-            u32 c = __popc(m), incl = c;
-#pragma unroll
-            for (u32 d = 1; d < 32; d <<= 1) { u32 t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
-            const u32 cnt = __shfl_sync(0xffffffffu, incl, 31);
-            if (cnt == 0) continue;
-            const u64 g0 = off[((u64)w * 64 + r) * ntiles + tile];
-            const u32 a = (u32)(g0 & 3);
-            u32 o = a + incl - c;
-            const u32 idb = lane * 32;
-            while (m) { u32 bit = __ffs(m) - 1; L[o++] = (unsigned short)(idb + bit); m &= m - 1; }
-            __syncwarp();
-            u32 *dst = Cj + (g0 - a);                       // 16-byte aligned; dst[i] <-> L[i] for i in [a, a + cnt)
-            const u32 total = a + cnt;
-            const u32 head_end = a ? (total < 4 ? total : 4) : 0;
-            if (lane >= a && lane < head_end) st_u32_stream(dst + lane, vb + L[lane], strm);
-            const u32 nfull = total >> 2;
-            const uint2 *L2 = reinterpret_cast<const uint2 *>(L);
-            uint4 *dv = reinterpret_cast<uint4 *>(dst);
-            for (u32 i = (a ? 1 : 0) + lane; i < nfull; i += 32) {
-                uint2 p = L2[i];
-                uint4 q;
-                q.x = vb + (p.x & 0xFFFFu); q.y = vb + (p.x >> 16); q.z = vb + (p.y & 0xFFFFu); q.w = vb + (p.y >> 16);
-                __stcs(dv + i, q);
-            }
-            const u32 tail = nfull * 4 > head_end ? nfull * 4 : head_end;
-            if (tail + lane < total) st_u32_stream(dst + tail + lane, vb + L[tail + lane], strm);
-            __syncwarp();
-        }
-    }
-}
-
-// Row-per-warp materialise over 2048-vertex tiles (fill_kernel = 3, default).  Same two phases as k_bits_fill_rows; what changed is
-// the bookkeeping per emitted entry, which is what bounds this kernel (issue slots, not bytes): a (row, tile) pass now
-// covers 2048 vertices (each lane owns a 64-bit mask), a warp scans the counts of its rows in PAIRS (two 16-bit fields per
-// shuffle), the four output offsets of a word column are fetched before the scans so their latency overlaps, and the staged ids
-// keep only their low 16 bits -- the high half is merged with one PRMT on the way out.  ~1.0 instructions per entry against 1.6.
-static const u32 F3_TILE = 2048, F3_THREADS = 512, F3_STRIDE = 66, F3_LIST = F3_TILE + 8;
-static const size_t F3_SMEM = 2 * 64 * F3_STRIDE * sizeof(u32) + (F3_THREADS / 32) * F3_LIST * sizeof(unsigned short);
-__global__ void __launch_bounds__(F3_THREADS, 2)
-k_bits_fill_v3(const u64 *__restrict__ X, u64 n, u32 W, u64 ntiles1k, const u64 *__restrict__ off, u32 *__restrict__ Cj) {
-    extern __shared__ __align__(16) unsigned char f3_smem[];
-    u32 *T = reinterpret_cast<u32 *>(f3_smem);                                      // [2][64][F3_STRIDE]
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    unsigned short *L = reinterpret_cast<unsigned short *>(f3_smem + 2 * 64 * F3_STRIDE * sizeof(u32)) + warp * F3_LIST;
-    constexpr u32 NW = F3_THREADS / 32, RPW = 64 / NW;                              // 16 warps, 4 rows per warp and word column
-    const u64 strm = policy_stream();
-    const u64 tile = blockIdx.x;
-    const u64 vbase = tile * F3_TILE;
-    const u32 lo16base = (u32)(vbase & 0xFFFFu), vbhi = (u32)(vbase >> 16);
-    for (u32 w = 0; w < W; w++) {
-        u32 *Tw = T + (w & 1) * 64 * F3_STRIDE;
-        // offsets of this warp's rows: issued first, consumed after the scans
-        u64 g0[RPW];
-#pragma unroll
-        for (u32 i = 0; i < RPW; i++) g0[i] = off[((u64)w * 64 + warp + NW * i) * ntiles1k + 2 * tile];
-#pragma unroll
-        for (u32 g = 0; g < 4; g++) {
-            const u64 v = vbase + (u64)warp * 128 + g * 32 + lane;
-            const u64 word = (v < n) ? X[v * W + w] : 0ULL;
-            u32 tl = 0, th = 0;
-            if (__ballot_sync(0xffffffffu, word != 0ULL)) {
-                tl = transpose32((u32)word, lane);
-                th = transpose32((u32)(word >> 32), lane);
-            }
-            Tw[lane * F3_STRIDE + 4 * warp + g] = tl;
-            Tw[(lane + 32) * F3_STRIDE + 4 * warp + g] = th;
-        }
-        __syncthreads();
-        u64 m[RPW];
-        u32 c[RPW];
-#pragma unroll
-        for (u32 i = 0; i < RPW; i++) {
-            m[i] = *reinterpret_cast<const u64 *>(Tw + (warp + NW * i) * F3_STRIDE + 2 * lane);
-            c[i] = __popcll(m[i]);
-        }
-        u32 pk[RPW / 2];
-#pragma unroll
-        for (u32 h = 0; h < RPW / 2; h++) pk[h] = c[2 * h] | (c[2 * h + 1] << 16);     // prefixes stay below 2^16 (tile = 2048)
-#pragma unroll
-        for (u32 d = 1; d < 32; d <<= 1) {
-#pragma unroll
-            for (u32 h = 0; h < RPW / 2; h++) { const u32 t = __shfl_up_sync(0xffffffffu, pk[h], d); if (lane >= d) pk[h] += t; }
-        }
-#pragma unroll
-        for (u32 i = 0; i < RPW; i++) {
-            const u32 field = (i & 1) ? (pk[i / 2] >> 16) : (pk[i / 2] & 0xFFFFu);
-            const u32 cnt = __shfl_sync(0xffffffffu, field, 31);
-            if (cnt == 0) continue;
-            const u32 a = (u32)(g0[i] & 3);
-            u32 o = a + field - c[i];
-            u32 idb = lo16base + lane * 64;
-            u32 lo = (u32)m[i], hi = (u32)(m[i] >> 32);
-            while (lo) { const u32 bit = __ffs(lo) - 1; L[o++] = (unsigned short)(idb + bit); lo &= lo - 1; }
-            idb += 32;
-            while (hi) { const u32 bit = __ffs(hi) - 1; L[o++] = (unsigned short)(idb + bit); hi &= hi - 1; }
-            __syncwarp();
-            u32 *dst = Cj + (g0[i] - a);                    // 16-byte aligned; dst[k] <-> L[k] for k in [a, a + cnt)
-            const u32 total = a + cnt;
-            const u32 head_end = a ? (total < 4 ? total : 4) : 0;
-            if (lane >= a && lane < head_end) st_u32_stream(dst + lane, (vbhi << 16) | L[lane], strm);
-            const u32 nfull = total >> 2;
-            const uint2 *L2 = reinterpret_cast<const uint2 *>(L);
-            uint4 *dv = reinterpret_cast<uint4 *>(dst);
-            for (u32 k = (a ? 1 : 0) + lane; k < nfull; k += 32) {
-                const uint2 p = L2[k];
-                uint4 q;
-                q.x = __byte_perm(p.x, vbhi, 0x5410); q.y = __byte_perm(p.x, vbhi, 0x5432);
-                q.z = __byte_perm(p.y, vbhi, 0x5410); q.w = __byte_perm(p.y, vbhi, 0x5432);
-                __stcs(dv + k, q);
-            }
-            const u32 tail = nfull * 4 > head_end ? nfull * 4 : head_end;
-            if (tail + lane < total) st_u32_stream(dst + tail + lane, (vbhi << 16) | L[tail + lane], strm);
-            __syncwarp();
-        }
-    }
-}
-
-// Materialise with the transposed masks kept (fill_kernel = 2, default).  k_bits_count_keep counts like k_bits_count and also
-// writes the 64 x 32 row masks of every (word column, tile) to global memory, coalesced (8 KB per tile); k_bits_fill_masks is
-// then phase B of k_bits_fill_rows alone: a warp reads one row's 32 mask words with one 128-byte load -- no second transpose,
-// no shared tile, no block barrier.  The masks cost one extra write + read of the bit-matrix (2 x 8*W*n bytes), cheap for
-// kernels that are instruction-bound, not DRAM-bound.
-__global__ void __launch_bounds__(TILE_THREADS)
-k_bits_count_keep(const u64 *__restrict__ X, u64 n, u32 W, u64 ntiles, u32 *__restrict__ tc, u32 *__restrict__ Tg) {
-    __shared__ __align__(16) u32 T[64 * FILL2_TSTRIDE];
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const u64 tile = blockIdx.x;
-    const u64 vbase = tile * TILE_V;
-    for (u32 w = 0; w < W; w++) {
-#pragma unroll
-        for (u32 g = 0; g < 2; g++) {
-            u64 v = vbase + (u64)warp * 64 + g * 32 + lane;
-            u64 word = (v < n) ? X[v * W + w] : 0ULL;
-            u32 tl = 0, th = 0;
-            if (__ballot_sync(0xffffffffu, word != 0ULL)) {
-                tl = transpose32((u32)word, lane);
-                th = transpose32((u32)(word >> 32), lane);
-            }
-            T[lane * FILL2_TSTRIDE + 2 * warp + g] = tl;
-            T[(lane + 32) * FILL2_TSTRIDE + 2 * warp + g] = th;
-        }
-        __syncthreads();
-        {   // thread (r, c4): 4 consecutive mask words of row r -> one 16-byte store; 8 threads cover the row
-            const u32 r = tid >> 3, c4 = (tid & 7) * 4;
-            uint4 q;
-            q.x = T[r * FILL2_TSTRIDE + c4]; q.y = T[r * FILL2_TSTRIDE + c4 + 1];
-            q.z = T[r * FILL2_TSTRIDE + c4 + 2]; q.w = T[r * FILL2_TSTRIDE + c4 + 3];
-            u32 c = __popc(q.x) + __popc(q.y) + __popc(q.z) + __popc(q.w);
-            c += __shfl_xor_sync(0xffffffffu, c, 1);
-            c += __shfl_xor_sync(0xffffffffu, c, 2);
-            c += __shfl_xor_sync(0xffffffffu, c, 4);
-            if ((tid & 7) == 0) tc[((u64)w * 64 + r) * ntiles + tile] = c;
-            *reinterpret_cast<uint4 *>(Tg + (((u64)w * ntiles + tile) * 64 + r) * 32 + c4) = q;
-        }
-        __syncthreads();
-    }
-}
-
-static const u32 FILLM_WARPS = 8;                          // warps per CTA of k_bits_fill_masks (one list each)
-__global__ void __launch_bounds__(FILLM_WARPS * 32)
-k_bits_fill_masks(const u32 *__restrict__ Tg, u32 W, u64 ntiles, const u64 *__restrict__ off, u32 *__restrict__ Cj) {
-    __shared__ __align__(16) unsigned short lists[FILLM_WARPS][FILL2_LIST];
-    const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    unsigned short *L = lists[warp];
-    const u64 strm = policy_stream();
-    const u64 ntasks = (u64)W * ntiles * 64;               // task = (word column, tile, row), masks stored in that order
-    const u64 nwarps = (u64)gridDim.x * FILLM_WARPS;
-    u64 task = (u64)blockIdx.x * FILLM_WARPS + warp;
-    u32 mnext = task < ntasks ? __ldg(Tg + task * 32 + lane) : 0;
-    for (; task < ntasks; task += nwarps) {
-        u32 m = mnext;
-        if (task + nwarps < ntasks) mnext = __ldg(Tg + (task + nwarps) * 32 + lane);   // next task's masks in flight
-        u32 c = __popc(m), incl = c;
-#pragma unroll
-        for (u32 d = 1; d < 32; d <<= 1) { u32 t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += t; }
-        const u32 cnt = __shfl_sync(0xffffffffu, incl, 31);
-        if (cnt == 0) continue;
-        const u32 r = (u32)(task & 63);
-        const u64 wt = task >> 6, w = wt / ntiles, tile = wt - w * ntiles;
-        const u32 vb = (u32)(tile * TILE_V);
-        const u64 g0 = off[(w * 64 + r) * ntiles + tile];
-        const u32 a = (u32)(g0 & 3);
-        u32 o = a + incl - c;
-        const u32 idb = lane * 32;
-        while (m) { u32 bit = __ffs(m) - 1; L[o++] = (unsigned short)(idb + bit); m &= m - 1; }
-        __syncwarp();
-        u32 *dst = Cj + (g0 - a);                           // 16-byte aligned; dst[i] <-> L[i] for i in [a, a + cnt)
-        const u32 total = a + cnt;
-        const u32 head_end = a ? (total < 4 ? total : 4) : 0;
-        if (lane >= a && lane < head_end) st_u32_stream(dst + lane, vb + L[lane], strm);
-        const u32 nfull = total >> 2;
-        const uint2 *L2 = reinterpret_cast<const uint2 *>(L);
-        uint4 *dv = reinterpret_cast<uint4 *>(dst);
-        for (u32 i = (a ? 1 : 0) + lane; i < nfull; i += 32) {
-            uint2 p = L2[i];
-            uint4 q;
-            q.x = vb + (p.x & 0xFFFFu); q.y = vb + (p.x >> 16); q.z = vb + (p.y & 0xFFFFu); q.w = vb + (p.y >> 16);
-            __stcs(dv + i, q);
-        }
-        const u32 tail = nfull * 4 > head_end ? nfull * 4 : head_end;
-        if (tail + lane < total) st_u32_stream(dst + tail + lane, vb + L[tail + lane], strm);
-        __syncwarp();
-    }
-}
-
-__global__ void __launch_bounds__(TILE_THREADS)
-k_bits_fill(const u64 *__restrict__ X, u64 n, u32 W, u64 ntiles, const u64 *__restrict__ off, u32 *__restrict__ Cj,
-            u32 cap) {
-    extern __shared__ unsigned short list[];             // `cap` tile-local ids (sized from the average tile density)
-    __shared__ unsigned short wp[TILE_THREADS / 32][64];  // per-warp exclusive prefix, per row
-    __shared__ u32 sbase[65];                            // row segment starts inside `list`
-    __shared__ u64 goff[64];                             // row segment starts in the output
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const u32 NW = TILE_THREADS / 32;
-    const u64 strm = policy_stream();
-    u64 tile = blockIdx.x;
-    u64 vbase = tile * TILE_V;
-    for (u32 w = 0; w < W; w++) {
-        u32 tlo[2], thi[2];
-        u32 clo = 0, chi = 0;
-#pragma unroll
-        for (u32 g = 0; g < 2; g++) {
-            u64 v = vbase + (u64)warp * 64 + g * 32 + lane;
-            u64 word = (v < n) ? X[v * W + w] : 0ULL;
-            tlo[g] = 0; thi[g] = 0;
-            if (__ballot_sync(0xffffffffu, word != 0ULL)) {
-                tlo[g] = transpose32((u32)word, lane);
-                thi[g] = transpose32((u32)(word >> 32), lane);
-            }
-            clo += __popc(tlo[g]);
-            chi += __popc(thi[g]);
-        }
-        wp[warp][lane] = (unsigned short)clo;
-        wp[warp][lane + 32] = (unsigned short)chi;
-        __syncthreads();
-        if (tid < 64) {
-            u32 run = 0;
-#pragma unroll
-            for (u32 q = 0; q < NW; q++) { u32 t = wp[q][tid]; wp[q][tid] = (unsigned short)run; run += t; }
-            sbase[tid + 1] = run; // totals for now
-            goff[tid] = off[((u64)w * 64 + tid) * ntiles + tile];
-        }
-        __syncthreads();
-        if (tid == 0) {
-            u32 run = 0;
-            sbase[0] = 0;
-            for (u32 r = 0; r < 64; r++) { u32 t = sbase[r + 1]; sbase[r + 1] = run + t; run += t; }
-        }
-        __syncthreads();
-        const bool staged = sbase[64] <= cap;   // denser-than-provisioned tiles write straight to global memory
-        if (!staged) {
-            u64 o = goff[lane] + wp[warp][lane];
+        if (p + 1 < NP) {                               // next pass's words in flight during this pass's expansion
 #pragma unroll
             for (u32 g = 0; g < 2; g++) {
-                u32 m = tlo[g];
-                u64 idb = vbase + warp * 64 + g * 32;
-                while (m) { u32 bit = __ffs(m) - 1; Cj[o++] = (u32)(idb + bit); m &= m - 1; }
-            }
-            o = goff[lane + 32] + wp[warp][lane + 32];
-#pragma unroll
-            for (u32 g = 0; g < 2; g++) {
-                u32 m = thi[g];
-                u64 idb = vbase + warp * 64 + g * 32;
-                while (m) { u32 bit = __ffs(m) - 1; Cj[o++] = (u32)(idb + bit); m &= m - 1; }
-            }
-            __syncthreads();
-            continue;
-        }
-        // expand: lane b owns rows b (low half) and 32+b (high half) of this warp's 64 vertices
-        {
-            u32 o = sbase[lane] + wp[warp][lane];
-#pragma unroll
-            for (u32 g = 0; g < 2; g++) {
-                u32 m = tlo[g];
-                u32 idb = warp * 64 + g * 32;
-                while (m) { u32 bit = __ffs(m) - 1; list[o++] = (unsigned short)(idb + bit); m &= m - 1; }
-            }
-            o = sbase[lane + 32] + wp[warp][lane + 32];
-#pragma unroll
-            for (u32 g = 0; g < 2; g++) {
-                u32 m = thi[g];
-                u32 idb = warp * 64 + g * 32;
-                while (m) { u32 bit = __ffs(m) - 1; list[o++] = (unsigned short)(idb + bit); m &= m - 1; }
+                const u64 v = vbase + (u64)warp * 64 + g * 32 + lane;
+                if (v < n) ld_words<G>(x[g], X + v * W + (p + 1) * G);
             }
         }
         __syncthreads();
-        // coalesced copy-out: warp q handles rows q, q+NW, ...
-        for (u32 r = warp; r < 64; r += NW) {
-            u32 s = sbase[r], cnt = sbase[r + 1] - s;
-            u32 *dst = Cj + goff[r];
-            for (u32 i = lane; i < cnt; i += 32) st_u32_stream(dst + i, (u32)(vbase + list[s + i]), strm);
+        // rows of this pass: r = warp + NW * i; row r is frontier row 64 * (p * G) + r
+        const u64 obase = (u64)p * ROWS;
+#pragma unroll 1
+        for (u32 i0 = 0; i0 < RPW; i0 += 4) {
+            u64 g0[4];
+#pragma unroll
+            for (u32 i = 0; i < 4; i++) g0[i] = off[(obase + warp + NW * (i0 + i)) * ntiles + tile];
+            u32 m[4], c[4];
+#pragma unroll
+            for (u32 i = 0; i < 4; i++) { m[i] = Tp[(warp + NW * (i0 + i)) * FILL_STRIDE + lane]; c[i] = __popc(m[i]); }
+            u32 pk[2] = {c[0] | (c[1] << 16), c[2] | (c[3] << 16)};          // prefixes stay below 2^16 (tile = 1024)
+#pragma unroll
+            for (u32 d = 1; d < 32; d <<= 1) {
+#pragma unroll
+                for (u32 h = 0; h < 2; h++) { const u32 t = __shfl_up_sync(0xffffffffu, pk[h], d); if (lane >= d) pk[h] += t; }
+            }
+#pragma unroll
+            for (u32 i = 0; i < 4; i++) {
+                const u32 field = (i & 1) ? (pk[i / 2] >> 16) : (pk[i / 2] & 0xFFFFu);
+                const u32 cnt = __shfl_sync(0xffffffffu, field, 31);
+                if (cnt == 0) continue;
+                const u32 a = (u32)(g0[i] & 3);
+                u32 o = a + field - c[i];
+                const u32 idb = lo16base + lane * 32;
+                u32 mm = m[i];
+                while (mm) { const u32 bit = __ffs(mm) - 1; L[o++] = (unsigned short)(idb + bit); mm &= mm - 1; }
+                __syncwarp();
+                u32 *dst = Cj + (g0[i] - a);                // 16-byte aligned; dst[k] <-> L[k] for k in [a, a + cnt)
+                const u32 total = a + cnt;
+                const u32 head_end = a ? (total < 4 ? total : 4) : 0;
+                if (lane >= a && lane < head_end) st_u32_stream(dst + lane, (vbhi << 16) | L[lane], strm);
+                const u32 nfull = total >> 2;
+                const uint2 *L2 = reinterpret_cast<const uint2 *>(L);
+                uint4 *dv = reinterpret_cast<uint4 *>(dst);
+                for (u32 k = (a ? 1 : 0) + lane; k < nfull; k += 32) {
+                    const uint2 q2 = L2[k];
+                    uint4 q;
+                    q.x = __byte_perm(q2.x, vbhi, 0x5410); q.y = __byte_perm(q2.x, vbhi, 0x5432);
+                    q.z = __byte_perm(q2.y, vbhi, 0x5410); q.w = __byte_perm(q2.y, vbhi, 0x5432);
+                    __stcs(dv + k, q);
+                }
+                const u32 tail = nfull * 4 > head_end ? nfull * 4 : head_end;
+                if (tail + lane < total) st_u32_stream(dst + tail + lane, (vbhi << 16) | L[tail + lane], strm);
+                __syncwarp();
+            }
         }
-        __syncthreads();
     }
 }
 
 __global__ void k_bits_rowptr(const u64 *__restrict__ off, u64 nrows, u64 ntiles, u64 *__restrict__ Cp) {
     u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (r <= nrows) Cp[r] = off[r * ntiles];
+}
+
+template <int W> static void launch_fill(const DevBits &X, u64 ntiles, const u64 *off, u32 *Cj) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        CUDA_TRY(cudaFuncSetAttribute(k_bits_fill<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fill_smem<W>()));
+        attr_set = true;
+    }
+    LAUNCH(k_bits_fill<W>, (u32)ntiles, TILE_THREADS, fill_smem<W>(), X.w.ptr, X.ncols, ntiles, off, Cj);
 }
 
 void bits_to_csr(const DevBits &X, DevCSR &C) {
@@ -543,13 +342,9 @@ void bits_to_csr(const DevBits &X, DevCSR &C) {
     u64 ncnt = (u64)64 * W * ntiles;
     DevBuf<u32> tc(ncnt + 1);
     DevBuf<u64> off(ncnt + 1);
-    const bool keep_masks = ctx().opt_fill_kernel == 2 && ctx().opt_fill_cap <= 0;
-    DevBuf<u32> masks;
-    if (keep_masks) masks.alloc((u64)W * ntiles * 64 * 32);
     {
-        TimedScope ts(TK_BITS_COUNT, 8ULL * W * n + (keep_masks ? 8ULL * W * ntiles * TILE_V : 0));
-        if (keep_masks) LAUNCH(k_bits_count_keep, (u32)ntiles, TILE_THREADS, 0, X.w.ptr, n, W, ntiles, tc.ptr, masks.ptr);
-        else if (ctx().opt_count_kernel == 1) {
+        TimedScope ts(TK_BITS_COUNT, 8ULL * W * n);
+        if (ctx().opt_count_kernel == 1) {
             const u64 nwarps = ntiles * pull_split((int)W);
             const u32 g = (u32)((nwarps + 3) / 4);
             switch (W) {
@@ -569,31 +364,13 @@ void bits_to_csr(const DevBits &X, DevCSR &C) {
     C.nnz = nnz;
     C.j.alloc(nnz);
     if (nnz) {
-        static bool attr_set = false;
-        if (!attr_set) {
-            CUDA_TRY(cudaFuncSetAttribute(k_bits_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(64 * TILE_V * sizeof(unsigned short))));
-            CUDA_TRY(cudaFuncSetAttribute(k_bits_fill_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FILL2_SMEM));
-            CUDA_TRY(cudaFuncSetAttribute(k_bits_fill_v3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F3_SMEM));
-            attr_set = true;
-        }
         TimedScope ts(TK_BITS_FILL, 8ULL * W * n + 4 * nnz);
-        if (keep_masks) {
-            LAUNCH(k_bits_fill_masks, (u32)ctx().num_sms * 8, FILLM_WARPS * 32, 0, masks.ptr, W, ntiles, off.ptr, C.j.ptr);
-        } else if (ctx().opt_fill_kernel == 3 && ctx().opt_fill_cap <= 0 && W <= 8) {
-            // (at W = 16 the 2048-vertex tile's 128 KB of frontier words per CTA no longer survives in L1 next to 100 KB of shared
-            // memory and the word columns are re-fetched from L2 -- the 1024-vertex kernel below takes W = 16)
-            LAUNCH(k_bits_fill_v3, (u32)((n + F3_TILE - 1) / F3_TILE), F3_THREADS, F3_SMEM, X.w.ptr, n, W, ntiles, off.ptr, C.j.ptr);
-        } else if ((ctx().opt_fill_kernel == 1 || ctx().opt_fill_kernel == 3) && ctx().opt_fill_cap <= 0) {
-            LAUNCH(k_bits_fill_rows, (u32)ntiles, TILE_THREADS, FILL2_SMEM, X.w.ptr, n, W, ntiles, off.ptr, C.j.ptr);
-        } else {
-            // staging capacity from the average (tile, word) population, 1.5x headroom, 8K-entry steps: sparse frontiers
-            // get small shared-memory footprints and therefore several resident CTAs per SM
-            u64 avg = nnz / (ntiles * W) + 1;
-            u32 cap = 8192;
-            while (cap < 65536 && (u64)cap < avg + avg / 2) cap += 8192;
-            if (ctx().opt_fill_cap > 0) cap = (u32)ctx().opt_fill_cap; // test hook: force the direct-write path
-            const size_t smem = (size_t)cap * sizeof(unsigned short);
-            LAUNCH(k_bits_fill, (u32)ntiles, TILE_THREADS, smem, X.w.ptr, n, W, ntiles, off.ptr, C.j.ptr, cap);
+        switch (W) {
+        case 1: launch_fill<1>(X, ntiles, off.ptr, C.j.ptr); break;
+        case 2: launch_fill<2>(X, ntiles, off.ptr, C.j.ptr); break;
+        case 4: launch_fill<4>(X, ntiles, off.ptr, C.j.ptr); break;
+        case 8: launch_fill<8>(X, ntiles, off.ptr, C.j.ptr); break;
+        default: launch_fill<16>(X, ntiles, off.ptr, C.j.ptr); break;
         }
     }
 }
@@ -652,7 +429,7 @@ void bits_diag(const DevBits &X, const DevCSR &A, DevBits &Y, u64 *flops_out) {
 // out as 128-byte row segments; rows >= nrows (padding of the last word column) are dropped.
 __global__ void __launch_bounds__(TILE_THREADS)
 k_bits_rowmajor(const u64 *__restrict__ X, u64 n, u32 W, u64 nrows, u64 wpr, u64 *__restrict__ out) {
-    __shared__ u32 T[2][64 * FILL2_TSTRIDE];
+    __shared__ u32 T[2][64 * FILL_STRIDE];
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const u64 tile = blockIdx.x;
     const u64 vbase = tile * TILE_V;
@@ -669,8 +446,8 @@ k_bits_rowmajor(const u64 *__restrict__ X, u64 n, u32 W, u64 nrows, u64 wpr, u64
                 tl = transpose32((u32)word, lane);
                 th = transpose32((u32)(word >> 32), lane);
             }
-            Tw[lane * FILL2_TSTRIDE + 2 * warp + g] = tl;
-            Tw[(lane + 32) * FILL2_TSTRIDE + 2 * warp + g] = th;
+            Tw[lane * FILL_STRIDE + 2 * warp + g] = tl;
+            Tw[(lane + 32) * FILL_STRIDE + 2 * warp + g] = th;
         }
         __syncthreads();
 #pragma unroll
@@ -678,7 +455,7 @@ k_bits_rowmajor(const u64 *__restrict__ X, u64 n, u32 W, u64 nrows, u64 wpr, u64
             u32 r = (tid >> 4) + 32 * h, c = tid & 15;
             u64 row = (u64)w * 64 + r, col = tile * (TILE_V / 64) + c;
             if (row < nrows && col < wpr) {
-                u64 val = (u64)Tw[r * FILL2_TSTRIDE + 2 * c] | ((u64)Tw[r * FILL2_TSTRIDE + 2 * c + 1] << 32);
+                u64 val = (u64)Tw[r * FILL_STRIDE + 2 * c] | ((u64)Tw[r * FILL_STRIDE + 2 * c + 1] << 32);
                 st_u64_stream(out + row * wpr + col, val, strm);
             }
         }

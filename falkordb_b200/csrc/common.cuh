@@ -66,8 +66,6 @@ struct Context {
     i64 opt_hints = -1;            // L2 createpolicy hints in the pull kernels: -1 = auto (on for W <= 2), 0 / 1 = off / on
     i64 opt_hot_bytes = 64 << 20;  // size of that hot prefix
     i64 opt_hot_pack = 1;          // gather through the degree-sorted, sink-free relabelling of the frontier
-    i64 opt_fill_cap = 0;          // 0 = auto; >0 forces the materialise staging capacity (test hook)
-    i64 opt_fill_kernel = 3;       // materialise: 3 = row-per-warp over 2048-vertex tiles, paired scans (default); 1 = row-per-warp, 1024-vertex tiles; 0 = block-staged lists; 2 = from kept masks
     i64 opt_fused_prep = 1;        // pull hops: pack the frontier, count flops / edges and OR it in one pass
     i64 opt_csr_push = 1;          // tiny CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes)
     i64 opt_diag_filter = 1;       // frontier-form mxm by a diagonal (label) matrix runs as an elementwise column filter

@@ -2490,10 +2490,8 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "hot_pack") c.opt_hot_pack = value;
     else if (n == "hot_bytes") c.opt_hot_bytes = value;
     else if (n == "early_exit") c.opt_early_exit = value;
-    else if (n == "fill_cap") c.opt_fill_cap = value;
     else if (n == "unroll") c.opt_unroll = value;
     else if (n == "pull_grid") c.opt_pull_grid = value;
-    else if (n == "fill_kernel") c.opt_fill_kernel = value;
     else if (n == "diag_filter") c.opt_diag_filter = value;
     else if (n == "csr_push") c.opt_csr_push = value;
     else if (n == "fused_prep") c.opt_fused_prep = value;
@@ -2502,6 +2500,8 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "perm_push") c.opt_perm_push = value;
     else if (n == "l2_reset") c.opt_l2_reset = value;
     else if (n == "count_kernel") c.opt_count_kernel = value;
+    // retired: the materialise has a single fill kernel now; the names stay accepted so callers that set them keep working
+    else if (n == "fill_kernel" || n == "fill_cap") {}
     else if (n == "bfs_direction") c.opt_bfs_direction = value;
     else if (n == "bfs_sparse_exchange") c.opt_bfs_sparse_exchange = value;
     else if (n == "timing") { c.opt_timing = value; if (c.ready) timed_reset(); }

@@ -17,7 +17,7 @@ WANT = [
     ("hop 2, CSR push", r"k_csr_push<8"),
     ("frontier totals in gather order", r"k_ordered_flops<8>"),
     ("materialise, count (carry-save)", r"k_bits_count_csa<8>"),
-    ("materialise, fill v3", r"k_bits_fill_v3("),
+    ("materialise, fill", r"k_bits_fill<8>"),
     ("bitmap hand-off", r"k_bits_rowmajor"),
     ("BFS top-down expand", r"k_do_expand"),
     ("BFS bottom-up", r"k_do_pull"),
