@@ -13,8 +13,6 @@
 #include "common.cuh"
 #include "ops.cuh"
 #include <cub/block/block_reduce.cuh>
-#include <algorithm>
-#include <cstring>
 
 namespace b200 {
 
@@ -26,8 +24,7 @@ template <int W> struct PullCfg {
     static constexpr int VG = 8 / SPLIT;           // vertices gathered per 8-lane group and unroll step
 };
 static const u64 PUSH_CHUNK = 8192;
-static const u64 LONG_ROW = 4096;   // pull: rows longer than this are split over several CTAs
-static const u64 LONG_CHUNK = 8192;
+static const u64 LONG_ROW = 4096;   // pull: rows longer than this are split into LONG_ROW-entry segments
 
 static void require_natural(const DevBits &X, const char *what);
 
@@ -94,38 +91,7 @@ __device__ __forceinline__ u32 transpose32(u32 x, u32 lane) {
     return x;
 }
 
-// tc[(w*64 + row) * ntiles + tile] = number of vertices of the tile in frontier row 64w+row
-__global__ void __launch_bounds__(TILE_THREADS)
-k_bits_count(const u64 *__restrict__ X, u64 n, u32 W, u64 ntiles, u32 *__restrict__ tc) {
-    __shared__ u32 wc[TILE_THREADS / 32][64];
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    u64 tile = blockIdx.x;
-    u64 v0 = tile * TILE_V + (u64)warp * 64;
-    for (u32 w = 0; w < W; w++) {
-        u32 clo = 0, chi = 0;
-#pragma unroll
-        for (u32 g = 0; g < 2; g++) {
-            u64 v = v0 + g * 32 + lane;
-            u64 word = (v < n) ? X[v * W + w] : 0ULL;
-            if (__ballot_sync(0xffffffffu, word != 0ULL)) {
-                clo += __popc(transpose32((u32)word, lane));
-                chi += __popc(transpose32((u32)(word >> 32), lane));
-            }
-        }
-        wc[warp][lane] = clo;
-        wc[warp][lane + 32] = chi;
-        __syncthreads();
-        if (tid < 64) {
-            u32 s = 0;
-#pragma unroll
-            for (u32 q = 0; q < TILE_THREADS / 32; q++) s += wc[q][tid];
-            tc[((u64)w * 64 + tid) * ntiles + tile] = s;
-        }
-        __syncthreads();
-    }
-}
-
-// Count pass with vertical counters (count_kernel = 1, default).  The counts per (frontier row, tile) are a positional
+// Count pass with vertical counters.  The counts per (frontier row, tile) are a positional
 // popcount: for each of the 64 bit positions of a word column, how many of the tile's 1024 words have that bit set.  No bit
 // transpose per 32 vertices is needed for that: a lane adds the words of 32 vertices (v = lane, lane + 32, ...) into a
 // carry-save adder tree -- 31 CSAs of two LOP3 per 32-bit half leave six bit-planes (weights 1, 2, .., 32) -- and only the
@@ -344,18 +310,15 @@ void bits_to_csr(const DevBits &X, DevCSR &C) {
     DevBuf<u64> off(ncnt + 1);
     {
         TimedScope ts(TK_BITS_COUNT, 8ULL * W * n);
-        if (ctx().opt_count_kernel == 1) {
-            const u64 nwarps = ntiles * pull_split((int)W);
-            const u32 g = (u32)((nwarps + 3) / 4);
-            switch (W) {
-            case 1: LAUNCH((k_bits_count_csa<1>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
-            case 2: LAUNCH((k_bits_count_csa<2>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
-            case 4: LAUNCH((k_bits_count_csa<4>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
-            case 8: LAUNCH((k_bits_count_csa<8>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
-            default: LAUNCH((k_bits_count_csa<16>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
-            }
+        const u64 nwarps = ntiles * pull_split((int)W);
+        const u32 g = (u32)((nwarps + 3) / 4);
+        switch (W) {
+        case 1: LAUNCH((k_bits_count_csa<1>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
+        case 2: LAUNCH((k_bits_count_csa<2>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
+        case 4: LAUNCH((k_bits_count_csa<4>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
+        case 8: LAUNCH((k_bits_count_csa<8>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
+        default: LAUNCH((k_bits_count_csa<16>), g, 128, 0, X.w.ptr, n, ntiles, tc.ptr); break;
         }
-        else LAUNCH(k_bits_count, (u32)ntiles, TILE_THREADS, 0, X.w.ptr, n, W, ntiles, tc.ptr);
     }
     CUDA_TRY(cudaMemsetAsync(tc.ptr + ncnt, 0, sizeof(u32), stream()));
     exclusive_scan_u32_to_u64(tc.ptr, off.ptr, ncnt + 1);
@@ -633,7 +596,7 @@ static void csr_push_impl(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 flop
 }
 // Y = F * A from the CSR form of F.  Returns false (nothing done) when the expansion is large enough that the
 // direction-optimising bit-matrix hop should take it: flops * 4 > nnz(A), the same switch bits_hop applies to edges.
-bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const LongRows *lr) {
+bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt) {
     if (F.ncols != A.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
     const u32 W = bits_words_for(F.nrows);
     u64 flops = 0;
@@ -653,10 +616,10 @@ bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops
     if (flops_out) *flops_out = flops;
     // a square operand with pull tables: write the result in its hot-set order, the form the next pull gathers from directly
     const u32 *perm = nullptr;
-    if (lr && ctx().opt_perm_push && lr->perm_tag && lr->pperm && A.nrows == A.ncols && lr->pperm->n == A.ncols) {
-        perm = lr->pperm->ptr;
-        Y.pvert = lr->pvert;
-        Y.perm_tag = lr->perm_tag;
+    if (pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
+        perm = pt->pperm->ptr;
+        Y.pvert = pt->pvert;
+        Y.perm_tag = pt->perm_tag;
     }
     if (flops == 0) return true;
     switch (W) {
@@ -689,8 +652,17 @@ static void require_natural(const DevBits &X, const char *what) {
 }
 
 // ---------------------------------------------------------------------------- pull
-// 8 lanes per output vertex j: OR of X[k] over k in A'(j,:).  Rows longer than LONG_ROW are
-// zeroed here and finished by k_bits_pull_long (several CTAs per row, RED.OR into Y).
+// Y[j] = OR of X[k] over k in A'(j,:).  What bounds a pull is the L1TEX tag stage: one 128-byte line per clock per SM, and a
+// warp-wide gather with every lane on a different vertex costs 32 of those "wavefronts" per instruction.  A vertex record of
+// W = 8 words is 64 bytes -- one line -- but a lane can fetch at most 16 bytes per instruction on sm_90 (LDG.128), so
+// one-lane-per-vertex spends FOUR wavefronts per vertex.  In k_pull_seg SPLIT = W / 2 adjacent lanes share a vertex: lane h loads
+// words [2h, 2h+2) of the record with one LDG.128, the requests fall into the same line and coalesce into one wavefront, and the
+// lanes never exchange data (each lane ORs, keeps and finally stores its own 16-byte part of the output row).
+// W = 4 -> half the wavefronts per gathered vertex; W = 8 -> a quarter; W = 16 -> an eighth; W <= 2 keeps one lane per record.
+// The rows of A' are binned once per matrix (build_pull_tables):
+//   small (<= SMALL_ROW entries) : k_pull_small, one lane per row in natural order; it also zero-fills the long rows
+//   mid   (<= LONG_ROW)          : k_pull_seg, 8 lanes per row, from a list sorted by length, descending
+//   long                         : the same list, as LONG_ROW-entry segments whose partial results are merged with RED.OR
 struct OrOp64 { __device__ u64 operator()(u64 a, u64 b) const { return a | b; } };
 
 // G[w] = OR over all vertices of word w: the terminal value of the OR monoid for this frontier.  A pull row whose
@@ -717,7 +689,6 @@ __global__ void __launch_bounds__(256) k_or_all(const u64 *__restrict__ X, u64 n
 }
 
 template <bool HINTS> __device__ __forceinline__ u32 ld_col(const u32 *p, u64 strm) { return HINTS ? ld_u32_stream(p, strm) : __ldg(p); }
-template <bool HINTS> __device__ __forceinline__ u64 ld_ptr(const u64 *p, u64 strm) { return HINTS ? ld_u64_stream(p, strm) : __ldg(p); }
 template <bool HINTS> __device__ __forceinline__ u64 ld_x(const u64 *p, u64 keep) { return HINTS ? ld_u64_hint(p, keep) : __ldg(p); }
 // acc |= the W frontier words of one vertex: ONE 16-byte load per word pair (a W=4 vertex is a single 32 B sector), so the
 // number of L1TEX wavefronts per gathered vertex does not grow with W
@@ -732,248 +703,7 @@ template <int W, bool HINTS> __device__ __forceinline__ void or_words(u64 (&acc)
     }
 }
 
-template <int W, bool HINTS, int U, bool EARLY>
-__global__ void __launch_bounds__(256)
-k_bits_pull(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
-            u64 *__restrict__ Y, const u64 *__restrict__ Gp, u32 hot_bytes, u32 tot_bytes) {
-    const u32 lane8 = threadIdx.x & 7;
-    const u32 sub = (threadIdx.x & 31) >> 3;
-    const u32 gmask = 0xFFu << (8 * sub);            // the 8 lanes that share a row
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0, strm = policy_stream();
-    u64 G[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) G[w] = Gp ? Gp[w] : ~0ULL;
-    u64 group = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
-    u64 ngroups = ((u64)gridDim.x * blockDim.x) >> 3;
-    u64 warp_first = group - sub; // group id of this warp's first 8-lane group
-    // software pipeline: row pointers of the NEXT row are in flight while the current row gathers
-    u64 ns = 0, ne = 0;
-    if (warp_first + sub < n) { ns = ld_ptr<HINTS>(ATp + warp_first + sub, strm); ne = ld_ptr<HINTS>(ATp + warp_first + sub + 1, strm); }
-    for (u64 base = warp_first; base < n; base += ngroups) {
-        u64 j = base + sub;
-        u64 s = ns, e = ne;
-        u64 jn = j + ngroups;
-        ns = 0; ne = 0;
-        if (jn < n) { ns = ld_ptr<HINTS>(ATp + jn, strm); ne = ld_ptr<HINTS>(ATp + jn + 1, strm); }
-        if (j >= n) { s = 0; e = 0; }
-        if (e - s > LONG_ROW) e = s;
-        u64 acc[W];
-#pragma unroll
-        for (int w = 0; w < W; w++) acc[w] = 0;
-        if (EARLY) {
-            // group-uniform trip count (all 8 lanes iterate together) so the lanes can vote inside the loop
-            for (u64 qb = s; qb < e; qb += 8 * U) {
-                u32 k[U];
-#pragma unroll
-                for (int u = 0; u < U; u++) { u64 q = qb + lane8 + 8 * u; k[u] = (q < e) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-#pragma unroll
-                for (int u = 0; u < U; u++)
-                    if (k[u] != 0xFFFFFFFFu) {
-                        or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
-                    }
-                if (qb + 8 * U < e) {   // more to come: stop if the row already holds the terminal value
-                    // cheap test every iteration (each lane's own partial saturated), exact cross-lane OR every 4th
-                    bool full = true;
-                    if ((((qb - s) / (8 * U)) & 3) == 3) {
-#pragma unroll
-                        for (int w = 0; w < W; w++) {
-                            u64 a = acc[w];
-                            a |= __shfl_xor_sync(gmask, a, 1);
-                            a |= __shfl_xor_sync(gmask, a, 2);
-                            a |= __shfl_xor_sync(gmask, a, 4);
-                            acc[w] = a;
-                            full = full && (a == G[w]);
-                        }
-                    } else {
-#pragma unroll
-                        for (int w = 0; w < W; w++) full = full && (acc[w] == G[w]);
-                        full = __all_sync(gmask, full);
-                    }
-                    if (full) break;
-                }
-            }
-        } else {
-            for (u64 q = s + lane8; q < e; q += 8 * U) {
-                u32 k[U];
-#pragma unroll
-                for (int u = 0; u < U; u++) k[u] = (q + 8 * u < e) ? ld_col<HINTS>(ATj + q + 8 * u, strm) : 0xFFFFFFFFu;
-#pragma unroll
-                for (int u = 0; u < U; u++)
-                    if (k[u] != 0xFFFFFFFFu) {
-                        or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
-                    }
-            }
-        }
-#pragma unroll
-        for (int w = 0; w < W; w++) {
-            u64 a = acc[w];
-            a |= __shfl_xor_sync(0xffffffffu, a, 1);
-            a |= __shfl_xor_sync(0xffffffffu, a, 2);
-            a |= __shfl_xor_sync(0xffffffffu, a, 4);
-            acc[w] = a;
-        }
-        if (j < n) {
-#pragma unroll
-            for (int w = 0; w < W; w++)
-                if ((w & 7) == (int)lane8) { if (HINTS) st_u64_stream(Y + j * W + w, acc[w], strm); else Y[j * W + w] = acc[w]; }
-        }
-    }
-}
-
-// Software-pipelined 8-lanes-per-row pull (pull_kernel = 3, default).  The dependent chain of one row is
-// rowptr -> col_idx batch -> X gathers; here all three stages of consecutive batches overlap: row pointers are loaded two
-// rows ahead, and the col_idx batch that follows the current one (the next 8*U entries of the same row, or the first
-// batch of the group's next row when this is the last) is in flight while the current batch gathers.
-#ifndef PIPE_MINB
-#define PIPE_MINB 0    // resident CTAs per SM the compiler must leave room for (0 = its own choice); fewer = more landing registers
-#endif
-#if PIPE_MINB > 0
-#define PIPE_BOUNDS __launch_bounds__(256, PIPE_MINB)
-#else
-#define PIPE_BOUNDS __launch_bounds__(256)
-#endif
-template <int W, bool HINTS, int U, bool EARLY>
-__global__ void PIPE_BOUNDS
-k_bits_pull_pipe(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
-                 u64 *__restrict__ Y, const u64 *__restrict__ Gp, u32 hot_bytes, u32 tot_bytes) {
-    const u32 lane8 = threadIdx.x & 7;
-    const u32 sub = (threadIdx.x & 31) >> 3;
-    const u32 gmask = 0xFFu << (8 * sub);
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0, strm = policy_stream();
-    u64 G[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) G[w] = (EARLY && Gp) ? Gp[w] : ~0ULL;
-    const u64 ngroups = ((u64)gridDim.x * blockDim.x) >> 3;
-    u64 j = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
-    const u64 warp_first = j - sub;
-    // rows j (s0,e0), j + ngroups (s1,e1); j + 2*ngroups is loaded inside the loop
-    u64 s0 = 0, e0 = 0, s1 = 0, e1 = 0;
-    if (j < n) { s0 = ld_ptr<HINTS>(ATp + j, strm); e0 = ld_ptr<HINTS>(ATp + j + 1, strm); }
-    if (j + ngroups < n) { s1 = ld_ptr<HINTS>(ATp + j + ngroups, strm); e1 = ld_ptr<HINTS>(ATp + j + ngroups + 1, strm); }
-    if (e0 - s0 > LONG_ROW) e0 = s0;
-    u32 k[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) { u64 q = s0 + lane8 + 8 * u; k[u] = (q < e0) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-    for (u64 base = warp_first; base < n; base += ngroups, j += ngroups) {
-        u64 s2 = 0, e2 = 0;
-        if (j + 2 * ngroups < n) { s2 = ld_ptr<HINTS>(ATp + j + 2 * ngroups, strm); e2 = ld_ptr<HINTS>(ATp + j + 2 * ngroups + 1, strm); }
-        if (e1 - s1 > LONG_ROW) e1 = s1;
-        u64 acc[W];
-#pragma unroll
-        for (int w = 0; w < W; w++) acc[w] = 0;
-        u64 qb = s0;
-        u32 it = 0;
-        while (true) {
-            const bool more = qb + 8 * U < e0;
-            // col_idx of the following batch: same row if it continues, else the first batch of the next row
-            const u64 nb = more ? qb + 8 * U : s1, ne = more ? e0 : e1;
-            u32 kn[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) { u64 q = nb + lane8 + 8 * u; kn[u] = (q < ne) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-#pragma unroll
-            for (int u = 0; u < U; u++)
-                if (k[u] != 0xFFFFFFFFu) or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
-#pragma unroll
-            for (int u = 0; u < U; u++) k[u] = kn[u];
-            if (!more) break;
-            if (EARLY) {
-                // cheap test every iteration (each lane holds a saturated partial), exact cross-lane OR every 4th
-                bool full = true;
-                if ((it & 3) == 3) {
-#pragma unroll
-                    for (int w = 0; w < W; w++) {
-                        u64 a = acc[w];
-                        a |= __shfl_xor_sync(gmask, a, 1);
-                        a |= __shfl_xor_sync(gmask, a, 2);
-                        a |= __shfl_xor_sync(gmask, a, 4);
-                        acc[w] = a;
-                        full = full && (a == G[w]);
-                    }
-                } else {
-#pragma unroll
-                    for (int w = 0; w < W; w++) full = full && (acc[w] == G[w]);
-                    full = __all_sync(gmask, full);
-                }
-                if (full) {   // row saturated: the prefetched batch belongs to this row, fetch the next row's instead
-#pragma unroll
-                    for (int u = 0; u < U; u++) { u64 q = s1 + lane8 + 8 * u; k[u] = (q < e1) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-                    break;
-                }
-            }
-            qb += 8 * U;
-            it++;
-        }
-#pragma unroll
-        for (int w = 0; w < W; w++) {
-            u64 a = acc[w];
-            a |= __shfl_xor_sync(gmask, a, 1);
-            a |= __shfl_xor_sync(gmask, a, 2);
-            a |= __shfl_xor_sync(gmask, a, 4);
-            acc[w] = a;
-        }
-        if (j < n) {
-#pragma unroll
-            for (int w = 0; w < W; w++)
-                if ((w & 7) == (int)lane8) { if (HINTS) st_u64_stream(Y + j * W + w, acc[w], strm); else Y[j * W + w] = acc[w]; }
-        }
-        s0 = s1; e0 = e1; s1 = s2; e1 = e2;
-    }
-}
-
-// ---------------------------------------------------------------------------- degree-binned pull (pull_kernel = 4)
-// The in-degree distribution of a power-law graph is what starves the 8-lane kernels: 86 % of the rows of A' hold <= 8
-// entries (56 % none) and ride in the same warp as rows hundreds of entries long, so most 8-lane groups idle while one
-// gathers -- and the rate of this kernel is set by the number of gathers in flight.  Rows are therefore binned once per matrix:
-//   small (<= SMALL_ROW) : one lane per row in natural order (k_bits_pull_small; also zero-fills empty and long rows)
-//   mid   (<= LONG_ROW)  : a list sorted by length, descending; the four 8-lane groups of a warp take ADJACENT list entries,
-//                          i.e. rows of (nearly) the same length, so they finish their batches together (k_bits_pull_mid)
-//   long                 : k_bits_pull_long, as before
 static const u32 SMALL_ROW = 8;
-
-__global__ void k_flag_mid(const u64 *__restrict__ p, u64 n, u32 *__restrict__ flag) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r < n; r += stride) {
-        u64 d = p[r + 1] - p[r];
-        flag[r] = (d > SMALL_ROW && d <= LONG_ROW) ? 1u : 0u;
-    }
-}
-// key = (LONG_ROW - len) << 32 | row : ascending sort = length descending, row ascending inside one length
-__global__ void k_mid_keys(const u32 *__restrict__ flag, const u64 *__restrict__ pos, u64 n, const u64 *__restrict__ p,
-                           u64 *__restrict__ keys) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r < n; r += stride)
-        if (flag[r]) keys[pos[r]] = ((LONG_ROW - (p[r + 1] - p[r])) << 32) | r;
-}
-__global__ void k_mid_unpack(const u64 *__restrict__ keys, u64 nm, const u64 *__restrict__ p, u32 *__restrict__ m_row,
-                             u32 *__restrict__ m_len, u64 *__restrict__ m_start) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nm) return;
-    u32 r = (u32)keys[i];
-    m_row[i] = r;
-    m_start[i] = p[r];
-    m_len[i] = (u32)(p[r + 1] - p[r]);
-}
-static void build_mid_list(const DevCSR &AT, LongRows &lr) {
-    u64 n = AT.nrows;
-    lr.nm = 0;
-    lr.m_row.release(); lr.m_len.release(); lr.m_start.release();
-    if (!n) return;
-    DevBuf<u32> flag(n + 1);
-    DevBuf<u64> pos(n + 1);
-    LAUNCH(k_flag_mid, grid_for(n, 256, 1 << 16), 256, 0, AT.p.ptr, n, flag.ptr);
-    CUDA_TRY(cudaMemsetAsync(flag.ptr + n, 0, sizeof(u32), stream()));
-    exclusive_scan_u32_to_u64(flag.ptr, pos.ptr, n + 1);
-    u64 nm = read_scalar(pos.ptr + n);
-    lr.nm = nm;
-    if (!nm) return;
-    DevBuf<u64> keys(nm);
-    LAUNCH(k_mid_keys, grid_for(n, 256, 1 << 16), 256, 0, flag.ptr, pos.ptr, n, AT.p.ptr, keys.ptr);
-    sort_keys_u64(keys.ptr, nm, 46);            // LONG_ROW = 2^12: 32 row bits + 13 length bits, rounded up
-    lr.m_row.alloc(nm); lr.m_len.alloc(nm); lr.m_start.alloc(nm);
-    LAUNCH(k_mid_unpack, grid_for(nm, 256), 256, 0, keys.ptr, nm, AT.p.ptr, lr.m_row.ptr, lr.m_len.ptr, lr.m_start.ptr);
-}
 
 template <int W> __device__ __forceinline__ void store_row(u64 *dst, const u64 (&acc)[W]) {
     if constexpr (W == 1) { dst[0] = acc[0]; }
@@ -982,13 +712,83 @@ template <int W> __device__ __forceinline__ void store_row(u64 *dst, const u64 (
         for (int w2 = 0; w2 < W / 2; w2++) reinterpret_cast<ulonglong2 *>(dst)[w2] = make_ulonglong2(acc[2 * w2], acc[2 * w2 + 1]);
     }
 }
+template <int WL> __device__ __forceinline__ void store_part(u64 *dst, const u64 (&acc)[WL]) { store_row<WL>(dst, acc); }
 
-// one lane per row, natural order: rows of <= SMALL_ROW entries are finished here, long rows are zero-filled (k_bits_pull_long
-// ORs into them), mid rows are left to k_bits_pull_mid
+static const u32 SEG_ATOMIC = 0x80000000u;
+
+// segments per row: 0 (small), 1 (mid), ceil(len / LONG_ROW) (long); maxlen = the longest row when it is longer than LONG_ROW
+__global__ void k_seg_count(const u64 *__restrict__ p, u64 n, u32 *__restrict__ cnt, u64 *__restrict__ maxlen) {
+    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 stride = (u64)gridDim.x * blockDim.x;
+    u64 mx = 0;
+    for (; r <= n; r += stride) {
+        if (r == n) { cnt[r] = 0; break; }
+        u64 d = p[r + 1] - p[r];
+        cnt[r] = d <= SMALL_ROW ? 0u : (u32)((d + LONG_ROW - 1) / LONG_ROW);
+        if (d > mx) mx = d;
+    }
+    if (mx > LONG_ROW) atomicMax((unsigned long long *)maxlen, mx);
+}
+// key = LONG_ROW - seglen (ascending sort = longest first), value = position of the segment: row << 20 | index inside the row
+__global__ void k_seg_emit(const u64 *__restrict__ p, u64 n, const u64 *__restrict__ pos, u64 *__restrict__ keys, u64 *__restrict__ vals) {
+    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 stride = (u64)gridDim.x * blockDim.x;
+    for (; r < n; r += stride) {
+        const u64 d = p[r + 1] - p[r];
+        if (d <= SMALL_ROW) continue;
+        u64 o = pos[r];
+        for (u64 s = 0, i = 0; s < d; s += LONG_ROW, i++) {
+            const u64 len = d - s < LONG_ROW ? d - s : LONG_ROW;
+            keys[o] = LONG_ROW - len;
+            vals[o] = (r << 20) | i;
+            o++;
+        }
+    }
+}
+__global__ void k_seg_unpack(const u64 *__restrict__ vals, u64 ns, const u64 *__restrict__ p, u32 *__restrict__ s_row,
+                             u32 *__restrict__ s_len, u64 *__restrict__ s_start) {
+    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ns) return;
+    const u64 v = vals[i];
+    const u32 r = (u32)(v >> 20);
+    const u64 k = v & 0xFFFFFu;
+    const u64 d = p[r + 1] - p[r];
+    const u64 s = k * LONG_ROW;
+    const u64 len = d - s < LONG_ROW ? d - s : LONG_ROW;
+    s_row[i] = r;
+    s_start[i] = p[r] + s;
+    s_len[i] = (u32)len | (d > LONG_ROW ? SEG_ATOMIC : 0u);
+}
+static void build_seg_list(const DevCSR &AT, PullTables &pt) {
+    const u64 n = AT.nrows;
+    pt.ns = 0;
+    pt.s_row.release(); pt.s_len.release(); pt.s_start.release();
+    if (!n) return;
+    DevBuf<u32> cnt(n + 1);
+    DevBuf<u64> pos(n + 1), mx(1);
+    mx.zero();
+    LAUNCH(k_seg_count, grid_for(n + 1, 256, 1 << 16), 256, 0, AT.p.ptr, n, cnt.ptr, mx.ptr);
+    // k_seg_emit addresses a segment as row << 20 | index inside the row
+    if (read_scalar(mx.ptr) >= ((u64)LONG_ROW << 20)) throw GrbError(-8, "pull: a row of A' exceeds 2^32 entries");
+    exclusive_scan_u32_to_u64(cnt.ptr, pos.ptr, n + 1);
+    const u64 ns = read_scalar(pos.ptr + n);
+    pt.ns = ns;
+    if (!ns) return;
+    DevBuf<u64> keys(ns), vals(ns);
+    LAUNCH(k_seg_emit, grid_for(n, 256, 1 << 16), 256, 0, AT.p.ptr, n, pos.ptr, keys.ptr, vals.ptr);
+    sort_pairs_u64(keys.ptr, vals.ptr, ns, 13);          // stable: rows ascending inside one length
+    pt.s_row.alloc(ns); pt.s_len.alloc(ns); pt.s_start.alloc(ns);
+    LAUNCH(k_seg_unpack, grid_for(ns, 256), 256, 0, vals.ptr, ns, AT.p.ptr, pt.s_row.ptr, pt.s_len.ptr, pt.s_start.ptr);
+}
+
+// one lane per row, natural order: rows of <= SMALL_ROW entries are finished here, rows longer than LONG_ROW are zero-filled
+// (their segments arrive through RED.OR), everything in between is left to k_pull_seg.  This kernel is latency-bound, not
+// L1TEX-bound: splitting the record across lanes as k_pull_seg does would divide the bytes each warp keeps in flight, so one lane
+// owns the whole record here.
 template <int W, bool HINTS>
 __global__ void __launch_bounds__(256)
-k_bits_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
-                  u64 *__restrict__ Y, u32 hot_bytes, u32 tot_bytes) {
+k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
+             u64 *__restrict__ Y, u32 hot_bytes, u32 tot_bytes) {
     const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0;
     u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const u64 stride = (u64)gridDim.x * blockDim.x;
@@ -1027,286 +827,12 @@ k_bits_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 
     }
 }
 
-// 8 lanes per mid row, rows taken from the length-sorted list; same three-stage software pipeline as k_bits_pull_pipe
-// (list entry two steps ahead, col_idx batch one step ahead, gathers now).  Step t of group g handles list entry
-// t * ngroups + g on even steps and t * ngroups + (ngroups - 1 - g) on odd ones, which evens out the totals per group.
-template <int W, bool HINTS, int U, bool EARLY>
-__global__ void PIPE_BOUNDS
-k_bits_pull_mid(const u32 *__restrict__ m_row, const u64 *__restrict__ m_start, const u32 *__restrict__ m_len, u64 nm,
-                const u32 *__restrict__ ATj, const u64 *__restrict__ X, u64 *__restrict__ Y, const u64 *__restrict__ Gp,
-                u32 hot_bytes, u32 tot_bytes) {
-    const u32 lane8 = threadIdx.x & 7;
-    const u32 sub = (threadIdx.x & 31) >> 3;
-    const u32 gmask = 0xFFu << (8 * sub);
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0, strm = policy_stream();
-    u64 G[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) G[w] = (EARLY && Gp) ? Gp[w] : ~0ULL;
-    const u64 ngroups = ((u64)gridDim.x * blockDim.x) >> 3;
-    const u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
-    const u64 steps = (nm + ngroups - 1) / ngroups;
-    auto entry = [&](u64 t) -> u64 { return t * ngroups + ((t & 1) ? ngroups - 1 - g : g); };
-    auto fetch = [&](u64 t, u64 &s, u64 &e) {
-        s = 0; e = 0;
-        if (t < steps) { u64 i = entry(t); if (i < nm) { s = m_start[i]; e = s + m_len[i]; } }
-    };
-    u64 s0, e0, s1, e1;
-    fetch(0, s0, e0);
-    fetch(1, s1, e1);
-    u32 k[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) { u64 q = s0 + lane8 + 8 * u; k[u] = (q < e0) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-    for (u64 t = 0; t < steps; t++) {
-        u64 s2, e2;
-        fetch(t + 2, s2, e2);
-        u64 acc[W];
-#pragma unroll
-        for (int w = 0; w < W; w++) acc[w] = 0;
-        u64 qb = s0;
-        u32 it = 0;
-        while (true) {
-            const bool more = qb + 8 * U < e0;
-            const u64 nb = more ? qb + 8 * U : s1, ne = more ? e0 : e1;
-            u32 kn[U];
-#pragma unroll
-            for (int u = 0; u < U; u++) { u64 q = nb + lane8 + 8 * u; kn[u] = (q < ne) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-#pragma unroll
-            for (int u = 0; u < U; u++)
-                if (k[u] != 0xFFFFFFFFu) or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
-#pragma unroll
-            for (int u = 0; u < U; u++) k[u] = kn[u];
-            if (!more) break;
-            if (EARLY) {
-                bool full = true;
-                if ((it & 3) == 3) {
-#pragma unroll
-                    for (int w = 0; w < W; w++) {
-                        u64 a = acc[w];
-                        a |= __shfl_xor_sync(gmask, a, 1);
-                        a |= __shfl_xor_sync(gmask, a, 2);
-                        a |= __shfl_xor_sync(gmask, a, 4);
-                        acc[w] = a;
-                        full = full && (a == G[w]);
-                    }
-                } else {
-#pragma unroll
-                    for (int w = 0; w < W; w++) full = full && (acc[w] == G[w]);
-                    full = __all_sync(gmask, full);
-                }
-                if (full) {
-#pragma unroll
-                    for (int u = 0; u < U; u++) { u64 q = s1 + lane8 + 8 * u; k[u] = (q < e1) ? ld_col<HINTS>(ATj + q, strm) : 0xFFFFFFFFu; }
-                    break;
-                }
-            }
-            qb += 8 * U;
-            it++;
-        }
-#pragma unroll
-        for (int w = 0; w < W; w++) {
-            u64 a = acc[w];
-            a |= __shfl_xor_sync(gmask, a, 1);
-            a |= __shfl_xor_sync(gmask, a, 2);
-            a |= __shfl_xor_sync(gmask, a, 4);
-            acc[w] = a;
-        }
-        if (e0 > s0 && lane8 == 0) {
-            const u64 i = entry(t);
-            store_row<W>(Y + (u64)m_row[i] * W, acc);
-        }
-        s0 = s1; e0 = e1; s1 = s2; e1 = e2;
-    }
-}
-
-template <int W>
-__global__ void __launch_bounds__(256)
-k_bits_pull_long(const u32 *__restrict__ lrows, const u64 *__restrict__ choff, u32 nlong, const u64 *__restrict__ ATp,
-                 const u32 *__restrict__ ATj, const u64 *__restrict__ X, u64 *__restrict__ Y, const u64 *__restrict__ Gp) {
-    typedef cub::BlockReduce<u64, 256> Red;
-    __shared__ typename Red::TempStorage ts;
-    __shared__ u32 s_li;
-    if (threadIdx.x == 0) {   // chunk -> (long row, chunk within the row): binary search in the per-row chunk prefix
-        u64 c = blockIdx.x, lo = 0, hi = nlong - 1;
-        while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (choff[mid] <= c) lo = mid; else hi = mid - 1; }
-        s_li = (u32)lo;
-    }
-    __syncthreads();
-    const u32 li = s_li;
-    u32 j = lrows[li];
-    u64 s = ATp[j], e = ATp[j + 1];
-    u64 c0 = s + ((u64)blockIdx.x - choff[li]) * LONG_CHUNK;
-    if (c0 >= e) return;
-    u64 c1 = c0 + LONG_CHUNK;
-    if (c1 > e) c1 = e;
-    u64 acc[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) acc[w] = 0;
-    u64 G[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) G[w] = Gp ? Gp[w] : ~0ULL;
-    // warp-uniform loop; leaves as soon as the warp holds the terminal value: cheap test every iteration (each lane holds a
-    // saturated partial), exact cross-lane OR every 4th
-    u32 it = 0;
-    for (u64 qb = c0 + (threadIdx.x & ~31u); qb < c1; qb += 256, it++) {
-        u64 q = qb + (threadIdx.x & 31);
-        if (q < c1) {
-            u32 k = __ldg(ATj + q);
-            or_words<W, false>(acc, X + (u64)k * W, 0);
-        }
-        bool full = true;
-        if ((it & 3) == 3) {
-#pragma unroll
-            for (int w = 0; w < W; w++) {
-                u64 a = acc[w];
-#pragma unroll
-                for (int d = 16; d; d >>= 1) a |= __shfl_xor_sync(0xffffffffu, a, d);
-                acc[w] = a;
-                full = full && (a == G[w]);
-            }
-        } else {
-#pragma unroll
-            for (int w = 0; w < W; w++) full = full && (acc[w] == G[w]);
-            full = __all_sync(0xffffffffu, full);
-        }
-        if (full) break;
-    }
-#pragma unroll
-    for (int w = 0; w < W; w++) {
-        u64 r = Red(ts).Reduce(acc[w], OrOp64());
-        __syncthreads();
-        if (threadIdx.x == 0 && r) atomicOr((unsigned long long *)&Y[(u64)j * W + w], r);
-    }
-}
-
-// ---------------------------------------------------------------------------- lane-split pull (pull_kernel = 5, default)
-// What bounds a pull is the L1TEX tag stage: one 128-byte line per clock per SM, and a warp-wide
-// gather with every lane on a different vertex costs 32 of those "wavefronts" per instruction.  A vertex record of W = 8 words
-// is 64 bytes -- one line -- but a lane can fetch at most 16 bytes per instruction on sm_90 (LDG.128), so one-lane-per-vertex
-// spends FOUR wavefronts per vertex.  Here SPLIT = W / 2 adjacent lanes share a vertex: lane h loads words [2h, 2h+2) of the
-// record with one LDG.128, the requests fall into the same line and coalesce into one wavefront, and the lanes never exchange
-// data (each lane ORs, keeps and finally stores its own 16-byte part of the output row).
-// W = 4 -> half the wavefronts per gathered vertex; W = 8 -> a quarter; W = 16 -> an eighth; W <= 2 is unchanged.
-// Rows longer than LONG_ROW are no longer a separate kernel: they enter the length-sorted list as LONG_ROW-entry segments whose
-// partial results are merged with RED.OR (the small-row kernel zero-fills those rows first).
-template <int WL> __device__ __forceinline__ void store_part(u64 *dst, const u64 (&acc)[WL]) { store_row<WL>(dst, acc); }
-
-static const u32 SEG_ATOMIC = 0x80000000u;
-
-// segments per row: 0 (small), 1 (mid), ceil(len / LONG_ROW) (long)
-__global__ void k_seg_count(const u64 *__restrict__ p, u64 n, u32 *__restrict__ cnt) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r <= n; r += stride) {
-        if (r == n) { cnt[r] = 0; break; }
-        u64 d = p[r + 1] - p[r];
-        cnt[r] = d <= SMALL_ROW ? 0u : (u32)((d + LONG_ROW - 1) / LONG_ROW);
-    }
-}
-// key = LONG_ROW - seglen (ascending sort = longest first), value = position of the segment: row << 20 | index inside the row
-__global__ void k_seg_emit(const u64 *__restrict__ p, u64 n, const u64 *__restrict__ pos, u64 *__restrict__ keys, u64 *__restrict__ vals) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r < n; r += stride) {
-        const u64 d = p[r + 1] - p[r];
-        if (d <= SMALL_ROW) continue;
-        u64 o = pos[r];
-        for (u64 s = 0, i = 0; s < d; s += LONG_ROW, i++) {
-            const u64 len = d - s < LONG_ROW ? d - s : LONG_ROW;
-            keys[o] = LONG_ROW - len;
-            vals[o] = (r << 20) | i;
-            o++;
-        }
-    }
-}
-__global__ void k_seg_unpack(const u64 *__restrict__ vals, u64 ns, const u64 *__restrict__ p, u32 *__restrict__ s_row,
-                             u32 *__restrict__ s_len, u64 *__restrict__ s_start) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= ns) return;
-    const u64 v = vals[i];
-    const u32 r = (u32)(v >> 20);
-    const u64 k = v & 0xFFFFFu;
-    const u64 d = p[r + 1] - p[r];
-    const u64 s = k * LONG_ROW;
-    const u64 len = d - s < LONG_ROW ? d - s : LONG_ROW;
-    s_row[i] = r;
-    s_start[i] = p[r] + s;
-    s_len[i] = (u32)len | (d > LONG_ROW ? SEG_ATOMIC : 0u);
-}
-static void build_seg_list(const DevCSR &AT, LongRows &lr) {
-    const u64 n = AT.nrows;
-    lr.ns = 0;
-    lr.s_row.release(); lr.s_len.release(); lr.s_start.release();
-    lr.seg_built = true;
-    if (!n) return;
-    if (lr.maxdeg >= ((u64)LONG_ROW << 20)) throw GrbError(-8, "pull: a row of A' exceeds 2^32 entries");
-    DevBuf<u32> cnt(n + 1);
-    DevBuf<u64> pos(n + 1);
-    LAUNCH(k_seg_count, grid_for(n + 1, 256, 1 << 16), 256, 0, AT.p.ptr, n, cnt.ptr);
-    exclusive_scan_u32_to_u64(cnt.ptr, pos.ptr, n + 1);
-    const u64 ns = read_scalar(pos.ptr + n);
-    lr.ns = ns;
-    if (!ns) return;
-    DevBuf<u64> keys(ns), vals(ns);
-    LAUNCH(k_seg_emit, grid_for(n, 256, 1 << 16), 256, 0, AT.p.ptr, n, pos.ptr, keys.ptr, vals.ptr);
-    sort_pairs_u64(keys.ptr, vals.ptr, ns, 13);          // stable: rows ascending inside one length
-    lr.s_row.alloc(ns); lr.s_len.alloc(ns); lr.s_start.alloc(ns);
-    LAUNCH(k_seg_unpack, grid_for(ns, 256), 256, 0, vals.ptr, ns, AT.p.ptr, lr.s_row.ptr, lr.s_len.ptr, lr.s_start.ptr);
-}
-
-// SPLIT lanes per row, natural order: rows of <= SMALL_ROW entries are finished here, rows longer than LONG_ROW are zero-filled
-// (their segments arrive through RED.OR), everything in between is left to k_pull_seg.  This kernel is latency-bound, not
-// L1TEX-bound: splitting the record across lanes divides the bytes each warp keeps in flight, so by default one lane owns the
-// whole record here (small_split = 0).
-template <int W, bool HINTS, int SPLIT>
-__global__ void __launch_bounds__(256)
-k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
-             u64 *__restrict__ Y, u32 hot_bytes, u32 tot_bytes) {
-    constexpr int WL = W / SPLIT;                  // words per lane: SPLIT = PullCfg<W>::SPLIT (one 16-byte load per record part) or 1
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0;
-    const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    const u32 h = (u32)(t % SPLIT);
-    const u64 *Xh = X + h * WL;
-    u64 j = t / SPLIT;
-    const u64 stride = ((u64)gridDim.x * blockDim.x) / SPLIT;
-    u64 s = 0, e = 0, s1 = 0, e1 = 0;
-    if (j < n) { s = __ldg(ATp + j); e = __ldg(ATp + j + 1); }
-    if (j + stride < n) { s1 = __ldg(ATp + j + stride); e1 = __ldg(ATp + j + stride + 1); }
-    u32 k[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) k[u] = (e - s <= SMALL_ROW && s + u < e) ? __ldg(ATj + s + u) : 0xFFFFFFFFu;
-    for (; j < n; j += stride) {
-        u64 s2 = 0, e2 = 0;
-        if (j + 2 * stride < n) { s2 = __ldg(ATp + j + 2 * stride); e2 = __ldg(ATp + j + 2 * stride + 1); }
-        u32 kn[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) kn[u] = (e1 - s1 <= SMALL_ROW && s1 + u < e1) ? __ldg(ATj + s1 + u) : 0xFFFFFFFFu;
-        u64 acc[WL];
-#pragma unroll
-        for (int w = 0; w < WL; w++) acc[w] = 0;
-        if (e - s <= SMALL_ROW) {
-#pragma unroll
-            for (int u = 0; u < 4; u++)
-                if (k[u] != 0xFFFFFFFFu) or_words<WL, HINTS>(acc, Xh + (u64)k[u] * W, keep);
-            if (e - s > 4) {
-#pragma unroll
-                for (int u = 0; u < 4; u++) k[u] = (s + 4 + u < e) ? __ldg(ATj + s + 4 + u) : 0xFFFFFFFFu;
-#pragma unroll
-                for (int u = 0; u < 4; u++)
-                    if (k[u] != 0xFFFFFFFFu) or_words<WL, HINTS>(acc, Xh + (u64)k[u] * W, keep);
-            }
-        }
-        if (e - s <= SMALL_ROW || e - s > LONG_ROW) store_part<WL>(Y + j * W + h * WL, acc);
-#pragma unroll
-        for (int u = 0; u < 4; u++) k[u] = kn[u];
-        s = s1; e = e1; s1 = s2; e1 = e2;
-    }
-}
-
 // 8 lanes per list entry (a mid row, or one LONG_ROW-entry segment of a long row); entries sorted by length, descending.
-// Same three-stage software pipeline as k_bits_pull_mid (list entry two steps ahead, col_idx batch one step ahead, gathers now);
-// the 8 lanes cover VG vertices x SPLIT record parts per unroll step.
+// Three-stage software pipeline: list entry two steps ahead, col_idx batch one step ahead, gathers now.  Step t of group g
+// handles list entry t * ngroups + g on even steps and t * ngroups + (ngroups - 1 - g) on odd ones, which evens out the totals per
+// group.  The 8 lanes cover VG vertices x SPLIT record parts per unroll step.
 template <int W, bool HINTS, int U, bool EARLY>
-__global__ void PIPE_BOUNDS
+__global__ void __launch_bounds__(256)
 k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const u32 *__restrict__ s_len, u64 ns,
            const u32 *__restrict__ ATj, const u64 *__restrict__ X, u64 *__restrict__ Y, const u64 *__restrict__ Gp,
            u32 hot_bytes, u32 tot_bytes) {
@@ -1396,144 +922,6 @@ k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const
         }
         s0 = s1; e0 = e1; s1 = s2; e1 = e2;
     }
-}
-
-// ---------------------------------------------------------------------------- pull, merge-path variant
-// Balanced over (rows + nnz) of A' exactly like merge-based CSR SpMV: every CTA takes TILE consecutive items of the
-// merged (row-end, nnz) sequence, so hub rows and runs of empty rows cost what they weigh.  Phase 1 gathers X[col]
-// for the tile's nnz with a flat coalesced mapping (IPT independent gather chains per thread: memory-level
-// parallelism), phase 2 is each thread's serial walk over its IPT merged items out of shared memory, phase 3 writes
-// finished rows with plain stores (tile-boundary rows with RED.OR; Y is pre-zeroed).
-template <int W> struct MpCfg { static const int TILE = (W <= 2) ? 2048 : (W == 4 ? 1024 : (W == 8 ? 512 : 256)); };
-
-template <int W>
-__global__ void __launch_bounds__(256)
-k_bits_pull_mp(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, u64 nnz, const u64 *__restrict__ X,
-               u64 *__restrict__ Y, const u64 *__restrict__ mp_r /* row coordinate of every 256th diagonal */) {
-    constexpr int T = 256, TILE = MpCfg<W>::TILE, IPT = TILE / T;
-    extern __shared__ u64 smem_mp[];
-    u64 *sx = smem_mp;                         // [TILE * W]   gathered words, nnz order
-    u64 *rowacc = sx + (size_t)TILE * W;       // [(TILE + 1) * W]
-    u32 *rend = (u32 *)(rowacc + (size_t)(TILE + 1) * W); // [TILE + 2] row ends relative to the tile's first nnz
-    const u32 tid = threadIdx.x;
-    const u64 keep = policy_keep(), strm = policy_stream();
-    const u64 total = n + nnz;
-    u64 d0 = (u64)blockIdx.x * TILE, d1 = d0 + TILE;
-    if (d1 > total) d1 = total;
-    // tile coordinates come from the per-matrix table built once by k_mp_coords (static for an immutable base)
-    const u64 r0 = mp_r[d0 / 256], r1 = (d1 == total) ? n : mp_r[d1 / 256];
-    const u64 z0 = d0 - r0, z1 = d1 - r1;
-    const u32 nr = (u32)(r1 - r0);   // row-ends consumed in this tile; row r1 may be entered but not finished
-    const u32 nz = (u32)(z1 - z0);
-    for (u32 i = tid; i <= nr; i += T) {
-        u64 r = r0 + i;
-        u64 e = (r < n) ? ld_u64_stream(ATp + r + 1, strm) : nnz;
-        u64 rel = e - z0;
-        rend[i] = rel > 0xffffffffULL ? 0xffffffffu : (u32)rel;  // rows ending past the tile clamp high
-#pragma unroll
-        for (int w = 0; w < W; w++) rowacc[(size_t)i * W + w] = 0;
-    }
-#pragma unroll
-    for (int k = 0; k < IPT; k++) {
-        u32 e = tid + k * T;
-        if (e < nz) {
-            u32 col = ld_u32_stream(ATj + z0 + e, strm);
-#pragma unroll
-            for (int w = 0; w < W; w++) sx[(size_t)e * W + w] = ld_u64_hint(X + (u64)col * W + w, keep);
-        }
-    }
-    __syncthreads();
-    // per-thread merge-path start inside the tile
-    u32 dt = tid * IPT;
-    u32 items = (u32)(d1 - d0);
-    if (dt > items) dt = items;
-    u32 lo = dt > nz ? dt - nz : 0, hi = dt < nr ? dt : nr;
-    while (lo < hi) {
-        u32 mid = (lo + hi) >> 1;
-        if (rend[mid] <= dt - mid - 1) lo = mid + 1; else hi = mid;
-    }
-    u32 r = lo, z = dt - lo;
-    u32 dend = dt + IPT;
-    if (dend > items) dend = items;
-    u64 acc[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) acc[w] = 0;
-    auto flush = [&](u32 row) {
-#pragma unroll
-        for (int w = 0; w < W; w++) {
-            u64 a = acc[w];
-            if (a) {
-                u32 *p32 = (u32 *)&rowacc[(size_t)row * W + w];
-                if ((u32)a) atomicOr(p32, (u32)a);
-                if ((u32)(a >> 32)) atomicOr(p32 + 1, (u32)(a >> 32));
-            }
-            acc[w] = 0;
-        }
-    };
-    for (u32 d = dt; d < dend; d++) {
-        if (r < nr ? (z < rend[r]) : true) {          // consume one nnz of row r (r == nr: the unfinished last row)
-#pragma unroll
-            for (int w = 0; w < W; w++) acc[w] |= sx[(size_t)z * W + w];
-            z++;
-        } else {
-            flush(r);
-            r++;
-        }
-    }
-    flush(r);
-    __syncthreads();
-    for (u32 i = tid; i <= nr; i += T) {
-        u64 row = r0 + i;
-        if (row >= n) continue;
-#pragma unroll
-        for (int w = 0; w < W; w++) {
-            u64 v = rowacc[(size_t)i * W + w];
-            if (v) {
-                if (i == 0 || i == nr) atomicOr((unsigned long long *)&Y[row * W + w], v);
-                else st_u64_stream(Y + row * W + w, v, strm);
-            }
-        }
-    }
-}
-
-// merge-path coordinates of every 256th diagonal of (row-ends, nnz): r = #rows finished before the diagonal
-__global__ void k_mp_coords(const u64 *__restrict__ ATp, u64 n, u64 nnz, u64 ndiag, u64 *__restrict__ mp_r) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ndiag) return;
-    u64 d = t * 256;
-    u64 total = n + nnz;
-    if (d > total) d = total;
-    u64 lo = d > nnz ? d - nnz : 0, hi = d < n ? d : n;
-    while (lo < hi) {
-        u64 mid = (lo + hi) >> 1;
-        if (ATp[mid + 1] <= d - mid - 1) lo = mid + 1; else hi = mid;
-    }
-    mp_r[t] = lo;
-}
-
-__global__ void k_flag_long(const u64 *__restrict__ p, u64 n, u32 *__restrict__ flag, u64 *__restrict__ maxdeg) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    u64 mx = 0;
-    for (; r < n; r += stride) {
-        u64 d = p[r + 1] - p[r];
-        flag[r] = d > LONG_ROW ? 1u : 0u;
-        if (d > mx) mx = d;
-    }
-    if (mx > LONG_ROW) atomicMax((unsigned long long *)maxdeg, mx);
-}
-__global__ void k_long_chunks(const u32 *__restrict__ lrows, u64 nl, const u64 *__restrict__ p, u64 *__restrict__ nch) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t > nl) return;
-    if (t == nl) { nch[t] = 0; return; }
-    u32 r = lrows[t];
-    nch[t] = (p[r + 1] - p[r] + LONG_CHUNK - 1) / LONG_CHUNK;
-}
-__global__ void k_scatter_flagged(const u32 *__restrict__ flag, const u64 *__restrict__ pos, u64 n, u32 *__restrict__ out) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r < n; r += stride)
-        if (flag[r]) out[pos[r]] = (u32)r;
 }
 
 // ---- hot-set packing of the gather index space ------------------------------------------------------------------
@@ -1666,247 +1054,75 @@ k_ordered_flops(const u32 *__restrict__ hdeg, u64 n1, const u64 *__restrict__ Xp
     if (threadIdx.x < W && sG[threadIdx.x]) atomicOr((unsigned long long *)&G[threadIdx.x], sG[threadIdx.x]);
 }
 
-void build_hot_pack(const DevCSR &A, const DevCSR &AT, LongRows &lr) {
+static void build_hot_pack(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     u64 n = A.nrows;
-    lr.vert.release(); lr.jp.release(); lr.slot.release(); lr.hdeg.release(); lr.n1 = 0; lr.packed = false;
+    pt.vert.release(); pt.jp.release(); pt.slot.release(); pt.hdeg.release(); pt.n1 = 0; pt.packed = false;
     if (n == 0 || AT.nnz == 0 || n >= 0xFFFFFFFFULL) return;
     DevBuf<u64> keys(n), cnt(1);
     cnt.zero();
     LAUNCH(k_degree_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, A.p.ptr, n, keys.ptr, cnt.ptr);
     sort_keys_u64(keys.ptr, n, 64);
     u64 n1 = read_scalar(cnt.ptr);
-    lr.n1 = n1;
-    lr.vert.alloc(n1 ? n1 : 1);
-    lr.slot.alloc(n);
-    lr.hdeg.alloc(n1 ? n1 : 1);
-    LAUNCH(k_slots_from_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, n, n1, lr.vert.ptr, lr.slot.ptr, lr.hdeg.ptr);
+    pt.n1 = n1;
+    pt.vert.alloc(n1 ? n1 : 1);
+    pt.slot.alloc(n);
+    pt.hdeg.alloc(n1 ? n1 : 1);
+    LAUNCH(k_slots_from_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, n, n1, pt.vert.ptr, pt.slot.ptr, pt.hdeg.ptr);
     // the order over ALL vertices (the sort already put the sinks last, by id): frontiers may be stored in it (permuted form)
-    lr.pvert = std::make_shared<DevBuf<u32>>(n);
-    lr.pperm = std::make_shared<DevBuf<u32>>(n);
-    LAUNCH(k_full_order, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, n, lr.pvert->ptr, lr.pperm->ptr);
+    pt.pvert = std::make_shared<DevBuf<u32>>(n);
+    pt.pperm = std::make_shared<DevBuf<u32>>(n);
+    LAUNCH(k_full_order, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, n, pt.pvert->ptr, pt.pperm->ptr);
     static std::atomic<u64> next_tag{1};
-    lr.perm_tag = next_tag.fetch_add(1);
-    lr.packed = true;
+    pt.perm_tag = next_tag.fetch_add(1);
+    pt.packed = true;
 }
 
-// ---- CSR-stream form of A' ----------------------------------------------------------------------------------------
-__global__ void k_short_len(const u64 *__restrict__ p, u64 n, u64 LONG, u32 *__restrict__ len_s, u32 *__restrict__ lflag,
-                            u64 *__restrict__ maxlong) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    u64 mx = 0;
-    for (; r <= n; r += stride) {
-        if (r == n) { len_s[r] = 0; lflag[r] = 0; break; }
-        u64 d = p[r + 1] - p[r];
-        bool lg = d > LONG;
-        len_s[r] = lg ? 0u : (u32)d;
-        lflag[r] = lg ? 1u : 0u;
-        if (lg && d > mx) mx = d;
+// The pull tables of one matrix, built once per immutable base (B200_Matrix_prepare, or the first hop that pulls): the hot-set order
+// when hot_pack is on, A'.col_idx relabelled to it, and the segment list.  Turning hot_pack on after the tables were built without
+// it adds the order and the relabelled col_idx.
+static void build_pull_tables(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
+    if (!pt.packed && ctx().opt_hot_pack) build_hot_pack(A, AT, pt);
+    if (pt.packed && !pt.jp.ptr) {
+        pt.jp.alloc(AT.nnz);
+        LAUNCH(k_relabel_cols, grid_for(AT.nnz, 256, (u64)ctx().num_sms * 32), 256, 0, AT.j.ptr, AT.nnz, pt.slot.ptr, pt.jp.ptr);
     }
-    if (mx) atomicMax((unsigned long long *)maxlong, mx);
-}
-__global__ void k_long_meta(const u64 *__restrict__ p, u64 n, const u32 *__restrict__ lflag, const u64 *__restrict__ lpos,
-                            u64 nlong, u32 *__restrict__ lrows, u64 *__restrict__ llen) {
-    u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    if (r == 0) llen[nlong] = 0;
-    for (; r < n; r += stride)
-        if (lflag[r]) { lrows[lpos[r]] = (u32)r; llen[lpos[r]] = p[r + 1] - p[r]; }
-}
-__global__ void k_fill_stream(const u64 *__restrict__ p, const u32 *__restrict__ j, u64 n, const u32 *__restrict__ slot,
-                              const u64 *__restrict__ rp_s, u32 *__restrict__ jp_s, const u32 *__restrict__ lflag,
-                              const u64 *__restrict__ lpos, const u64 *__restrict__ lrp, u32 *__restrict__ jp_l) {
-    u64 warp = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    u64 nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
-    u32 lane = threadIdx.x & 31;
-    for (u64 r = warp; r < n; r += nwarps) {
-        u64 s = p[r], e = p[r + 1];
-        u32 *dst = lflag[r] ? (jp_l + lrp[lpos[r]]) : (jp_s + rp_s[r]);
-        for (u64 q = lane; q < e - s; q += 32) dst[q] = slot ? slot[j[s + q]] : j[s + q];
-    }
-}
-__global__ void k_window_starts(const u64 *__restrict__ rp_s, u64 n, u64 WIN, u64 nwin, u32 *__restrict__ wstart) {
-    u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k > nwin) return;
-    if (k == nwin) { wstart[k] = (u32)n; return; }
-    u64 target = k * WIN, lo = 0, hi = n;      // first row r in [0,n) with rp_s[r] >= target, else n
-    while (lo < hi) {
-        u64 mid = (lo + hi) >> 1;
-        if (rp_s[mid] < target) lo = mid + 1; else hi = mid;
-    }
-    wstart[k] = (u32)lo;
-}
-
-static u64 stream_window(u32 W) { return 1024 / W; }   // window (and short-row limit) in nnz; W <= 4
-
-void build_stream(const DevCSR &AT, LongRows &lr, u32 W) {
-    u64 n = AT.nrows;
-    u64 WIN = stream_window(W);
-    lr.sW = W; lr.swin = WIN; lr.s_packed = lr.packed;
-    DevBuf<u32> len_s(n + 1), lflag(n + 1);
-    DevBuf<u64> lpos(n + 1), mx(1);
-    mx.zero();
-    LAUNCH(k_short_len, grid_for(n + 1, 256, (u64)ctx().num_sms * 16), 256, 0, AT.p.ptr, n, WIN, len_s.ptr, lflag.ptr, mx.ptr);
-    lr.rp_s.alloc(n + 1);
-    exclusive_scan_u32_to_u64(len_s.ptr, lr.rp_s.ptr, n + 1);
-    exclusive_scan_u32_to_u64(lflag.ptr, lpos.ptr, n + 1);
-    lr.nnz_s = read_scalar(lr.rp_s.ptr + n);
-    lr.nlong = read_scalar(lpos.ptr + n);
-    lr.maxlong = read_scalar(mx.ptr);
-    lr.lrows.alloc(lr.nlong ? lr.nlong : 1);
-    lr.lrp.alloc(lr.nlong + 1);
-    LAUNCH(k_long_meta, grid_for(n ? n : 1, 256, (u64)ctx().num_sms * 16), 256, 0, AT.p.ptr, n, lflag.ptr, lpos.ptr, lr.nlong, lr.lrows.ptr, lr.lrp.ptr);
-    exclusive_scan_u64(lr.lrp.ptr, lr.lrp.ptr, lr.nlong + 1);
-    lr.jp_s.alloc(lr.nnz_s ? lr.nnz_s : 1);
-    lr.jp_l.alloc(AT.nnz - lr.nnz_s ? AT.nnz - lr.nnz_s : 1);
-    if (n) LAUNCH(k_fill_stream, grid_for(n * 32, 256, (u64)ctx().num_sms * 32), 256, 0, AT.p.ptr, AT.j.ptr, n, lr.packed ? lr.slot.ptr : (const u32 *)nullptr,
-                  lr.rp_s.ptr, lr.jp_s.ptr, lflag.ptr, lpos.ptr, lr.lrp.ptr, lr.jp_l.ptr);
-    lr.nwin = lr.nnz_s / WIN + 1;
-    lr.wstart.alloc(lr.nwin + 1);
-    LAUNCH(k_window_starts, grid_for(lr.nwin + 1, 256), 256, 0, lr.rp_s.ptr, n, WIN, lr.nwin, lr.wstart.ptr);
-}
-
-// flat coalesced gather of one window's nnz into shared memory, then one thread per row reduces its segment
-template <int W>
-__global__ void __launch_bounds__(128)
-k_bits_pull_stream(const u64 *__restrict__ rp_s, const u32 *__restrict__ jp_s, const u32 *__restrict__ wstart,
-                   const u64 *__restrict__ Xp, u64 *__restrict__ Y) {
-    extern __shared__ u64 sxs[];
-    const u32 tid = threadIdx.x;
-    u32 r0 = wstart[blockIdx.x], r1 = wstart[blockIdx.x + 1];
-    if (r0 == r1) return;
-    u64 base = rp_s[r0];
-    u32 nnzb = (u32)(rp_s[r1] - base);
-    const u32 *cols = jp_s + base;
-#pragma unroll 4
-    for (u32 e = tid; e < nnzb; e += 128) {
-        u32 col = cols[e];
-#pragma unroll
-        for (int w = 0; w < W; w++) sxs[(size_t)e * W + w] = Xp[(u64)col * W + w];
-    }
-    __syncthreads();
-    for (u32 r = r0 + tid; r < r1; r += 128) {
-        u32 s = (u32)(rp_s[r] - base), e = (u32)(rp_s[r + 1] - base);
-        u64 acc[W];
-#pragma unroll
-        for (int w = 0; w < W; w++) acc[w] = 0;
-        for (u32 q = s; q < e; q++) {
-#pragma unroll
-            for (int w = 0; w < W; w++) acc[w] |= sxs[(size_t)q * W + w];
-        }
-#pragma unroll
-        for (int w = 0; w < W; w++) Y[(u64)r * W + w] = acc[w];
+    if (!pt.built) {
+        build_seg_list(AT, pt);
+        pt.built = true;
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(256)
-k_bits_pull_stream_long(const u32 *__restrict__ lrows, const u64 *__restrict__ lrp, const u32 *__restrict__ jp_l,
-                        const u64 *__restrict__ Xp, u64 *__restrict__ Y) {
-    typedef cub::BlockReduce<u64, 256> Red;
-    __shared__ typename Red::TempStorage ts;
-    u64 s = lrp[blockIdx.x], e = lrp[blockIdx.x + 1];
-    u64 c0 = s + (u64)blockIdx.y * LONG_CHUNK;
-    if (c0 >= e) return;
-    u64 c1 = c0 + LONG_CHUNK;
-    if (c1 > e) c1 = e;
-    u64 acc[W];
-#pragma unroll
-    for (int w = 0; w < W; w++) acc[w] = 0;
-#pragma unroll 4
-    for (u64 q = c0 + threadIdx.x; q < c1; q += 256) {
-        u32 k = jp_l[q];
-#pragma unroll
-        for (int w = 0; w < W; w++) acc[w] |= Xp[(u64)k * W + w];
-    }
-    u32 row = lrows[blockIdx.x];
-#pragma unroll
-    for (int w = 0; w < W; w++) {
-        u64 r = Red(ts).Reduce(acc[w], OrOp64());
-        __syncthreads();
-        if (threadIdx.x == 0 && r) atomicOr((unsigned long long *)&Y[(u64)row * W + w], r);
-    }
-}
-
-void build_long_rows(const DevCSR &AT, LongRows &lr) {
-    u64 n = AT.nrows;
-    lr.rows.release();
-    lr.n = 0;
-    lr.built = true;
-    if (n == 0) return;
-    DevBuf<u32> flag(n + 1);
-    DevBuf<u64> pos(n + 1), mx(1);
-    mx.zero();
-    LAUNCH(k_flag_long, grid_for(n, 256, 1 << 16), 256, 0, AT.p.ptr, n, flag.ptr, mx.ptr);
-    CUDA_TRY(cudaMemsetAsync(flag.ptr + n, 0, sizeof(u32), stream()));
-    exclusive_scan_u32_to_u64(flag.ptr, pos.ptr, n + 1);
-    u64 nl = read_scalar(pos.ptr + n);
-    lr.n = nl;
-    lr.maxdeg = read_scalar(mx.ptr);
-    if (nl) {
-        lr.rows.alloc(nl);
-        LAUNCH(k_scatter_flagged, grid_for(n, 256, 1 << 16), 256, 0, flag.ptr, pos.ptr, n, lr.rows.ptr);
-        lr.choff.alloc(nl + 1);
-        LAUNCH(k_long_chunks, grid_for(nl + 1, 256), 256, 0, lr.rows.ptr, nl, AT.p.ptr, lr.choff.ptr);
-        exclusive_scan_u64(lr.choff.ptr, lr.choff.ptr, nl + 1);
-        lr.nchunks = read_scalar(lr.choff.ptr + nl);
-    }
-    build_mid_list(AT, lr);
-    if (lr.packed) {
-        lr.jp.alloc(AT.nnz);
-        LAUNCH(k_relabel_cols, grid_for(AT.nnz, 256, (u64)ctx().num_sms * 32), 256, 0, AT.j.ptr, AT.nnz, lr.slot.ptr, lr.jp.ptr);
-    }
-    u64 ndiag = (n + AT.nnz) / 256 + 2;
-    lr.mp_r.alloc(ndiag);
-    LAUNCH(k_mp_coords, grid_for(ndiag, 256), 256, 0, AT.p.ptr, n, AT.nnz, ndiag, lr.mp_r.ptr);
-}
-
-// persisting-L2 access-policy window on the library stream (cudaLimitPersistingL2CacheSize is set at context bring-up)
-static u64 g_l2_carved = 0;        // bytes of L2 currently set aside for persisting accesses
-static void carve_l2(u64 bytes) {
-    if (bytes == g_l2_carved) return;
-    CUDA_TRY(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, bytes));
-    g_l2_carved = bytes;
-}
-static void set_l2_window(const void *base, u64 bytes) {
+// k_pull_small over every row of A', then k_pull_seg over the segment list.  The segment kernel's grid is every CTA resident at
+// once (occupancy x SMs) unless pull_grid overrides it: entries are dealt round-robin to 8-lane groups, so one full wave keeps all
+// SMs busy to the end.
+template <int W, bool HINTS>
+static void launch_pull(const DevCSR &AT, const PullTables &pt, u64 m, const u32 *gj, const u64 *gx, u64 *Y, const u64 *Gp,
+                        u32 hot_bytes, u32 tot_bytes) {
     Context &cx = ctx();
-    if (cx.l2_persist_max == 0) return;
-    carve_l2(std::min<u64>(bytes, cx.l2_persist_max));
-    cudaStreamAttrValue a;
-    memset(&a, 0, sizeof(a));
-    u64 nb = bytes;
-    if (nb > cx.l2_window_max) nb = cx.l2_window_max;
-    a.accessPolicyWindow.base_ptr = const_cast<void *>(base);
-    a.accessPolicyWindow.num_bytes = nb;
-    a.accessPolicyWindow.hitRatio = nb <= g_l2_carved ? 1.0f : (float)((double)g_l2_carved / (double)nb);
-    a.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    a.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    CUDA_TRY(cudaStreamSetAttribute(stream(), cudaStreamAttributeAccessPolicyWindow, &a));
-}
-static void clear_l2_window() {
-    Context &cx = ctx();
-    if (cx.l2_persist_max == 0) return;
-    cudaStreamAttrValue a;
-    memset(&a, 0, sizeof(a));
-    a.accessPolicyWindow.num_bytes = 0;
-    a.accessPolicyWindow.hitRatio = 0.0f;
-    a.accessPolicyWindow.hitProp = cudaAccessPropertyNormal;
-    a.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
-    CUDA_TRY(cudaStreamSetAttribute(stream(), cudaStreamAttributeAccessPolicyWindow, &a));
-    if (cx.opt_l2_reset) CUDA_TRY(cudaCtxResetPersistingL2Cache());
-    if (cx.opt_l2_reset >= 2) carve_l2(0);       // hand the set-aside back to the other kernels until the next pull
+    LAUNCH((k_pull_small<W, HINTS>), grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT.p.ptr, gj, m, gx, Y, hot_bytes, tot_bytes);
+    if (!pt.ns) return;
+    auto seg = [&](auto kern) {
+        int per_sm = 0;
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, 0));
+        if (per_sm < 1) per_sm = 1;
+        if (cx.opt_pull_grid > 0) per_sm = (int)cx.opt_pull_grid;
+        LAUNCH(kern, (u32)cx.num_sms * (u32)per_sm, 256, 0, pt.s_row.ptr, pt.s_start.ptr, pt.s_len.ptr, pt.ns, gj, gx, Y, Gp, hot_bytes,
+               tot_bytes);
+    };
+    if (Gp) seg(k_pull_seg<W, HINTS, 4, true>);
+    else seg(k_pull_seg<W, HINTS, 4, false>);
 }
 
 template <int W>
-static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, LongRows *lr, DevBits &Y,
+static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y,
                      u64 *flops_out, int *path_out) {
     Context &cx = ctx();
     u64 n = A.nrows, m = A.ncols;
     // X in permuted form: usable as it stands only by the pull through the tables it was ordered for; anything else works on a
     // natural-order copy (cannot happen on the bench path: the caller orders a frontier only for the operand it is pushed through)
     DevBits Xnat;
-    const bool ordered = Xin.permuted() && AT && lr && lr->packed && Xin.perm_tag == lr->perm_tag && lr->jp.ptr && lr->hdeg.ptr &&
-                         cx.opt_pull_mode != 0 && cx.opt_hot_pack && cx.opt_pull_kernel >= 4 && n == m;
+    const bool ordered = Xin.permuted() && AT && pt && pt->packed && Xin.perm_tag == pt->perm_tag && pt->jp.ptr && pt->hdeg.ptr &&
+                         cx.opt_pull_mode != 0 && cx.opt_hot_pack && n == m;
     const DevBits *Xuse = &Xin;
     if (Xin.permuted() && !ordered) { bits_copy(Xin, Xnat); bits_naturalise(Xnat); Xuse = &Xnat; }
     const DevBits &X = *Xuse;
@@ -1918,18 +1134,18 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Long
     st.zero();
     // fused_prep: when the hot-set tables exist, one pass packs the frontier for the pull AND yields flops / edges / the OR
     // terminal; the separate flops pass (needed for its per-vertex flags) then only runs if the push direction wins
-    const bool fused = cx.opt_fused_prep && AT && lr && cx.opt_hot_pack && lr->packed && lr->jp.ptr && lr->hdeg.ptr &&
-                       cx.opt_pull_mode != 0 && cx.opt_pull_kernel != 2 && n == m;
+    const bool fused = cx.opt_fused_prep && AT && pt && cx.opt_hot_pack && pt->packed && pt->jp.ptr && pt->hdeg.ptr &&
+                       cx.opt_pull_mode != 0 && n == m;
     DevBuf<u64> Xp, Gd;
     if (ordered) {            // already in gather order: totals only
         Gd.alloc(W);
         Gd.zero();
-        if (lr->n1) LAUNCH((k_ordered_flops<W>), grid_for(lr->n1 * W, 256, (u64)ctx().num_sms * 16), 256, 0, lr->hdeg.ptr, lr->n1, X.w.ptr, st.ptr, Gd.ptr);
+        if (pt->n1) LAUNCH((k_ordered_flops<W>), grid_for(pt->n1 * W, 256, (u64)ctx().num_sms * 16), 256, 0, pt->hdeg.ptr, pt->n1, X.w.ptr, st.ptr, Gd.ptr);
     } else if (fused) {
-        Xp.alloc(lr->n1 * W);
+        Xp.alloc(pt->n1 * W);
         Gd.alloc(W);
         Gd.zero();
-        if (lr->n1) LAUNCH((k_pack_flops<W>), grid_for(lr->n1 * W, 256, (u64)ctx().num_sms * 16), 256, 0, lr->vert.ptr, lr->hdeg.ptr, lr->n1, X.w.ptr, Xp.ptr, st.ptr, Gd.ptr);
+        if (pt->n1) LAUNCH((k_pack_flops<W>), grid_for(pt->n1 * W, 256, (u64)ctx().num_sms * 16), 256, 0, pt->vert.ptr, pt->hdeg.ptr, pt->n1, X.w.ptr, Xp.ptr, st.ptr, Gd.ptr);
     } else if (n) LAUNCH(k_bits_flops, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, X.w.ptr, (u32)W, n, A.p.ptr, flag.ptr, st.ptr);
     u64 hst[2] = {0, 0};
     d2h(hst, st.ptr, 2);
@@ -1937,175 +1153,25 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Long
     if (flops_out) *flops_out = hst[0];
     u64 edges = hst[1];
     bool pull = false;
-    if (AT && lr) {
+    if (AT && pt) {
         if (cx.opt_pull_mode == 1) pull = true;
         else if (cx.opt_pull_mode == 0) pull = false;
         else pull = edges * 4 > A.nnz; // direction switch: frontier touches > 1/4 of the edges
     }
     if (edges == 0) { Y.w.zero(); if (path_out) *path_out = 0; return; }
-    const u32 *gj = AT ? AT->j.ptr : nullptr;   // gather index stream
-    const u64 *gx = X.w.ptr;                    // gather source
-    u64 gn = n;                                 // gather footprint in vertices
     if (ordered && !pull) {                     // the push direction works on natural order: undo the frontier's order and start over
         DevBits Xn;
         bits_copy(Xin, Xn);
         bits_naturalise(Xn);
-        hop_impl<W>(Xn, A, AT, lr, Y, flops_out, path_out);
+        hop_impl<W>(Xn, A, AT, pt, Y, flops_out, path_out);
         return;
     }
-    if (fused && !ordered && !pull) {           // push needs the per-vertex active flags of the classic pass
-        DevBuf<u64> st2(2);
-        st2.zero();
-        LAUNCH(k_bits_flops, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, X.w.ptr, (u32)W, n, A.p.ptr, flag.ptr, st2.ptr);
-    }
-    const bool stream_kernel = pull && W <= 4 && cx.opt_pull_kernel == 2;
-    if (pull) {   // auxiliary tables are built once per (immutable) matrix, lazily
-        if (!lr->packed && cx.opt_hot_pack) build_hot_pack(A, *AT, *lr);
-        if (stream_kernel) { if (lr->sW != (u32)W || lr->s_packed != lr->packed) build_stream(*AT, *lr, W); }
-        else if (!lr->built || (lr->packed && !lr->jp.ptr)) build_long_rows(*AT, *lr);
-    }
-    if (stream_kernel) {
-        if (lr->s_packed) {
-            Xp.alloc(lr->n1 * W);
-            if (lr->n1) LAUNCH((k_pack_frontier<W>), grid_for(lr->n1 * W, 256, (u64)ctx().num_sms * 32), 256, 0, lr->vert.ptr, lr->n1, X.w.ptr, Xp.ptr);
-            gx = Xp.ptr; gn = lr->n1;
+    if (!pull) {
+        if (fused) {                            // push needs the per-vertex active flags of the classic pass
+            DevBuf<u64> st2(2);
+            st2.zero();
+            LAUNCH(k_bits_flops, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, X.w.ptr, (u32)W, n, A.p.ptr, flag.ptr, st2.ptr);
         }
-        const size_t smem = (size_t)2 * lr->swin * W * sizeof(u64);
-        {
-            TimedScope ts(TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + 8ULL * W * m);
-            LAUNCH((k_bits_pull_stream<W>), (u32)lr->nwin, 128, smem, lr->rp_s.ptr, lr->jp_s.ptr, lr->wstart.ptr, gx, Y.w.ptr);
-        }
-        if (lr->nlong) {
-            dim3 g((u32)lr->nlong, (u32)((lr->maxlong + LONG_CHUNK - 1) / LONG_CHUNK));
-            TimedScope ts(TK_BITS_PULL_LONG, 0);
-            LAUNCH((k_bits_pull_stream_long<W>), g, 256, 0, lr->lrows.ptr, lr->lrp.ptr, lr->jp_l.ptr, gx, Y.w.ptr);
-        }
-        if (path_out) *path_out = 5;
-        return;
-    }
-    if (ordered) {                              // the frontier already is the packed gather source (its first n1 records)
-        gj = lr->jp.ptr; gx = X.w.ptr; gn = lr->n1;
-    } else if (pull && cx.opt_hot_pack && lr->packed && lr->jp.ptr) {
-        if (!fused) {
-            Xp.alloc(lr->n1 * W);
-            if (lr->n1) LAUNCH((k_pack_frontier<W>), grid_for(lr->n1 * W, 256, (u64)ctx().num_sms * 32), 256, 0, lr->vert.ptr, lr->n1, X.w.ptr, Xp.ptr);
-        }
-        gj = lr->jp.ptr; gx = Xp.ptr; gn = lr->n1;
-    }
-    const u64 *Gp = nullptr;
-    // opt_early_exit: 0 never, 1 auto, 2 always.  Auto: the in-loop vote pays for itself at W = 2 and 4 (hub rows saturate),
-    // costs more than it saves at W = 1 (few rows ever hold all 64 bits) and at W >= 8; very dense frontiers always benefit.
-    const bool dense_frontier = hst[0] >= (hst[1] * X.nrows) / 4;   // flops/edges = degree-weighted mean popcount of a gathered word
-    if (pull && (cx.opt_early_exit == 2 || (cx.opt_early_exit == 1 && (dense_frontier || W == 2 || W == 4)))) {
-        if (!((fused && gx == Xp.ptr) || ordered)) {   // the fused / ordered pass already left the OR of the packed frontier in Gd
-            Gd.alloc(W);
-            Gd.zero();
-            if (gn) LAUNCH((k_or_all<W>), grid_for(gn, 256, (u64)ctx().num_sms * 8), 256, 0, gx, gn, Gd.ptr);
-        }
-        Gp = Gd.ptr;
-    }
-    if (pull && cx.opt_pull_kernel == 1) {
-        constexpr int TILE = MpCfg<W>::TILE;
-        const size_t smem = ((size_t)TILE * W + (size_t)(TILE + 1) * W) * sizeof(u64) + (size_t)(TILE + 2) * sizeof(u32);
-        static bool attr_set = false;
-        if (!attr_set) {
-            CUDA_TRY(cudaFuncSetAttribute(k_bits_pull_mp<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr_set = true;
-        }
-        Y.w.zero();
-        u64 total = m + AT->nnz;
-        u64 ntiles = (total + TILE - 1) / TILE;
-        TimedScope ts(TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + 8ULL * W * m);
-        LAUNCH((k_bits_pull_mp<W>), (u32)ntiles, 256, smem, AT->p.ptr, gj, m, AT->nnz, gx, Y.w.ptr, lr->mp_r.ptr);
-        if (path_out) *path_out = 4;
-    } else if (pull) {
-        {
-            // compulsory traffic: stream A' col_idx + rowptr, read X once, write Y once (X gathers hit L2)
-            TimedScope ts(TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + 8ULL * W * m);
-            // early termination only pays when the gathered words are dense (degree-weighted mean popcount >= 1/4 of the rows)
-            const bool early = Gp != nullptr;
-            u64 totb = gn * W * 8;
-            const u32 tot_bytes = totb > 0xFFFFFFF0ULL ? 0xFFFFFFF0u : (u32)totb;
-            const u32 hot_bytes = (u64)cx.opt_hot_bytes < tot_bytes ? (u32)cx.opt_hot_bytes : tot_bytes;
-            // grid = every CTA resident at once (occupancy x SMs) unless pull_grid overrides it: rows are dealt round-robin to
-            // 8-lane groups, so one full wave keeps all SMs busy to the end
-            if (cx.opt_pull_kernel >= 5) {
-                if (!lr->seg_built) build_seg_list(*AT, *lr);
-                auto occ = [&](auto kern) {
-                    int per_sm = 0;
-                    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, 0));
-                    if (per_sm < 1) per_sm = 1;
-                    if (cx.opt_pull_grid > 0) per_sm = (int)cx.opt_pull_grid;
-                    return (u32)cx.num_sms * (u32)per_sm;
-                };
-                // keep the hot prefix of the packed frontier L2-resident for the duration of the pull: a persisting access-policy
-                // window on the library stream (the per-instruction hints are off by default above W = 2)
-                const bool window = cx.opt_l2_window > 0 && (gx == Xp.ptr || ordered) && gn;
-                if (window) set_l2_window(gx, std::min<u64>((u64)cx.opt_l2_window, gn * W * 8));
-                auto small = [&](auto kern, u64 split) {
-                    LAUNCH(kern, grid_for(m * split, 256, (u64)cx.num_sms * 32), 256, 0, AT->p.ptr, gj, m, gx, Y.w.ptr, hot_bytes, tot_bytes);
-                };
-                constexpr int SP = PullCfg<W>::SPLIT;
-                auto seg = [&](auto kern) {
-                    if (lr->ns) LAUNCH(kern, occ(kern), 256, 0, lr->s_row.ptr, lr->s_start.ptr, lr->s_len.ptr, lr->ns, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-                };
-#define SEG_LAUNCH(H) do { \
-        if (cx.opt_unroll >= 8) { if (early) seg(k_pull_seg<W, H, 8, true>); else seg(k_pull_seg<W, H, 8, false>); } \
-        else if (cx.opt_unroll >= 4) { if (early) seg(k_pull_seg<W, H, 4, true>); else seg(k_pull_seg<W, H, 4, false>); } \
-        else { if (early) seg(k_pull_seg<W, H, 2, true>); else seg(k_pull_seg<W, H, 2, false>); } } while (0)
-#define SMALL_LAUNCH(H) do { if (cx.opt_small_split && SP > 1) small(k_pull_small<W, H, SP>, SP); else small(k_pull_small<W, H, 1>, 1); } while (0)
-                if (cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2)) { SMALL_LAUNCH(true); SEG_LAUNCH(true); }
-                else { SMALL_LAUNCH(false); SEG_LAUNCH(false); }
-#undef SMALL_LAUNCH
-#undef SEG_LAUNCH
-                if (window) clear_l2_window();
-                if (path_out) *path_out = 3;
-                return;
-            } else if (cx.opt_pull_kernel == 4) {
-                auto occ = [&](auto kern) {
-                    int per_sm = 0;
-                    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, 0));
-                    if (per_sm < 1) per_sm = 1;
-                    if (cx.opt_pull_grid > 0) per_sm = (int)cx.opt_pull_grid;
-                    return (u32)cx.num_sms * (u32)per_sm;
-                };
-                auto small = [&](auto kern) { LAUNCH(kern, grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT->p.ptr, gj, m, gx, Y.w.ptr, hot_bytes, tot_bytes); };
-                auto mid = [&](auto kern) {
-                    if (lr->nm) LAUNCH(kern, occ(kern), 256, 0, lr->m_row.ptr, lr->m_start.ptr, lr->m_len.ptr, lr->nm, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-                };
-#define MID_LAUNCH(H) do { \
-        if (cx.opt_unroll >= 8) { if (early) mid(k_bits_pull_mid<W, H, 8, true>); else mid(k_bits_pull_mid<W, H, 8, false>); } \
-        else if (cx.opt_unroll >= 4) { if (early) mid(k_bits_pull_mid<W, H, 4, true>); else mid(k_bits_pull_mid<W, H, 4, false>); } \
-        else { if (early) mid(k_bits_pull_mid<W, H, 2, true>); else mid(k_bits_pull_mid<W, H, 2, false>); } } while (0)
-                if (cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2)) { small(k_bits_pull_small<W, true>); MID_LAUNCH(true); }
-                else { small(k_bits_pull_small<W, false>); MID_LAUNCH(false); }
-#undef MID_LAUNCH
-            } else {
-            auto go = [&](auto kern) {
-                int per_sm = 0;
-                CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, 0));
-                if (per_sm < 1) per_sm = 1;
-                if (cx.opt_pull_grid > 0) per_sm = (int)cx.opt_pull_grid;
-                const u32 g = (u32)cx.num_sms * (u32)per_sm;
-                LAUNCH(kern, g, 256, 0, AT->p.ptr, gj, m, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-            };
-#define PULL_LAUNCH(H, UU) do { \
-        if (cx.opt_pull_kernel == 0) { if (early) go(k_bits_pull<W, H, UU, true>); else go(k_bits_pull<W, H, UU, false>); } \
-        else { if (early) go(k_bits_pull_pipe<W, H, UU, true>); else go(k_bits_pull_pipe<W, H, UU, false>); } } while (0)
-            if (cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2)) {
-                if (cx.opt_unroll >= 4) PULL_LAUNCH(true, 4); else if (cx.opt_unroll >= 2) PULL_LAUNCH(true, 2); else PULL_LAUNCH(true, 1);
-            } else {
-                if (cx.opt_unroll >= 4) PULL_LAUNCH(false, 4); else if (cx.opt_unroll >= 2) PULL_LAUNCH(false, 2); else PULL_LAUNCH(false, 1);
-            }
-#undef PULL_LAUNCH
-            }
-        }
-        if (lr->n) {
-            TimedScope ts(TK_BITS_PULL_LONG, 0);
-            LAUNCH((k_bits_pull_long<W>), (u32)lr->nchunks, 256, 0, lr->rows.ptr, lr->choff.ptr, (u32)lr->n, AT->p.ptr, gj, gx, Y.w.ptr, Gp);
-        }
-        if (path_out) *path_out = 3;
-    } else {
         Y.w.zero();
         CUDA_TRY(cudaMemsetAsync(flag.ptr + n, 0, sizeof(u32), stream()));
         DevBuf<u64> pos(n + 1);
@@ -2123,27 +1189,60 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Long
             LAUNCH((k_bits_push<W>), (u32)nchunks, 256, 0, act.ptr, cum.ptr, astart.ptr, nact, edges, A.j.ptr, X.w.ptr, Y.w.ptr);
         }
         if (path_out) *path_out = 2;
+        return;
     }
+    build_pull_tables(A, *AT, *pt);             // a no-op once the matrix has them
+    const u32 *gj = AT->j.ptr;                  // gather index stream
+    const u64 *gx = X.w.ptr;                    // gather source
+    u64 gn = n;                                 // gather footprint in vertices
+    if (ordered) {                              // the frontier already is the packed gather source (its first n1 records)
+        gj = pt->jp.ptr; gx = X.w.ptr; gn = pt->n1;
+    } else if (cx.opt_hot_pack && pt->packed) {
+        if (!fused) {
+            Xp.alloc(pt->n1 * W);
+            if (pt->n1) LAUNCH((k_pack_frontier<W>), grid_for(pt->n1 * W, 256, (u64)ctx().num_sms * 32), 256, 0, pt->vert.ptr, pt->n1, X.w.ptr, Xp.ptr);
+        }
+        gj = pt->jp.ptr; gx = Xp.ptr; gn = pt->n1;
+    }
+    const u64 *Gp = nullptr;
+    // opt_early_exit: 0 never, 1 auto, 2 always.  Auto: the in-loop vote pays for itself at W = 2 and 4 (hub rows saturate),
+    // costs more than it saves at W = 1 (few rows ever hold all 64 bits) and at W >= 8; very dense frontiers always benefit.
+    const bool dense_frontier = hst[0] >= (hst[1] * X.nrows) / 4;   // flops/edges = degree-weighted mean popcount of a gathered word
+    if (cx.opt_early_exit == 2 || (cx.opt_early_exit == 1 && (dense_frontier || W == 2 || W == 4))) {
+        if (!((fused && gx == Xp.ptr) || ordered)) {   // the fused / ordered pass already left the OR of the packed frontier in Gd
+            Gd.alloc(W);
+            Gd.zero();
+            if (gn) LAUNCH((k_or_all<W>), grid_for(gn, 256, (u64)ctx().num_sms * 8), 256, 0, gx, gn, Gd.ptr);
+        }
+        Gp = Gd.ptr;
+    }
+    {
+        // compulsory traffic: stream A' col_idx + rowptr, read X once, write Y once (X gathers hit L2)
+        TimedScope ts(TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + 8ULL * W * m);
+        u64 totb = gn * W * 8;
+        const u32 tot_bytes = totb > 0xFFFFFFF0ULL ? 0xFFFFFFF0u : (u32)totb;
+        const u32 hot_bytes = (u64)cx.opt_hot_bytes < tot_bytes ? (u32)cx.opt_hot_bytes : tot_bytes;
+        if (cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2)) launch_pull<W, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+        else launch_pull<W, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+    }
+    if (path_out) *path_out = 3;
 }
 
-// builds every per-matrix table of the pull direction now (B200_Matrix_prepare) instead of inside the first hop that pulls
-void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, LongRows &lr) {
+// builds the pull tables of a square operand now (B200_Matrix_prepare) instead of inside the first hop that pulls
+void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     if (A.nrows != A.ncols || !AT.nnz) return;
-    Context &cx = ctx();
-    if (!lr.packed && cx.opt_hot_pack) build_hot_pack(A, AT, lr);
-    if (!lr.built || (lr.packed && !lr.jp.ptr)) build_long_rows(AT, lr);
-    if (cx.opt_pull_kernel >= 5 && !lr.seg_built) build_seg_list(AT, lr);
+    build_pull_tables(A, AT, pt);
 }
 
-void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, LongRows *lr, DevBits &Y, u64 *flops_out,
+void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y, u64 *flops_out,
               int *path_out) {
     if (X.ncols != A.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
     switch (X.W) {
-    case 1: hop_impl<1>(X, A, AT, lr, Y, flops_out, path_out); break;
-    case 2: hop_impl<2>(X, A, AT, lr, Y, flops_out, path_out); break;
-    case 4: hop_impl<4>(X, A, AT, lr, Y, flops_out, path_out); break;
-    case 8: hop_impl<8>(X, A, AT, lr, Y, flops_out, path_out); break;
-    case 16: hop_impl<16>(X, A, AT, lr, Y, flops_out, path_out); break;
+    case 1: hop_impl<1>(X, A, AT, pt, Y, flops_out, path_out); break;
+    case 2: hop_impl<2>(X, A, AT, pt, Y, flops_out, path_out); break;
+    case 4: hop_impl<4>(X, A, AT, pt, Y, flops_out, path_out); break;
+    case 8: hop_impl<8>(X, A, AT, pt, Y, flops_out, path_out); break;
+    case 16: hop_impl<16>(X, A, AT, pt, Y, flops_out, path_out); break;
     default: throw GrbError(-8, "bit-frontier: unsupported word count");
     }
 }

@@ -53,15 +53,9 @@ struct Context {
     i64 opt_bits_min_flops = 1 << 22;     // auto mode: use bit-frontier when flops >= this
     i64 opt_sync_after_op = 0;
     i64 opt_timing = 0;
-    i64 opt_pull_kernel = 5;       // 5 = lane-split degree-binned (default); 4 = degree-binned, one lane per vertex record; 0..3 = earlier kernels
     i64 opt_perm_push = 1;         // a CSR frontier pushed through a prepared matrix lands in that matrix's hot-set order (no packing pass before the next pull)
-    i64 opt_small_split = 0;       // small-row pull kernel: 1 = split the vertex record across lanes like the segment kernel, 0 = one lane per record
-    i64 opt_l2_window = 0;         // bytes of the packed frontier's hot prefix kept L2-resident through a persisting access-policy window (0 = off)
-    i64 opt_l2_reset = 0;          // cudaCtxResetPersistingL2Cache after each windowed pull
-    i64 opt_count_kernel = 1;      // materialise count pass: 1 = vertical (carry-save) counters, 0 = transpose + popcount
     i64 opt_bfs_direction = 0;     // 0 = direction-optimising, 1 = top-down only, 2 = bottom-up only (test hooks)
     i64 opt_bfs_sparse_exchange = 1;   // partitioned BFS: ship discovered-vertex lists instead of bitmaps when the frontier is sparse
-    u64 l2_persist_max = 0, l2_window_max = 0;   // device limits (bytes), read at bring-up
     i64 opt_early_exit = 1;        // stop a pull row once it holds the OR monoid's terminal value (exact)
     i64 opt_hints = -1;            // L2 createpolicy hints in the pull kernels: -1 = auto (on for W <= 2), 0 / 1 = off / on
     i64 opt_hot_bytes = 64 << 20;  // size of that hot prefix
@@ -69,8 +63,7 @@ struct Context {
     i64 opt_fused_prep = 1;        // pull hops: pack the frontier, count flops / edges and OR it in one pass
     i64 opt_csr_push = 1;          // tiny CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes)
     i64 opt_diag_filter = 1;       // frontier-form mxm by a diagonal (label) matrix runs as an elementwise column filter
-    i64 opt_pull_grid = 0;         // CTAs per SM of the grid-stride pull kernels (0 = occupancy: one resident wave)
-    i64 opt_unroll = 4;            // gathers in flight per lane in the 8-lane pull kernel
+    i64 opt_pull_grid = 0;         // CTAs per SM of the segment pull kernel (0 = occupancy: one resident wave)
 };
 Context &ctx();
 void ensure_init();
@@ -78,7 +71,7 @@ void ensure_init();
 inline cudaStream_t stream() { return ctx().stream; }
 
 // ---- optional per-kernel timing (CUDA events on the launch stream; B200_set_option("timing",1)) ----
-enum TimedId { TK_BITS_PULL = 0, TK_BITS_PULL_LONG, TK_BITS_PUSH, TK_HEAVY_ACC, TK_SMALL_ROWS, TK_BITS_FILL, TK_BITS_COUNT,
+enum TimedId { TK_BITS_PULL = 0, TK_BITS_PUSH, TK_HEAVY_ACC, TK_SMALL_ROWS, TK_BITS_FILL, TK_BITS_COUNT,
                TK_BITMAP_EXPAND, TK_BFS_EXPAND, TK_UNION, TK_FILTER, TK_MXV, TK_MASKED, TK_TRANSPOSE, TK_COUNT_ };
 const char *timed_name(int id);
 void timed_begin(int id);
@@ -196,7 +189,7 @@ struct DevBits {
     u32 W = 0;
     DevBuf<u64> w;
     // Permuted form (bits.cu, "hot-set order"): the words of vertex v live at position pos(v) instead of v, pos = the degree-sorted
-    // gather order of the matrix this frontier is about to be multiplied by (LongRows::pperm), so the pull of the next hop gathers
+    // gather order of the matrix this frontier is about to be multiplied by (PullTables::pperm), so the pull of the next hop gathers
     // straight from it with no packing pass.  pvert[position] = vertex undoes it; perm_tag names the permutation (0 = natural).
     std::shared_ptr<DevBuf<u32>> pvert;
     u64 perm_tag = 0;

@@ -139,7 +139,7 @@ struct GB_Matrix_opaque : UObject {
     DevBits bits;
     bool devT_valid = false;
     DevCSR devT;
-    LongRows lr;
+    PullTables pt;   // pull-direction tables of devT (bits.cu)
     DevBuf<u32> bfs_deg; u64 bfs_edges = 0; bool bfs_deg_valid = false;   // out-degree table of the BFS engine (bfs_do.cu)
     int sparsity_control = GxB_HYPERSPARSE | GxB_SPARSE | GxB_BITMAP | GxB_FULL;
     int hyper_hash = 1;
@@ -244,7 +244,7 @@ static void invalidate_aux(GrB_Matrix A) {
     A->bfs_deg.release(); A->bfs_deg_valid = false; A->bfs_edges = 0;
     A->devT_valid = false;
     A->devT.clear();
-    A->lr.clear();
+    A->pt.clear();
 }
 
 static void set_dev(GrB_Matrix A, DevCSR &&d) {
@@ -1066,14 +1066,14 @@ GrB_Info GrB_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_BinaryOp accum, GrB_Semiring
                 // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
                 const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
                                       A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
-                                      !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, &fl, (B->devT_valid && !Mask) ? &B->lr : (const LongRows *)nullptr);
+                                      !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, &fl, (B->devT_valid && !Mask) ? &B->pt : (const PullTables *)nullptr);
                 if (from_csr) path = 7;
                 else if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
                 if (from_csr) {}
                 else if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, &fl); path = 5; }
                 else {
                     if (cx.opt_pull_mode != 0) ensure_devT(B);
-                    bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->lr : (LongRows *)nullptr, Y, &fl, &path);
+                    bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, &fl, &path);
                 }
                 if (Mask) {
                     ensure_bits(Mask);
@@ -2121,7 +2121,7 @@ GrB_Info B200_Matrix_prepare(GrB_Matrix A, int want_transpose) {
         ensure_dev(A);
         if (want_transpose) {
             ensure_devT(A);
-            bits_prepare_pull(A->dev, A->devT, A->lr);     // hot-set order, degree bins, segment list: off the first query's path
+            bits_prepare_pull(A->dev, A->devT, A->pt);     // hot-set order, relabelled col_idx, segment list: off the first query's path
         }
         sync_stream();
         return GrB_SUCCESS;
@@ -2453,10 +2453,8 @@ uint64_t B200_get_stat(const char *name) {
     if (n == "h2d_bytes") return c.h2d_bytes.load();
     if (n == "d2h_bytes") return c.d2h_bytes.load();
     if (n == "num_sms") return (uint64_t)c.num_sms;
-    if (n == "l2_persist_max") return c.l2_persist_max;
     if (n == "host_bytes") return g_host_bytes.load();     // live bytes obtained through the GxB_init allocator hooks
     if (n == "host_allocs") return g_host_allocs.load();
-    if (n == "l2_window_max") return c.l2_window_max;
     return ~0ULL;
 }
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes) {
@@ -2485,23 +2483,19 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "bitmap_budget") c.opt_bitmap_budget = value;
     else if (n == "bits_min_flops") c.opt_bits_min_flops = value;
     else if (n == "sync_after_op") c.opt_sync_after_op = value;
-    else if (n == "pull_kernel") c.opt_pull_kernel = value;
     else if (n == "hints") c.opt_hints = value;
     else if (n == "hot_pack") c.opt_hot_pack = value;
     else if (n == "hot_bytes") c.opt_hot_bytes = value;
     else if (n == "early_exit") c.opt_early_exit = value;
-    else if (n == "unroll") c.opt_unroll = value;
     else if (n == "pull_grid") c.opt_pull_grid = value;
     else if (n == "diag_filter") c.opt_diag_filter = value;
     else if (n == "csr_push") c.opt_csr_push = value;
     else if (n == "fused_prep") c.opt_fused_prep = value;
-    else if (n == "l2_window") c.opt_l2_window = value;
-    else if (n == "small_split") c.opt_small_split = value;
     else if (n == "perm_push") c.opt_perm_push = value;
-    else if (n == "l2_reset") c.opt_l2_reset = value;
-    else if (n == "count_kernel") c.opt_count_kernel = value;
-    // retired: the materialise has a single fill kernel now; the names stay accepted so callers that set them keep working
-    else if (n == "fill_kernel" || n == "fill_cap") {}
+    // retired: the pull, the count pass and the fill have a single kernel each now, and there is no persisting-L2 window; the
+    // names stay accepted so callers that set them keep working
+    else if (n == "fill_kernel" || n == "fill_cap" || n == "pull_kernel" || n == "unroll" || n == "small_split" ||
+             n == "count_kernel" || n == "l2_window" || n == "l2_reset") {}
     else if (n == "bfs_direction") c.opt_bfs_direction = value;
     else if (n == "bfs_sparse_exchange") c.opt_bfs_sparse_exchange = value;
     else if (n == "timing") { c.opt_timing = value; if (c.ready) timed_reset(); }

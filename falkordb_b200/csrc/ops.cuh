@@ -18,55 +18,41 @@ void rmat_block_csr(int scale, u64 edge_factor, u64 seed, u64 lo, u64 hi, int by
 void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out);
 u64 spgemm_flops(const DevCSR &A, const DevCSR &B);
 
-struct LongRows;
+struct PullTables;
 // bits.cu : frontier bit-matrix path for short-fat left operands (<= 1024 rows)
 u32 bits_words_for(u64 nrows);
 void bits_from_csr(const DevCSR &F, DevBits &X);
 void bits_to_csr(const DevBits &X, DevCSR &C);
 u64 bits_nvals(const DevBits &X);
 // Y = F * A expanded straight from F's CSR (tiny frontiers); false = too much work for this path, nothing was done
-// lr (optional): A's pull tables; when they carry a vertex order the result is written in it (permuted form)
-bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const LongRows *lr = nullptr);
+// pt (optional): A's pull tables; when they carry a vertex order the result is written in it (permuted form)
+bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr);
 void bits_naturalise(DevBits &X);                                // permuted form -> natural vertex order (no-op when natural)
 bool csr_is_diagonal(const DevCSR &A);                          // square, every entry (i,i)
 void bits_diag(const DevBits &X, const DevCSR &A, DevBits &Y, u64 *flops_out);   // Y = X * A for diagonal A
 void bits_to_rowmajor(const DevBits &X, u64 *out, u64 wpr);   // out[row * wpr + (col >> 6)], every word written
 void csr_to_rowmajor(const DevCSR &A, u64 *out, u64 wpr);     // out must be zero on entry
-struct LongRows {   // per-matrix auxiliary data of the pull direction, cached with the transpose mirror
-    bool built = false;
-    // legacy 8-lane / merge-path kernels
-    DevBuf<u32> rows; u64 n = 0; u64 maxdeg = 0;      // rows of A' longer than LONG_ROW
-    DevBuf<u64> choff; u64 nchunks = 0;               // chunk table of those rows (prefix of ceil(len / LONG_CHUNK))
-    DevBuf<u64> mp_r;                                  // merge-path coordinates of every 256th diagonal
-    DevBuf<u32> m_row, m_len; DevBuf<u64> m_start; u64 nm = 0;   // mid rows (SMALL_ROW < len <= LONG_ROW), longest first
-    DevBuf<u32> jp;                                    // relabelled col_idx of A' (all rows)
-    // lane-split pull (pull_kernel = 5): mid rows and LONG_ROW-entry segments of long rows, longest first; bit 31 of s_len marks a
-    // segment of a long row (merged with RED.OR)
-    DevBuf<u32> s_row, s_len; DevBuf<u64> s_start; u64 ns = 0; bool seg_built = false;
-    // hot-set packing: vertices with out-edges, by out-degree descending
+struct PullTables {   // per-matrix tables of the pull direction, cached with the transpose mirror
+    // hot-set order: vertices with out-edges, by out-degree descending
     DevBuf<u32> vert, slot, hdeg; u64 n1 = 0; bool packed = false;   // hdeg[s] = out-degree of vert[s]
     // the same order extended to ALL vertices (sinks follow the n1 slots, by id): a frontier stored in it needs no packing pass
     std::shared_ptr<DevBuf<u32>> pvert, pperm; u64 perm_tag = 0;    // pvert[position] = vertex, pperm[vertex] = position
-    // CSR-stream form for the pull kernel: short rows of A' (cols relabelled to slots), window -> first row,
-    // and the long rows kept apart; built per frontier word count W
-    u32 sW = 0; u64 swin = 0; bool s_packed = false;
-    DevBuf<u64> rp_s; DevBuf<u32> jp_s, wstart; u64 nwin = 0, nnz_s = 0;
-    DevBuf<u32> lrows, jp_l; DevBuf<u64> lrp; u64 nlong = 0, maxlong = 0;
+    DevBuf<u32> jp;                                    // col_idx of A' relabelled to hot-set slots (when packed)
+    // segment list: rows of A' longer than SMALL_ROW -- whole rows up to LONG_ROW entries, LONG_ROW-entry segments of longer ones --
+    // longest first; bit 31 of s_len marks a segment of a long row (merged with RED.OR)
+    DevBuf<u32> s_row, s_len; DevBuf<u64> s_start; u64 ns = 0;
+    bool built = false;                                // the segment list is built
     void clear() {
-        s_row.release(); s_len.release(); s_start.release(); ns = 0; seg_built = false;
-        built = false; rows.release(); n = 0; maxdeg = 0; choff.release(); nchunks = 0; mp_r.release(); jp.release(); m_row.release(); m_len.release(); m_start.release(); nm = 0;
         vert.release(); slot.release(); hdeg.release(); n1 = 0; packed = false; pvert.reset(); pperm.reset(); perm_tag = 0;
-        sW = 0; swin = 0; s_packed = false; rp_s.release(); jp_s.release(); wstart.release(); nwin = 0; nnz_s = 0;
-        lrows.release(); jp_l.release(); lrp.release(); nlong = 0; maxlong = 0;
+        jp.release();
+        s_row.release(); s_len.release(); s_start.release(); ns = 0;
+        built = false;
     }
 };
-void build_hot_pack(const DevCSR &A, const DevCSR &AT, LongRows &lr);
-void build_stream(const DevCSR &AT, LongRows &lr, u32 W);
-void build_long_rows(const DevCSR &AT, LongRows &lr);
-// Y = X * A.  AT (= A') + its long-row list enable the pull direction; may be null (push only).
-void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, LongRows *lr, DevBits &Y, u64 *flops_out,
+// Y = X * A.  AT (= A') and its pull tables enable the pull direction; may be null (push only).
+void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y, u64 *flops_out,
               int *path_out);
-void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, LongRows &lr);
+void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt);   // square A: build the pull tables now
 void bits_andnot(DevBits &Y, const DevBits &M); // Y &= ~M
 void bits_or(DevBits &Y, const DevBits &Z);     // Y |= Z
 void bits_copy(const DevBits &X, DevBits &Y);

@@ -35,11 +35,6 @@ void ensure_init() {
     CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     c.num_sms = prop.multiProcessorCount;
     CUDA_TRY(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
-    // persisting-L2 limits for the frontier's hot prefix (bits.cu: set_l2_window).  The carve-out itself is NOT made here: it is
-    // taken from every other kernel's L2 (50 MB on an H100), so it is only set when the l2_window option asks for it, and sized
-    // to that window.
-    c.l2_persist_max = (u64)prop.persistingL2CacheMaxSize;
-    c.l2_window_max = (u64)prop.accessPolicyMaxWindowSize;
     c.ready = true;
 }
 
@@ -155,7 +150,7 @@ static double g_ms[TK_COUNT_];
 static u64 g_n[TK_COUNT_], g_bytes[TK_COUNT_];
 
 const char *timed_name(int id) {
-    static const char *names[] = {"bits_pull", "bits_pull_long", "bits_push", "heavy_accumulate", "small_rows", "bits_fill",
+    static const char *names[] = {"bits_pull", "bits_push", "heavy_accumulate", "small_rows", "bits_fill",
                                   "bits_count", "bitmap_expand", "bfs_expand", "union", "filter", "mxv_fp64", "spgemm_masked", "transpose"};
     return (id >= 0 && id < TK_COUNT_) ? names[id] : "?";
 }

@@ -363,7 +363,7 @@ uint64_t B200_get_stat(const char *name);
 void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
- * "bits_pull", "bits_pull_long", "bits_push", "heavy_accumulate", "bits_fill", "bits_count".  0 on success. */
+ * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */

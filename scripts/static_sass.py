@@ -13,7 +13,7 @@ SO = os.path.join(ROOT, "falkordb_b200", "libb200grb.so")
 # demangled-name prefixes of the instantiations the 512-source chain (W = 8), the BFS engine and the side kernels launch
 WANT = [
     ("hop, pull (mid + long-row segments), W = 8", r"k_pull_seg<8, false, 4, false>"),
-    ("hop, pull (rows <= 8), W = 8", r"k_pull_small<8, false, 1>"),
+    ("hop, pull (rows <= 8), W = 8", r"k_pull_small<8, false>"),
     ("hop 2, CSR push", r"k_csr_push<8"),
     ("frontier totals in gather order", r"k_ordered_flops<8>"),
     ("materialise, count (carry-save)", r"k_bits_count_csa<8>"),

@@ -223,19 +223,20 @@ def test_mxm_chain_bit_frontier_matches_oracle(nsrc, pull):
     assert list(F.iter(0, 0)) == [(0, int(c)) for c in want.j[want.p[0]:want.p[1]]]
 
 
-@pytest.mark.parametrize("opts", [{"fill_cap": 64}, {"hot_pack": 0}, {"pull_kernel": 0, "hot_pack": 0}, {"pull_kernel": 0, "unroll": 1},
-                                  {"pull_kernel": 1}, {"pull_kernel": 0, "hints": 0, "unroll": 2}, {"pull_kernel": 2}, {"early_exit": 0}, {"early_exit": 2},
-                                  {"pull_kernel": 3}, {"pull_kernel": 3, "early_exit": 2, "unroll": 2}, {"pull_kernel": 3, "early_exit": 0, "hints": 0},
-                                  {"pull_kernel": 3, "pull_grid": 1}, {"pull_kernel": 0, "pull_grid": 16}, {"fill_kernel": 0}, {"fill_kernel": 2}, {"fill_kernel": 1}, {"fill_kernel": 3},
-                                  {"pull_kernel": 4}, {"pull_kernel": 4, "hints": 0, "early_exit": 0}, {"pull_kernel": 4, "early_exit": 2, "pull_grid": 2},
-                                  {"pull_kernel": 4, "hot_pack": 0}, {"fused_prep": 0}, {"fused_prep": 0, "early_exit": 2}, {"fused_prep": 1, "early_exit": 2},
-                                  {"fused_prep": 1, "pull_kernel": 3}, {"fused_prep": 1, "pull_kernel": 1},
-                                  {"pull_kernel": 5}, {"pull_kernel": 5, "early_exit": 2}, {"pull_kernel": 5, "early_exit": 0, "hints": 0}, {"pull_kernel": 5, "hints": 1},
-                                  {"pull_kernel": 5, "unroll": 8, "early_exit": 2}, {"pull_kernel": 5, "unroll": 2, "hot_pack": 0},
-                                  {"pull_kernel": 5, "l2_window": 1 << 20}, {"pull_kernel": 5, "l2_window": 1 << 30, "l2_reset": 1},
-                                  {"count_kernel": 0}, {"count_kernel": 1}, {"pull_kernel": 5, "small_split": 1}])
+# names that no longer select anything; setting them all at once must leave every result bit-exact
+RETIRED_OPTIONS = {"pull_kernel": 0, "unroll": 8, "small_split": 1, "count_kernel": 0, "l2_window": 1 << 20, "l2_reset": 1,
+                   "fill_kernel": 0, "fill_cap": 64}
+# every combination of the pull's switches -- hot-set order and the fused prep pass on / off, L2 hints and early exit at each of
+# their settings (both template branches of k_pull_small / k_pull_seg) -- then the CTA-count override, then the retired names
+PULL_OPTION_SETS = ([{"hot_pack": hp, "fused_prep": fp, "hints": h, "early_exit": ee}
+                     for hp in (1, 0) for fp in (1, 0) for h in (-1, 0, 1) for ee in (1, 0, 2)]
+                    + [{"pull_grid": g} for g in (1, 2, 16)] + [RETIRED_OPTIONS])
+
+
+@pytest.mark.parametrize("opts", PULL_OPTION_SETS)
 def test_bit_frontier_kernel_variants(opts):
-    """every selectable kernel variant (direct-write materialise, hot-set packing on/off, merge-path pull, L2 hints)"""
+    """every combination of the pull's options (hot-set packing, fused prep, L2 hints, early exit), the grid size override and
+    the retired kernel-selection names, which must change nothing"""
     fb.set_option("bits_mode", 1)
     fb.set_option("pull_mode", 1)
     for k, v in opts.items():
@@ -255,8 +256,7 @@ def test_bit_frontier_kernel_variants(opts):
             F.wait()
             assert_same(F, want, f"variant {opts} nsrc={nsrc}")
     finally:
-        for k, v in (("fill_cap", 0), ("hot_pack", 1), ("unroll", 4), ("pull_kernel", 5), ("hints", -1), ("early_exit", 1), ("pull_grid", 0), ("fill_kernel", 3), ("fused_prep", 1),
-                     ("l2_window", 0), ("l2_reset", 0), ("count_kernel", 1), ("small_split", 0)):
+        for k, v in (("hot_pack", 1), ("hints", -1), ("early_exit", 1), ("pull_grid", 0), ("fused_prep", 1)):
             fb.set_option(k, v)
 
 
@@ -554,13 +554,13 @@ def test_row_iterator_walks_dense_chain_result_from_bitmap(materialise_first):
     assert_same(F, want, "after iterating")
 
 
-@pytest.mark.parametrize("opts", [{"pull_kernel": 4}, {"pull_kernel": 4, "early_exit": 2}, {"pull_kernel": 4, "early_exit": 0, "hot_pack": 0},
-                                  {"pull_kernel": 3}, {"pull_kernel": 0, "early_exit": 2}, {"pull_kernel": 1},
-                                  {"pull_kernel": 5}, {"pull_kernel": 5, "early_exit": 2}, {"pull_kernel": 5, "early_exit": 0, "hot_pack": 0},
-                                  {"pull_kernel": 5, "unroll": 8}, {"pull_kernel": 5, "l2_window": 4 << 20}, {"pull_kernel": 5, "small_split": 1}])
+# early exit at each setting x hot-set order on / off x occupancy grid or one CTA per SM (fewer 8-lane groups, so each deals
+# more list entries and more long-row segments), then the retired names
+@pytest.mark.parametrize("opts", [{"early_exit": ee, "hot_pack": hp, "pull_grid": g} for ee in (1, 2, 0) for hp in (1, 0) for g in (0, 1)]
+                         + [RETIRED_OPTIONS])
 def test_pull_bins_small_mid_long_rows(opts):
     """a graph whose transpose has empty, small (<= 8), mid and long (> 4096 entries) rows, so every bin of the
-    degree-binned pull (and the long-row chunk table) is exercised; W = 1, 8 and 16 word columns"""
+    degree-binned pull (small rows, whole mid rows, segments of long rows) is exercised; W = 1, 8 and 16 word columns"""
     rng = np.random.default_rng(2024)
     n = 20000
     src, dst = [], []
@@ -590,11 +590,11 @@ def test_pull_bins_small_mid_long_rows(opts):
             for _ in range(3):
                 F.lmxm(dA)
                 want = orc.mxm(want, A)
-            assert fb.get_stat("last_path") in (3, 4), "the pull direction was not taken"
+            assert fb.get_stat("last_path") == 3, "the pull direction was not taken"
             F.wait()
             assert_same(F, want, f"binned pull {opts} nsrc={nsrc}")
     finally:
-        for k, v in (("hot_pack", 1), ("pull_kernel", 5), ("early_exit", 1), ("pull_mode", -1), ("bits_mode", -1), ("unroll", 4), ("l2_window", 0), ("small_split", 0)):
+        for k, v in (("hot_pack", 1), ("early_exit", 1), ("pull_grid", 0), ("pull_mode", -1), ("bits_mode", -1)):
             fb.set_option(k, v)
 
 
