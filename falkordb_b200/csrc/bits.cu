@@ -562,7 +562,8 @@ __global__ void k_csr_entry_info(const u64 *__restrict__ Fp, const u32 *__restri
         edeg[q] = Ap[k + 1] - Ap[k];
     }
 }
-template <int W>
+// ANDNOT (the dirty hop's deleted-edge term, bits_apply_deltas) clears bit i instead of setting it
+template <int W, bool ANDNOT>
 __global__ void __launch_bounds__(256)
 k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *__restrict__ cum, u64 nent, u64 total,
            const u64 *__restrict__ Ap, const u32 *__restrict__ Aj, u64 *__restrict__ Y, const u32 *__restrict__ perm) {
@@ -584,7 +585,9 @@ k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *
             const u32 i = erow[e];
             u32 col = Aj[Ap[Fj[e]] + (t - cum[e])];
             if (perm) col = __ldg(perm + col);          // hot-set order: hubs of the next gather become neighbours (64 MB table, L2)
-            atomicOr((unsigned long long *)&Y[(u64)col * W + (i >> 6)], 1ULL << (i & 63));
+            unsigned long long *dst = (unsigned long long *)&Y[(u64)col * W + (i >> 6)];
+            if (ANDNOT) atomicAnd(dst, ~(1ULL << (i & 63)));
+            else atomicOr(dst, 1ULL << (i & 63));
         }
     }
 }
@@ -592,7 +595,7 @@ template <int W>
 static void csr_push_impl(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 flops, const u32 *erow, const u64 *cum, const u32 *perm) {
     u64 nchunks = (flops + PUSH_CHUNK - 1) / PUSH_CHUNK;
     TimedScope ts(TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops);
-    LAUNCH((k_csr_push<W>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, A.j.ptr, Y.w.ptr, perm);
+    LAUNCH((k_csr_push<W, false>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, A.j.ptr, Y.w.ptr, perm);
 }
 // Y = F * A from the CSR form of F.  Returns false (nothing done) when the expansion is large enough that the
 // direction-optimising bit-matrix hop should take it: flops * 4 > nnz(A), the same switch bits_hop applies to edges.
@@ -619,6 +622,7 @@ bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops
     if (pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
         perm = pt->pperm->ptr;
         Y.pvert = pt->pvert;
+        Y.pperm = pt->pperm;
         Y.perm_tag = pt->perm_tag;
     }
     if (flops == 0) return true;
@@ -645,6 +649,7 @@ void bits_naturalise(DevBits &X) {
     if (n) LAUNCH(k_unpermute, grid_for(n * X.W, 256, (u64)ctx().num_sms * 32), 256, 0, X.w.ptr, X.pvert->ptr, n, X.W, out.ptr);
     X.w = std::move(out);
     X.pvert.reset();
+    X.pperm.reset();
     X.perm_tag = 0;
 }
 static void require_natural(const DevBits &X, const char *what) {
@@ -1275,7 +1280,123 @@ void bits_copy(const DevBits &X, DevBits &Y) {
     Y.nrows = X.nrows; Y.ncols = X.ncols; Y.W = X.W;
     Y.w.alloc(X.ncols * X.W);
     d2d(Y.w.ptr, X.w.ptr, X.ncols * X.W);
-    Y.pvert = X.pvert; Y.perm_tag = X.perm_tag;       // a copy keeps the vertex order of its source
+    Y.pvert = X.pvert; Y.pperm = X.pperm; Y.perm_tag = X.perm_tag;       // a copy keeps the vertex order of its source
+}
+
+// ---------------------------------------------------------------------------- pending deltas (delta_lmxm in one pass)
+// A dirty hop is F <- (F*m AND NOT F*dm) OR F*dp (matrix.rs:1317-1402, with the reference's over-masking: (i, j) is dropped
+// whenever any deleted edge reaches j from row i).  With Y = F*m already computed, the two delta terms need only the deltas'
+// entries: for each (k, j) of dm, Y[j] &= ~X[k]; then for each (k, j) of dp, Y[j] |= X[k].  The passes run in stream order,
+// every AND-NOT before any OR, which is the phase separation the formula needs.  Work is O(W * nnz(delta)): no pass over the n
+// vertices and no product bit-matrix.  X and Y are addressed through the order they are stored in (pperm: vertex ->
+// position), so a frontier in hot-set order keeps that order across a dirty hop.
+enum { DELTA_ANDNOT = 0, DELTA_OR = 1 };
+// delta entries per CTA.  A small delta is spread over n rows, so every entry's row is a binary search over the whole row
+// pointer array (about log2(n) dependent loads): short chunks keep that latency chain per CTA short (1 to 8 searches).
+static const u64 DELTA_CHUNK = 256;
+
+// The delta's entries in chunks of DELTA_CHUNK per CTA; each entry is handled by SPLIT lanes (the pull's 16-byte record parts),
+// which gather their part of X[pos(k)] and reduce it into Y[pos(j)] with RED.AND / RED.OR.  The row k of an entry comes from a
+// binary search over the delta's row pointers inside the CTA's row range.  flops += popcount(X[k]) per entry.
+template <int W, int OP>
+__global__ void __launch_bounds__(256)
+k_bits_delta(const u64 *__restrict__ Dp, const u32 *__restrict__ Dj, u64 nrows, u64 nnz, const u64 *__restrict__ X,
+             const u32 *__restrict__ xperm, u64 *__restrict__ Y, const u32 *__restrict__ yperm, u64 *__restrict__ flops) {
+    constexpr int WL = PullCfg<W>::WL, SPLIT = PullCfg<W>::SPLIT;
+    constexpr u32 EPS = 256 / SPLIT;                 // entries per CTA step
+    typedef cub::BlockReduce<u64, 256> Red;
+    __shared__ typename Red::TempStorage ts;
+    __shared__ u64 s_r0, s_r1;
+    const u64 lo = (u64)blockIdx.x * DELTA_CHUNK;
+    const u64 hi = lo + DELTA_CHUNK < nnz ? lo + DELTA_CHUNK : nnz;
+    if (threadIdx.x == 0) s_r0 = find_le64(Dp, 0, nrows - 1, lo);          // the two bounds are independent searches
+    if (threadIdx.x == 32) s_r1 = find_le64(Dp, 0, nrows - 1, hi - 1);
+    __syncthreads();
+    const u64 r1 = s_r1;
+    u64 k = s_r0;
+    const u32 h = threadIdx.x % SPLIT;
+    u64 fl = 0;
+    for (u64 q = lo + threadIdx.x / SPLIT; q < hi; q += EPS) {
+        k = find_le64(Dp, k, r1, q);                 // entries only move forward: the previous row bounds the search
+        const u64 j = __ldg(Dj + q);
+        const u64 px = xperm ? __ldg(xperm + k) : k, py = yperm ? __ldg(yperm + j) : j;
+        u64 x[WL];
+        ld_part<WL>(x, X + px * W + h * WL);
+        unsigned long long *dst = reinterpret_cast<unsigned long long *>(Y + py * W + h * WL);
+#pragma unroll
+        for (int w = 0; w < WL; w++) {
+            if (!x[w]) continue;
+            fl += __popcll(x[w]);
+            if (OP == DELTA_OR) atomicOr(dst + w, x[w]);
+            else atomicAnd(dst + w, ~x[w]);
+        }
+    }
+    const u64 tot = Red(ts).Sum(fl);
+    if (threadIdx.x == 0 && tot) atomicAdd((unsigned long long *)flops, tot);
+}
+
+template <int W>
+static void bits_delta_impl(const DevBits &X, const DevCSR &D, int op, DevBits &Y, u64 *fl) {
+    const u32 *xperm = X.permuted() ? X.pperm->ptr : nullptr, *yperm = Y.permuted() ? Y.pperm->ptr : nullptr;
+    const u32 grid = (u32)((D.nnz + DELTA_CHUNK - 1) / DELTA_CHUNK);
+    // delta entries (8-byte row pointer share + 4-byte column), the gathered records, the reduced words
+    TimedScope ts(TK_BITS_DELTA, 12 * D.nnz + 16ULL * W * D.nnz);
+    if (op == DELTA_OR) LAUNCH((k_bits_delta<W, DELTA_OR>), grid, 256, 0, D.p.ptr, D.j.ptr, D.nrows, D.nnz, X.w.ptr, xperm, Y.w.ptr, yperm, fl);
+    else LAUNCH((k_bits_delta<W, DELTA_ANDNOT>), grid, 256, 0, D.p.ptr, D.j.ptr, D.nrows, D.nnz, X.w.ptr, xperm, Y.w.ptr, yperm, fl);
+}
+
+// The first hop: F is still a CSR of <= 1024 rows and Y came from bits_push_from_csr.  Entry (i, k) of F walks delta row k and
+// applies bit i to Y[pos(j)] -- k_csr_push with the delta as its operand.  Returns flops(F * D).
+template <int W>
+static u64 csr_delta_impl(const DevCSR &F, const DevCSR &D, int op, DevBits &Y) {
+    if (!F.nnz || !D.nnz) return 0;
+    DevBuf<u32> erow(F.nnz);
+    DevBuf<u64> cum(F.nnz + 1);
+    LAUNCH(k_csr_entry_info, grid_for(F.nrows * 32, 256), 256, 0, F.p.ptr, F.j.ptr, F.nrows, D.p.ptr, erow.ptr, cum.ptr);
+    CUDA_TRY(cudaMemsetAsync(cum.ptr + F.nnz, 0, sizeof(u64), stream()));
+    exclusive_scan_u64(cum.ptr, cum.ptr, F.nnz + 1);
+    const u64 flops = read_scalar(cum.ptr + F.nnz);
+    if (!flops) return 0;
+    const u32 *yperm = Y.permuted() ? Y.pperm->ptr : nullptr;
+    const u32 grid = (u32)((flops + PUSH_CHUNK - 1) / PUSH_CHUNK);
+    TimedScope ts(TK_BITS_DELTA, 4 * flops + 16 * F.nnz + 8 * flops);
+    if (op == DELTA_OR) LAUNCH((k_csr_push<W, false>), grid, 256, 0, erow.ptr, F.j.ptr, cum.ptr, F.nnz, flops, D.p.ptr, D.j.ptr, Y.w.ptr, yperm);
+    else LAUNCH((k_csr_push<W, true>), grid, 256, 0, erow.ptr, F.j.ptr, cum.ptr, F.nnz, flops, D.p.ptr, D.j.ptr, Y.w.ptr, yperm);
+    return flops;
+}
+
+template <int W>
+static u64 apply_deltas_impl(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y) {
+    u64 flops = 0;
+    DevBuf<u64> fl;
+    const DevCSR *ds[2] = {dm, dp};
+    const int ops[2] = {DELTA_ANDNOT, DELTA_OR};
+    for (int t = 0; t < 2; t++) {
+        const DevCSR *D = ds[t];
+        if (!D || !D->nnz) continue;
+        if (Xc) { flops += csr_delta_impl<W>(*Xc, *D, ops[t], Y); continue; }
+        if (!fl.ptr) { fl.alloc(1); fl.zero(); }
+        bits_delta_impl<W>(*Xb, *D, ops[t], Y, fl.ptr);
+    }
+    if (fl.ptr) flops += read_scalar(fl.ptr);
+    return flops;
+}
+
+u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y) {
+    const u64 inner = Xc ? Xc->ncols : Xb->ncols;
+    for (const DevCSR *D : {dm, dp})
+        if (D && (D->nrows != inner || D->ncols != Y.ncols)) throw GrbError(-6, "delta_lmxm: delta dimensions differ from the operand");
+    if (!Xc && Xb->W != Y.W) throw GrbError(-101, "delta_lmxm: frontier and product word counts differ");
+    if ((Y.permuted() && !Y.pperm) || (Xb && Xb->permuted() && !Xb->pperm))
+        throw GrbError(-101, "delta_lmxm: permuted frontier without its vertex -> position table");
+    switch (Y.W) {
+    case 1: return apply_deltas_impl<1>(Xb, Xc, dm, dp, Y);
+    case 2: return apply_deltas_impl<2>(Xb, Xc, dm, dp, Y);
+    case 4: return apply_deltas_impl<4>(Xb, Xc, dm, dp, Y);
+    case 8: return apply_deltas_impl<8>(Xb, Xc, dm, dp, Y);
+    case 16: return apply_deltas_impl<16>(Xb, Xc, dm, dp, Y);
+    default: throw GrbError(-8, "bit-frontier: unsupported word count");
+    }
 }
 
 } // namespace b200

@@ -72,7 +72,7 @@ inline cudaStream_t stream() { return ctx().stream; }
 
 // ---- optional per-kernel timing (CUDA events on the launch stream; B200_set_option("timing",1)) ----
 enum TimedId { TK_BITS_PULL = 0, TK_BITS_PUSH, TK_HEAVY_ACC, TK_SMALL_ROWS, TK_BITS_FILL, TK_BITS_COUNT,
-               TK_BITMAP_EXPAND, TK_BFS_EXPAND, TK_UNION, TK_FILTER, TK_MXV, TK_MASKED, TK_TRANSPOSE, TK_COUNT_ };
+               TK_BITMAP_EXPAND, TK_BFS_EXPAND, TK_UNION, TK_FILTER, TK_MXV, TK_MASKED, TK_TRANSPOSE, TK_BITS_DELTA, TK_COUNT_ };
 const char *timed_name(int id);
 void timed_begin(int id);
 void timed_end(int id, u64 algorithmic_bytes) noexcept;
@@ -191,11 +191,12 @@ struct DevBits {
     // Permuted form (bits.cu, "hot-set order"): the words of vertex v live at position pos(v) instead of v, pos = the degree-sorted
     // gather order of the matrix this frontier is about to be multiplied by (PullTables::pperm), so the pull of the next hop gathers
     // straight from it with no packing pass.  pvert[position] = vertex undoes it; perm_tag names the permutation (0 = natural).
-    std::shared_ptr<DevBuf<u32>> pvert;
+    // pperm[vertex] = position addresses single vertices in place (the delta terms of a dirty hop).
+    std::shared_ptr<DevBuf<u32>> pvert, pperm;
     u64 perm_tag = 0;
     bool valid() const { return w.ptr != nullptr; }
     bool permuted() const { return perm_tag != 0; }
-    void clear() { w.release(); W = 0; pvert.reset(); perm_tag = 0; }
+    void clear() { w.release(); W = 0; pvert.reset(); pperm.reset(); perm_tag = 0; }
 };
 
 // ---- L2 residency hints (createpolicy descriptors; sm_80+) ---------------------------------------

@@ -1025,6 +1025,56 @@ static bool bits_legal(GrB_Matrix C, GrB_Matrix M, GrB_Matrix A, GrB_Matrix B, c
     return true;
 }
 
+// The frontier bit-matrix path of GrB_mxm (short-fat A, CondTraverse's F*A): C<!M, RSC> = A*B kept in device frontier form.
+// Returns false when the path does not apply (not legal, switched off, or the automatic choice prefers the general row-wise
+// path); C is then unchanged.  dm / dp (B200_Matrix_delta_lmxm): device-resident deltas of B whose terms are applied to the
+// product before it replaces C, while A's frontier is still intact: C = (A*B AND NOT A*dm) OR A*dp.
+static bool frontier_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_Matrix A, GrB_Matrix B, const Desc &d, bool accum,
+                         const DevCSR *dm = nullptr, const DevCSR *dp = nullptr) {
+    Context &cx = ctx();
+    if (accum || d.t0 || d.t1 || cx.opt_bits_mode == 0 || !bits_legal(C, Mask, A, B, d)) return false;
+    bool use_bits = (cx.opt_bits_mode == 1);
+    u64 known_flops = ~0ULL;
+    finish_pending(A);
+    if (!use_bits) {
+        if (A->bits_valid && !A->dev_valid && !A->host_valid) use_bits = true; // stay in frontier form mid-chain
+        else {
+            ensure_dev(A); ensure_dev(B);
+            u64 fl = spgemm_flops(A->dev, B->dev);
+            known_flops = fl;
+            use_bits = fl >= (u64)cx.opt_bits_min_flops;
+        }
+    }
+    if (!use_bits) return false;
+    ensure_dev(B);
+    if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
+    DevBits Y;
+    u64 fl = 0;
+    int path = 0;
+    // a frontier that is still a (small) CSR expands straight from its entries; large expansions decline
+    // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
+    const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
+                          A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
+                          !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, &fl, (B->devT_valid && !Mask) ? &B->pt : (const PullTables *)nullptr);
+    if (from_csr) path = 7;
+    else if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
+    if (from_csr) {}
+    else if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, &fl); path = 5; }
+    else {
+        if (cx.opt_pull_mode != 0) ensure_devT(B);
+        bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, &fl, &path);
+    }
+    if (Mask) {
+        ensure_bits(Mask);
+        bits_andnot(Y, Mask->bits);
+    }
+    if (dm || dp) fl += bits_apply_deltas(from_csr ? nullptr : &A->bits, from_csr ? &A->dev : nullptr, dm, dp, Y);
+    cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
+    set_bits(C, std::move(Y));
+    if (cx.opt_sync_after_op) sync_stream();
+    return true;
+}
+
 GrB_Info GrB_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_BinaryOp accum, GrB_Semiring semiring, GrB_Matrix A, GrB_Matrix B,
                  GrB_Descriptor desc) {
     CHECK_MAT(C); CHECK_MAT(A); CHECK_MAT(B); CHECK_PTR(semiring);
@@ -1043,48 +1093,7 @@ GrB_Info GrB_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_BinaryOp accum, GrB_Semiring
         check_mask_dims(C, Mask);
 
         // ---- frontier bit-matrix path (short-fat A, CondTraverse's F*A) ----
-        if (!accum && !d.t0 && !d.t1 && cx.opt_bits_mode != 0 && bits_legal(C, Mask, A, B, d)) {
-            bool use_bits = (cx.opt_bits_mode == 1);
-            u64 known_flops = ~0ULL;
-            finish_pending(A);
-            if (!use_bits) {
-                if (A->bits_valid && !A->dev_valid && !A->host_valid) use_bits = true; // stay in frontier form mid-chain
-                else {
-                    ensure_dev(A); ensure_dev(B);
-                    u64 fl = spgemm_flops(A->dev, B->dev);
-                    known_flops = fl;
-                    use_bits = fl >= (u64)cx.opt_bits_min_flops;
-                }
-            }
-            if (use_bits) {
-                ensure_dev(B);
-                if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
-                DevBits Y;
-                u64 fl = 0;
-                int path = 0;
-                // a frontier that is still a (small) CSR expands straight from its entries; large expansions decline
-                // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
-                const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
-                                      A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
-                                      !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, &fl, (B->devT_valid && !Mask) ? &B->pt : (const PullTables *)nullptr);
-                if (from_csr) path = 7;
-                else if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
-                if (from_csr) {}
-                else if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, &fl); path = 5; }
-                else {
-                    if (cx.opt_pull_mode != 0) ensure_devT(B);
-                    bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, &fl, &path);
-                }
-                if (Mask) {
-                    ensure_bits(Mask);
-                    bits_andnot(Y, Mask->bits);
-                }
-                cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
-                set_bits(C, std::move(Y));
-                if (cx.opt_sync_after_op) sync_stream();
-                return GrB_SUCCESS;
-            }
-        }
+        if (frontier_mxm(C, Mask, A, B, d, accum != nullptr)) return GrB_SUCCESS;
 
         // ---- general row-wise path ----
         ensure_dev(A); ensure_dev(B);
@@ -2291,6 +2300,65 @@ GrB_Info B200_bfs_dist_parents(GrB_Matrix ATlocal, uint64_t row_lo, const int32_
     });
 }
 
+// ---- delta_lmxm as ONE C call (matrix.rs:1317-1402): F <- (F*m AND NOT F*dm) OR F*dp over GxB_ANY_PAIR_BOOL ----
+// The reference composes three GrB_mxm calls and an eWiseAdd, each of which builds or rewrites a whole |F| x n bit-matrix.  In
+// frontier form only the deltas' entries are touched here: F*m runs through GrB_mxm's frontier path unchanged, then the dm and dp
+// terms are applied to the product in place (bits_apply_deltas) before it replaces F.  Where the frontier path does not apply
+// (bits_mode 0, more than 1024 rows, or the automatic choice takes the general row-wise path) the three-call composition runs.
+// last_flops = flops(F*m) + flops(F*dp) + flops(F*dm), as the composition reports them.
+static GrB_Info delta_compose(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_Matrix dm) {
+    GrB_Index np = 0, nm = 0;
+    GrB_Info info = GrB_SUCCESS;
+    if (dp) info = GrB_Matrix_nvals(&np, dp);
+    if (!info && dm) info = GrB_Matrix_nvals(&nm, dm);
+    if (info) return info;
+    if (!np && !nm) return GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, m, nullptr);
+    GrB_Matrix mk = nullptr, ac = nullptr;
+    u64 flops = 0;
+    auto product = [&](GrB_Matrix *out, GrB_Matrix D) {        // *out = F * D, dropped when empty
+        GrB_Index nv = 0;
+        GrB_Info e = GrB_Matrix_new(out, GrB_BOOL, F->nrows, m->ncols);
+        if (!e) e = GrB_mxm(*out, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, D, nullptr);
+        if (!e) { flops += ctx().last_flops.load(); e = GrB_Matrix_nvals(&nv, *out); }
+        if (!e && !nv) GrB_Matrix_free(out);
+        return e;
+    };
+    if (nm) info = product(&mk, dm);
+    if (!info && np) info = product(&ac, dp);
+    if (!info) info = GrB_mxm(F, mk, nullptr, GxB_ANY_PAIR_BOOL, F, m, mk ? GrB_DESC_RSC : nullptr);
+    if (!info) flops += ctx().last_flops.load();
+    if (!info && ac) info = GrB_Matrix_eWiseAdd_BinaryOp(F, nullptr, nullptr, GxB_ANY_BOOL, F, ac, nullptr);
+    GrB_Matrix_free(&mk);
+    GrB_Matrix_free(&ac);
+    if (!info) ctx().last_flops = flops;
+    return info;
+}
+
+GrB_Info B200_Matrix_delta_lmxm(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_Matrix dm) {
+    CHECK_MAT(F); CHECK_MAT(m);
+    if (dp) CHECK_MAT(dp);
+    if (dm) CHECK_MAT(dm);
+    if (F->ncols != m->nrows || F->ncols != m->ncols) { tl_error = "delta_lmxm: F * m does not fit F"; return GrB_DIMENSION_MISMATCH; }
+    for (GrB_Matrix D : {dp, dm})
+        if (D && (D->nrows != m->nrows || D->ncols != m->ncols)) { tl_error = "delta_lmxm: delta dimensions differ from m"; return GrB_DIMENSION_MISMATCH; }
+    if (!dp && !dm) return GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, m, nullptr);
+    bool done = false;
+    GrB_Info info = guarded([&]() {
+        GpuLock g;
+        MultiLock lk{F, m, dp, dm};
+        for (GrB_Matrix X : {F, m, dp, dm})
+            if (is_huge(X)) throw GrbError(GrB_NOT_IMPLEMENTED, "delta_lmxm: host-resident matrix");
+        ensure_init();
+        const DevCSR *ddm = nullptr, *ddp = nullptr;
+        if (dm) { ensure_dev(dm); if (dm->dev.nnz) ddm = &dm->dev; }      // pending tuples finish first (dm.wait())
+        if (dp) { ensure_dev(dp); if (dp->dev.nnz) ddp = &dp->dev; }
+        done = frontier_mxm(F, nullptr, F, m, Desc(), false, ddm, ddp);
+        return GrB_SUCCESS;
+    });
+    if (info || done) return info;
+    return delta_compose(F, m, dp, dm);
+}
+
 // ---- the coalesced traversal as ONE C call (SURVEY 8f-1: CondTraverseOp's batch coalescing, cond_traverse.rs:600-608, 1264-1285) ----
 // F(i, sources[i]) = 1;  F <- F * hops[0] * ... * hops[nhops-1] over GxB_ANY_PAIR_BOOL;  result rows to HOST memory.
 //   B200_OUT_BITMAP : out_bits[row * words_per_row + (col >> 6)], one bit per slot.  The batch is processed in 128-row slices and
@@ -2301,13 +2369,18 @@ GrB_Info B200_bfs_dist_parents(GrB_Matrix ATlocal, uint64_t row_lo, const int32_
 //   B200_OUT_AUTO   : bitmap when the result holds more than one entry per 32 slots (fewer bytes over PCIe), else CSR; the choice
 //                     is reported in *format_out.  Needs both output buffers.
 // Composed from the public entry points (each takes the submission lock for its own duration), so other threads' calls interleave.
-GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, int nhops, int format,
-                             uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
-                             uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
+// Hop h is B200_Matrix_delta_lmxm(F, hops[h], dp[h], dm[h]); dp / dm NULL (B200_traverse_batch) or holding NULL entries: clean hops.
+static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, const GrB_Matrix *dp,
+                              const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p,
+                              uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
     CHECK_PTR(hops);
     if (nsrc) CHECK_PTR(sources);
     if (nhops < 1) { tl_error = "traverse_batch: nhops < 1"; return GrB_INVALID_VALUE; }
-    for (int h = 0; h < nhops; h++) CHECK_MAT(hops[h]);
+    for (int h = 0; h < nhops; h++) {
+        CHECK_MAT(hops[h]);
+        if (dp && dp[h]) CHECK_MAT(dp[h]);
+        if (dm && dm[h]) CHECK_MAT(dm[h]);
+    }
     if (format != B200_OUT_BITMAP && format != B200_OUT_CSR && format != B200_OUT_AUTO) { tl_error = "traverse_batch: unknown format"; return GrB_INVALID_VALUE; }
     if ((format != B200_OUT_CSR && !out_bits) || (format != B200_OUT_BITMAP && (!out_p || (!out_j && out_j_capacity)))) {
         tl_error = "traverse_batch: output buffer missing for the requested format"; return GrB_NULL_POINTER;
@@ -2327,7 +2400,7 @@ GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB
         for (u64 i = 0; i < r1 - r0; i++) rows[i] = i;
         GrB_Info e = GxB_Matrix_build_Scalar(F, rows.data(), sources + r0, one, r1 - r0);
         for (int h = 0; h < nhops && !e; h++) {
-            e = GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, hops[h], nullptr);
+            e = B200_Matrix_delta_lmxm(F, hops[h], dp ? dp[h] : nullptr, dm ? dm[h] : nullptr);
             if (!e) flops += ctx().last_flops.load();
             if (!e && h + 1 < nhops && F->ncols != hops[h + 1]->nrows) { tl_error = "traverse_batch: hop dimensions do not chain"; e = GrB_DIMENSION_MISMATCH; }
         }
@@ -2339,8 +2412,11 @@ GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB
     };
     // GrB_mxm(C = F, A = F, B) needs C's dimensions to match the product: a chain over square n x n operands (what the reference
     // stores, graph.rs:1191, 1211) keeps them; rectangular chains are rejected up front
-    for (int h = 0; h < nhops; h++)
+    for (int h = 0; h < nhops; h++) {
         if (hops[h]->nrows != inner || hops[h]->ncols != inner) { GrB_Scalar_free(&one); tl_error = "traverse_batch: operands must be square and equally sized"; return GrB_DIMENSION_MISMATCH; }
+        for (GrB_Matrix D : {dp ? dp[h] : nullptr, dm ? dm[h] : nullptr})
+            if (D && (D->nrows != inner || D->ncols != inner)) { GrB_Scalar_free(&one); tl_error = "traverse_batch: delta dimensions differ from the hop's"; return GrB_DIMENSION_MISMATCH; }
+    }
     if (format == B200_OUT_AUTO || format == B200_OUT_CSR) {
         // density is known only after the hops: run the whole batch once, then pick the hand-off
         GrB_Matrix F = nullptr;
@@ -2377,6 +2453,22 @@ GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB
     if (flops_out) *flops_out = flops;
     if (format_out) *format_out = chosen;
     return info;
+}
+
+GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, int nhops, int format,
+                             uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
+                             uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
+    return traverse_impl(sources, nsrc, hops, nullptr, nullptr, nhops, format, out_bits, words_per_row, out_p, out_j, out_j_capacity,
+                         nvals_out, flops_out, format_out);
+}
+
+// The same traversal over operands with pending writes: hop h is (m[h], dp[h], dm[h]) through B200_Matrix_delta_lmxm.
+GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
+                                   const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row,
+                                   uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out,
+                                   int *format_out) {
+    return traverse_impl(sources, nsrc, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j, out_j_capacity, nvals_out,
+                         flops_out, format_out);
 }
 
 // ---- multi-source reachability as ONE C call (SURVEY 8f-1: the multiplicity-insensitive core of CondVarLenTraverse with

@@ -32,14 +32,42 @@ struct TraversalMatrix {
         if (vm) f.delta_lmxm(vm->m(), vm->dp(), vm->dm());
         else f.delta_lmxm(t->fwd_m(), t->fwd_dp(), t->fwd_dm());
     }
+    // the (m, dp, dm) handles delta_lmxm_into multiplies by, for B200_traverse_batch_delta
+    void operands(GrB_Matrix *m, GrB_Matrix *dp, GrB_Matrix *dm) const {
+        if (vm) { vm->dp().wait(); vm->dm().wait(); *m = vm->m().inner(); *dp = vm->dp().inner(); *dm = vm->dm().inner(); }
+        else { t->fwd_dp().wait(); t->fwd_dm().wait(); *m = t->fwd_m().inner(); *dp = t->fwd_dp().inner(); *dm = t->fwd_dm().inner(); }
+    }
 };
+
+// Every hop of a batch in one library call (B200_traverse_batch_delta, CSR hand-off): (row, dest) pairs of F * hops, in
+// ascending order.  The batch rows are the surviving sources' positions in the input batch.
+inline void traverse_coalesced(const std::vector<uint64_t> &rows, const std::vector<uint64_t> &srcs,
+                               const std::vector<TraversalMatrix> &hops, std::vector<uint64_t> &out_row, std::vector<uint64_t> &out_dest) {
+    std::vector<GrB_Matrix> m(hops.size()), dp(hops.size()), dm(hops.size());
+    for (size_t h = 0; h < hops.size(); h++) hops[h].operands(&m[h], &dp[h], &dm[h]);
+    std::vector<uint64_t> p(srcs.size() + 1);
+    std::vector<uint32_t> j(std::max<size_t>(1024, 16 * srcs.size()));
+    uint64_t nv = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {              // a result larger than the first guess is rerun into its size
+        GrB_Info info = B200_traverse_batch_delta(srcs.data(), srcs.size(), m.data(), dp.data(), dm.data(), (int)hops.size(),
+                                                  B200_OUT_CSR, nullptr, 0, p.data(), j.data(), j.size(), &nv, nullptr, nullptr);
+        if (info == GrB_INSUFFICIENT_SPACE && attempt == 0) { j.resize(nv); continue; }
+        grb_ok(info, "B200_traverse_batch_delta");
+        break;
+    }
+    for (size_t r = 0; r < srcs.size(); r++)
+        for (uint64_t q = p[r]; q < p[r + 1]; q++) { out_row.push_back(rows[r]); out_dest.push_back(j[q]); }
+}
 
 // fuse_dst_labels (SURVEY 8f-2): label matrices are diagonal (graph.rs:1191), so the destination filter F*A*L_dst
 // (graph.rs:2600-2626) is one more delta_lmxm against the label's VersionedMatrix -- a column filter in frontier form on
 // the device -- instead of a node_has_label probe (1-3 extractElement calls) per output pair on the host.
+// coalesced: every hop, clean or dirty, and every fused label hop go to the library in ONE call (traverse_coalesced) instead of a
+// delta_lmxm per hop; the same pairs come back.
 inline ExpandResult expand_batch(const std::vector<uint64_t> &src_ids, const std::vector<TraversalMatrix> &hops,
                                  const std::vector<const VersionedMatrix *> &src_labels,
-                                 const std::vector<const VersionedMatrix *> &dst_labels, bool fuse_dst_labels = false) {
+                                 const std::vector<const VersionedMatrix *> &dst_labels, bool fuse_dst_labels = false,
+                                 bool coalesced = false) {
     ExpandResult out;
     if (hops.empty() || src_ids.empty()) return out;
     uint64_t ncols = hops[0].ncols();
@@ -54,6 +82,22 @@ inline ExpandResult expand_batch(const std::vector<uint64_t> &src_ids, const std
         col_idx_buf.push_back(src_ids[i]);
     }
     if (row_idx_buf.empty()) return out;
+    if (coalesced) {
+        std::vector<TraversalMatrix> all(hops);
+        if (fuse_dst_labels)
+            for (const VersionedMatrix *l : dst_labels) all.push_back(TraversalMatrix(l));
+        std::vector<uint64_t> rows, dests;
+        traverse_coalesced(row_idx_buf, col_idx_buf, all, rows, dests);
+        for (size_t k = 0; k < dests.size(); k++) {
+            bool ok = true;
+            if (!fuse_dst_labels)
+                for (const VersionedMatrix *l : dst_labels) if (!node_has_label(*l, dests[k])) { ok = false; break; }
+            if (!ok) continue;                   // post-filter final-hop dst label (= F * A * R_dst)
+            out.row_idx.push_back(rows[k]);
+            out.dest.push_back(dests[k]);
+        }
+        return out;
+    }
     Matrix<bool> f(src_ids.size(), ncols);
     f.build(row_idx_buf, col_idx_buf);
     for (const TraversalMatrix &h : hops) h.delta_lmxm_into(f);

@@ -553,6 +553,37 @@ static void t_traverse_over_tensor_operand() {
     REQUIRE(got == want, "3 fused hops over a dirty tensor snapshot");
 }
 
+// the coalesced form (one B200_traverse_batch_delta call) gives the per-hop delta_lmxm pairs over clean and dirty tensor operands
+static void t_coalesced_traverse_over_tensor_operand() {
+    auto pairs = [](const ExpandResult &r) {
+        std::vector<std::pair<uint64_t, uint64_t>> v;
+        for (size_t k = 0; k < r.dest.size(); k++) v.push_back({r.row_idx[k], r.dest[k]});
+        return v;
+    };
+    uint64_t n = 256;
+    std::vector<uint64_t> s, d, ids;
+    for (uint64_t i = 0; i < 250; i++) { s.push_back((i * 37) % n); d.push_back((i * 101 + 7) % n); ids.push_back(i); }
+    Tensor t(n, n);
+    t.set_all_from_slices(s, d, ids);                             // pending: everything still in the deltas
+    Tensor folded = t.dup();
+    folded.flush();                                               // clean: everything in the base
+    Tensor dirty = folded.dup();
+    std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> gone;
+    for (uint64_t i = 0; i < 250; i += 5) gone.push_back(std::make_tuple(ids[i], s[i], d[i]));   // (edge id, src, dst)
+    dirty.remove_all(gone);                                       // tombstones over the base
+    dirty.set_all_from_slices({1, 2, 3}, {200, 201, 202}, {900, 901, 902});
+    VersionedMatrix lab(n, n);
+    for (uint64_t v = 0; v < n; v += 3) lab.set(v, v);
+    std::vector<uint64_t> src = {0, 1, 5, 9, 17, 64, 100, 255};
+    for (const Tensor *x : {&t, &folded, &dirty}) {
+        std::vector<TraversalMatrix> hops = {TraversalMatrix(x), TraversalMatrix(x), TraversalMatrix(&lab), TraversalMatrix(x)};
+        for (bool fuse : {false, true}) {
+            ExpandResult a = expand_batch(src, hops, {&lab}, {&lab}, fuse), b = expand_batch(src, hops, {&lab}, {&lab}, fuse, true);
+            REQUIRE(pairs(a) == pairs(b), "coalesced tensor traversal differs from the per-hop delta_lmxm");
+        }
+    }
+}
+
 // ---- the C-compatible RDB form of a Tensor (tensor.rs:1049-1204) and of a VersionedMatrix (versioned_matrix.rs:1082-1113) ----
 typedef std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> EdgeList;
 static EdgeList sorted_edges(const Tensor &t) {
@@ -800,6 +831,7 @@ static TestEntry TESTS[] = {
     {"batch_demote_leaves_every_survivor_inline", t_batch_demote_leaves_every_survivor_inline},
     {"batch_can_demote_and_then_empty_the_same_pair", t_batch_can_demote_and_then_empty_the_same_pair},
     {"traverse_over_tensor_operand", t_traverse_over_tensor_operand},
+    {"coalesced_traverse_over_tensor_operand", t_coalesced_traverse_over_tensor_operand},
     {"repack_output_batches", t_repack_output_batches},
     {"repack_logic", t_repack_logic},
     {"var_len_trails", t_var_len_trails},
@@ -844,7 +876,8 @@ int64_t fdbh_vm_nvals(void *vm) { try { return (int64_t)((VersionedMatrix *)vm)-
 
 // CondTraverse batched path.  Outputs are malloc'ed; free with fdbh_free.
 static int expand_batch_c(const uint64_t *src_ids, uint64_t nsrc, void **hops, uint64_t nhops, void **src_labels, uint64_t nsl,
-                          void **dst_labels, uint64_t ndl, uint64_t **out_rows, uint64_t **out_dest, uint64_t *nout, bool fuse) {
+                          void **dst_labels, uint64_t ndl, uint64_t **out_rows, uint64_t **out_dest, uint64_t *nout, bool fuse,
+                          bool coalesced = false) {
     try {
         std::vector<uint64_t> src(src_ids, src_ids + nsrc);
         std::vector<TraversalMatrix> h;
@@ -852,7 +885,7 @@ static int expand_batch_c(const uint64_t *src_ids, uint64_t nsrc, void **hops, u
         for (uint64_t k = 0; k < nhops; k++) h.push_back(TraversalMatrix((const VersionedMatrix *)hops[k]));
         for (uint64_t k = 0; k < nsl; k++) sl.push_back((const VersionedMatrix *)src_labels[k]);
         for (uint64_t k = 0; k < ndl; k++) dl.push_back((const VersionedMatrix *)dst_labels[k]);
-        ExpandResult r = expand_batch(src, h, sl, dl, fuse);
+        ExpandResult r = expand_batch(src, h, sl, dl, fuse, coalesced);
         *nout = r.dest.size();
         *out_rows = (uint64_t *)malloc(sizeof(uint64_t) * (r.dest.size() + 1));
         *out_dest = (uint64_t *)malloc(sizeof(uint64_t) * (r.dest.size() + 1));
@@ -869,6 +902,13 @@ int fdbh_expand_batch(const uint64_t *src_ids, uint64_t nsrc, void **hops, uint6
 int fdbh_expand_batch_fused(const uint64_t *src_ids, uint64_t nsrc, void **hops, uint64_t nhops, void **src_labels, uint64_t nsl,
                             void **dst_labels, uint64_t ndl, uint64_t **out_rows, uint64_t **out_dest, uint64_t *nout) {
     return expand_batch_c(src_ids, nsrc, hops, nhops, src_labels, nsl, dst_labels, ndl, out_rows, out_dest, nout, true);
+}
+// every hop (and, with fuse_dst_labels, every destination label) in one B200_traverse_batch_delta call
+int fdbh_expand_batch_coalesced(const uint64_t *src_ids, uint64_t nsrc, void **hops, uint64_t nhops, void **src_labels, uint64_t nsl,
+                                void **dst_labels, uint64_t ndl, uint64_t **out_rows, uint64_t **out_dest, uint64_t *nout,
+                                int fuse_dst_labels) {
+    return expand_batch_c(src_ids, nsrc, hops, nhops, src_labels, nsl, dst_labels, ndl, out_rows, out_dest, nout, fuse_dst_labels != 0,
+                          true);
 }
 void fdbh_free(void *p) { free(p); }
 

@@ -230,6 +230,15 @@ class Matrix {
         if (accum.valid()) element_wise_add<bool>(nullptr, nullptr, &accum);
         mark_pending();
     }
+    // the same product as one library call (B200_Matrix_delta_lmxm): same result and flops, the delta terms applied in place
+    template <class TV>
+    void delta_lmxm_fused(const Matrix<TV> &m, const Matrix<TV> &dp, const Matrix<bool> &dm) {
+        static_assert(std::is_same<T, bool>::value, "delta_lmxm is defined on Matrix<bool>");
+        dp.wait();
+        dm.wait();
+        grb_ok(B200_Matrix_delta_lmxm(h->m, m.inner(), dp.inner(), dm.inner()), "B200_Matrix_delta_lmxm");
+        mark_pending();
+    }
 
     // ---- iteration: the reference's loop over the C row iterator (matrix.rs:1471-1605) ----
     class Iter {

@@ -56,6 +56,10 @@ void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt);   // 
 void bits_andnot(DevBits &Y, const DevBits &M); // Y &= ~M
 void bits_or(DevBits &Y, const DevBits &Z);     // Y |= Z
 void bits_copy(const DevBits &X, DevBits &Y);
+// The delta terms of delta_lmxm applied in place to Y = X * m:  Y = (Y AND NOT X * dm) OR X * dp, one pass over each delta's
+// entries.  The left operand is the bit-matrix Xb, or the CSR Xc when Y came from bits_push_from_csr (Xb null).  dm / dp may be
+// null.  X and Y stay in the vertex order they are stored in.  Returns flops(X * dm) + flops(X * dp).
+u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y);
 
 // ewise.cu : search-based set algebra on sorted CSR rows
 void csr_copy(const DevCSR &A, DevCSR &out, bool keep_values);

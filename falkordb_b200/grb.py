@@ -267,6 +267,11 @@ class Matrix:
         if accum is not None:
             self.element_wise_add(None, None, accum, None)
 
+    def delta_lmxm_fused(self, m, dp, dm):
+        """B200_Matrix_delta_lmxm: `delta_lmxm` as one call -- same result and flops; in device frontier form the dp / dm terms
+        are applied to F*m in place, touching only the deltas' entries.  dp / dm may be None."""
+        check(lib().B200_Matrix_delta_lmxm(self.h, m.h, None if dp is None else dp.h, None if dm is None else dm.h))
+
     def element_wise_add(self, mask=None, a=None, b=None, descriptor=None):
         op = obj("GxB_ANY_BOOL") if self.dtype is bool else obj("GrB_SECOND_UINT64")
         check(lib().GrB_Matrix_eWiseAdd_BinaryOp(self.h, mask.h if mask is not None else None, None, op,
@@ -404,18 +409,27 @@ def wait_ticket(ticket):
 OUT_AUTO, OUT_BITMAP, OUT_CSR = 0, 1, 2
 
 
-def traverse_batch(sources, hop_matrices, fmt=OUT_AUTO, out_bitmap=None, out_p=None, out_j=None):
+def traverse_batch(sources, hop_matrices, fmt=OUT_AUTO, out_bitmap=None, out_p=None, out_j=None, deltas=None):
     """B200_traverse_batch: the batched traversal an operator runs (cond_traverse.rs:600-608), host to host, as ONE C call.
     F(i, sources[i]) = 1, F <- F * hop_matrices[0] * ... ; the result lands in `out_bitmap` (uint64[nsrc, ceil(n/64)], pinned for
-    overlapped copies) and / or (`out_p` uint64[nsrc+1], `out_j` uint32[capacity]).  Returns (flops, nvals or None, format)."""
+    overlapped copies) and / or (`out_p` uint64[nsrc+1], `out_j` uint32[capacity]).  Returns (flops, nvals or None, format).
+    `deltas`: one (dp, dm) pair per hop (either may be None) -- hop h is then delta_lmxm by (hop_matrices[h], dp, dm), through
+    B200_traverse_batch_delta."""
     sources = _u64arr(sources)
-    hs = (C.c_void_p * len(hop_matrices))(*[m.h for m in hop_matrices])
+    nh = len(hop_matrices)
+    hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
     nv, fl, chosen = U64(0), U64(0), C.c_int(0)
     wpr = out_bitmap.shape[1] if out_bitmap is not None else 0
-    info = lib().B200_traverse_batch(sources.ctypes.data, len(sources), hs, len(hop_matrices), fmt,
-                                     None if out_bitmap is None else out_bitmap.ctypes.data, wpr,
-                                     None if out_p is None else out_p.ctypes.data, None if out_j is None else out_j.ctypes.data,
-                                     0 if out_j is None else len(out_j), C.byref(nv), C.byref(fl), C.byref(chosen))
+    outs = (fmt, None if out_bitmap is None else out_bitmap.ctypes.data, wpr,
+            None if out_p is None else out_p.ctypes.data, None if out_j is None else out_j.ctypes.data,
+            0 if out_j is None else len(out_j), C.byref(nv), C.byref(fl), C.byref(chosen))
+    if deltas is None:
+        info = lib().B200_traverse_batch(sources.ctypes.data, len(sources), hs, nh, *outs)
+    else:
+        assert len(deltas) == nh, "one (dp, dm) pair per hop"
+        dps = (C.c_void_p * nh)(*[None if d[0] is None else d[0].h for d in deltas])
+        dms = (C.c_void_p * nh)(*[None if d[1] is None else d[1].h for d in deltas])
+        info = lib().B200_traverse_batch_delta(sources.ctypes.data, len(sources), hs, dps, dms, nh, *outs)
     if info == -103:                     # GrB_INSUFFICIENT_SPACE: nv holds the entries needed
         raise BufferError(f"out_j holds {0 if out_j is None else len(out_j)} entries, the result has {nv.value}")
     check(info)

@@ -349,6 +349,18 @@ GrB_Info B200_Matrix_extract_pairs(GrB_Matrix A, const GrB_Index *I, const GrB_I
 GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, int nhops, int format,
                              uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
                              uint64_t *nvals_out, uint64_t *flops_out, int *format_out);
+/* delta_lmxm (matrix.rs:1317-1402) as one call, for an operand with pending writes held as base m plus deltas dp (added) and dm
+ * (deleted): F <- (F*m AND NOT F*dm) OR F*dp over GxB_ANY_PAIR_BOOL, the reference's three-mxm-plus-eWiseAdd composition with its
+ * over-masking ((i,j) is dropped whenever a deleted edge reaches j from row i).  Holds for arbitrary deltas; dp / dm may be NULL or
+ * empty; values are ignored (m and dp may be UINT64); pending tuples of dp / dm are finished first.  In device frontier form the
+ * delta terms touch only the deltas' entries; otherwise the composition runs.  last_flops = flops(F*m) + flops(F*dp) + flops(F*dm). */
+GrB_Info B200_Matrix_delta_lmxm(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_Matrix dm);
+/* B200_traverse_batch over operands with pending writes: hop h is B200_Matrix_delta_lmxm(F, m[h], dp[h], dm[h]).  dp / dm may be
+ * NULL arrays or hold NULL entries (clean hops); outputs and formats as B200_traverse_batch. */
+GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
+                                   const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row,
+                                   uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out,
+                                   int *format_out);
 /* Multi-source reachability in one call (SURVEY 8f-1: CondVarLenTraverse with emit_path = false, cond_var_len_traverse.rs:196;
  * AllShortestPaths' BFS phase, all_shortest_paths.rs:7-25): row i of *reached (new nsrc x n BOOL matrix) = the vertices reachable
  * from sources[i] by 1..max_hops edges of the square matrix A (max_hops < 0: to the fixed point); include_sources adds the
@@ -363,7 +375,7 @@ uint64_t B200_get_stat(const char *name);
 void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
- * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count".  0 on success. */
+ * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
