@@ -91,10 +91,7 @@ def lib():
         "B200_set_option": [C.c_char_p, I64],
         "B200_Matrix_extract_pairs": [P, P, P, U64, P, P],
         "B200_Matrix_rmat_block": [C.POINTER(P), C.c_int, U64, U64, U64, U64, C.c_int],
-        "B200_bfs_dist_expand": [P, U64, P, U64, P, P, U64, C.POINTER(U64)],
-        "B200_bfs_dist_merge": [P, C.c_int, U64, P, U64, U64, P, C.c_int32, P, P, P],
-        "B200_bfs_dist_pull": [P, U64, P, P, P, U64, C.POINTER(U64)],
-        "B200_bfs_dist_parents": [P, U64, P, P], "B200_bfs": [P, U64, I64, P, P, C.c_int, C.POINTER(U64)],
+        "B200_bfs": [P, U64, I64, P, P, C.c_int, C.POINTER(U64)],
         "B200_bfs_ex": [P, U64, I64, I64, P, P, C.c_int, P],
         "B200_comm_unique_id": [P], "B200_comm_init": [C.POINTER(P), C.c_int, C.c_int, P], "B200_comm_free": [C.POINTER(P)],
         "B200_bfs_partitioned": [P, P, U64, U64, P, U64, I64, I64, P, P, C.c_int, P],

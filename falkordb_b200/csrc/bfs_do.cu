@@ -15,6 +15,9 @@
 // vertices; bottom-up all-gathers the owned n/P-bit slices in place.  Switch rule (Beamer): bottom-up while the frontier's
 // out-edges exceed 1/ALPHA of the unexplored edges, back to top-down when the frontier shrinks below n/BETA.
 // One small host read per level (frontier size / edges / dest flag) steers the loop; nothing else leaves the device.
+//
+// Without A' (one BFS on a fresh matrix, where building the mirror would cost more than the search) bfs_run runs a plain
+// top-down BFS on one GPU with the same level and min-id parent; it has no dest early exit.
 #include "common.cuh"
 #include "ops.cuh"
 #include <nccl.h>
@@ -270,6 +273,54 @@ k_do_stats(const u64 *__restrict__ newb, u64 nw, u64 *__restrict__ visited, cons
     if ((threadIdx.x & 31) == 0 && cnt) { atomicAdd((unsigned long long *)&st[0], cnt); atomicAdd((unsigned long long *)&st[1], ed); }
 }
 
+// ---------------------------------------------------------------------------------------------- top-down only (no A')
+__global__ void k_bfs_init(i64 *__restrict__ level, i64 *__restrict__ parent, u64 *__restrict__ cand, u64 n, u64 src) {
+    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 stride = (u64)gridDim.x * blockDim.x;
+    for (; t < n; t += stride) {
+        level[t] = (t == src) ? 0 : -1;
+        if (parent) parent[t] = (t == src) ? (i64)src : -1;
+        cand[t] = ~0ULL;
+    }
+}
+
+// PHASE 0: cand[v] = min(cand[v], u) for unvisited v.  PHASE 1: the winning (u,v) claims v.
+template <int PHASE>
+__global__ void __launch_bounds__(256)
+k_bfs_expand(const u32 *__restrict__ fr, const u64 *__restrict__ cum, const u64 *__restrict__ start, u64 nf, u64 total,
+             const u32 *__restrict__ Aj, i64 *__restrict__ level, i64 *__restrict__ parent, u64 *__restrict__ cand,
+             i64 next_level, u32 *__restrict__ next, u32 *__restrict__ next_count) {
+    __shared__ u64 s_e0, s_e1;
+    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    u64 lo = (u64)blockIdx.x * DO_CHUNK, hi = lo + DO_CHUNK;
+    if (hi > total) hi = total;
+    if (tid == 0) {
+        s_e0 = do_find_le(cum, 0, nf - 1, lo);
+        s_e1 = do_find_le(cum, 0, nf - 1, hi - 1);
+    }
+    __syncthreads();
+    u64 e0 = s_e0, e1 = s_e1;
+    for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
+        u64 e = do_find_le(cum, e0, e1, t0);
+        u64 t = t0 + lane;
+        if (t < hi) {
+            while (e < e1 && cum[e + 1] <= t) e++;
+            u32 u = fr[e];
+            u32 v = Aj[start[e] + (t - cum[e])];
+            if (PHASE == 0) {
+                if (level[v] < 0) atomicMin((unsigned long long *)&cand[v], (unsigned long long)u);
+            } else {
+                // level[v] is only ever written here, by the unique (u,v) with u == cand[v]
+                if (cand[v] == (u64)u && level[v] < 0) {
+                    level[v] = next_level;
+                    if (parent) parent[v] = (i64)u;
+                    next[atomicAdd(next_count, 1u)] = v;
+                }
+            }
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- driver
 // deg_all: device u32[n_pad] (out-degrees of every vertex, replicated); total_edges = sum of it.
 void bfs_build_degrees(const DevCSR &Aloc, u64 n, u64 lo, u64 hi, BfsComm *comm, DevBuf<u32> &deg_all, u64 *total_edges) {
@@ -426,6 +477,40 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
         rec.edges = edges;
         *info = rec;
     }
+}
+
+// Top-down BFS over A alone.  The parent is made deterministic by a candidate pass before the claim pass: cand[v] = the minimum
+// frontier id with an edge to v (atomicMin), so only that u claims v.
+// Algorithmic bytes (SURVEY 8d): 4*m_visited*2 + 16*n_visited + 16*n_reached.
+void bfs_run(const DevCSR &A, u64 src, i64 max_level, i64 *d_level, i64 *d_parent, u64 *edges_traversed) {
+    u64 n = A.nrows;
+    if (src >= n) throw GrbError(-4, "BFS source out of range");
+    DevBuf<u64> cand(n);
+    LAUNCH(k_bfs_init, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, d_level, d_parent, cand.ptr, n, src);
+    DevBuf<u32> fa(n), fb(n), ncount(1);
+    u32 s32 = (u32)src;
+    h2d(fa.ptr, &s32, 1);
+    u64 nf = 1, edges = 0;
+    i64 lvl = 0;
+    u32 *cur = fa.ptr, *nxt = fb.ptr;
+    DevBuf<u64> cum(n + 1), start(n);
+    while (nf > 0 && (max_level < 0 || lvl < max_level)) {
+        LAUNCH(k_do_frontier_deg, grid_for(nf + 1, 256, (u64)ctx().num_sms * 16), 256, 0, cur, nf, (u64)0, A.p.ptr, cum.ptr, start.ptr);
+        exclusive_scan_u64(cum.ptr, cum.ptr, nf + 1);
+        u64 total = read_scalar(cum.ptr + nf);
+        if (total == 0) break;
+        edges += total;
+        ncount.zero();
+        u32 grid = (u32)((total + DO_CHUNK - 1) / DO_CHUNK);
+        LAUNCH((k_bfs_expand<0>), grid, 256, 0, cur, cum.ptr, start.ptr, nf, total, A.j.ptr, d_level, d_parent, cand.ptr,
+               lvl + 1, nxt, ncount.ptr);
+        LAUNCH((k_bfs_expand<1>), grid, 256, 0, cur, cum.ptr, start.ptr, nf, total, A.j.ptr, d_level, d_parent, cand.ptr,
+               lvl + 1, nxt, ncount.ptr);
+        nf = read_scalar(ncount.ptr);
+        u32 *t = cur; cur = nxt; nxt = t;
+        lvl++;
+    }
+    if (edges_traversed) *edges_traversed = edges;
 }
 
 } // namespace b200

@@ -1800,24 +1800,36 @@ int LAGraph_cdlp(GrB_Vector *CDLP_handle, LAGraph_Graph G, int itermax, char *ms
     if (info && msg) snprintf(msg, 256, "%s", tl_error.c_str());
     return info;
 }
-// Single-GPU BFS.  With the transpose mirror in place (B200_Matrix_prepare(A, 1), or any earlier pull) the direction-optimising
-// engine runs (bfs_do.cu); without it -- one BFS on a fresh matrix, where building A' would cost more than the search -- the
-// top-down kernel of bfs.cu.  Both give level and minimum-id parent.  dest >= 0 stops once that vertex is reached.
-static void bfs_any(GrB_Matrix A, u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, u64 *edges, BfsInfo *info) {
-    if (A->devT_valid && ctx().opt_bfs_direction != 3) {
-        if (!A->bfs_deg_valid) { bfs_build_degrees(A->dev, A->nrows, 0, A->nrows, nullptr, A->bfs_deg, &A->bfs_edges); A->bfs_deg_valid = true; }
-        BfsInfo rec;
-        bfs_do(A->dev, A->devT, A->nrows, 0, A->nrows, A->bfs_deg.ptr, A->bfs_edges, nullptr, src, max_level, dest, d_level, d_parent, &rec);
-        if (edges) *edges = rec.edges;
-        if (info) *info = rec;
+// One BFS over rows [lo, lo + nrows(A)) of the n-vertex graph; level / parent of those rows go to `location` memory.  With AT
+// (the same rows of A') the direction-optimising engine runs, its out-degree table cached on A; without it (one GPU, lo = 0)
+// the top-down bfs_run.  Both give level and minimum-id parent.  dest >= 0 stops once that vertex is reached.
+static void bfs_staged(GrB_Matrix A, const DevCSR *AT, u64 n, u64 lo, BfsComm *comm, u64 src, i64 max_level, i64 dest,
+                       i64 *level, i64 *parent, int location, B200_BfsInfo *info_out) {
+    const u64 nloc = A->nrows, hi = lo + nloc;
+    DevBuf<i64> dl, dp;
+    i64 *d_level = level, *d_parent = parent;
+    if (location != B200_LOC_DEVICE) {
+        dl.alloc(nloc ? nloc : 1); d_level = dl.ptr;
+        if (parent) { dp.alloc(nloc ? nloc : 1); d_parent = dp.ptr; }
+    }
+    BfsInfo rec;
+    memset(&rec, 0, sizeof(rec));
+    if (AT) {
+        if (!A->bfs_deg_valid) { bfs_build_degrees(A->dev, n, lo, hi, comm, A->bfs_deg, &A->bfs_edges); A->bfs_deg_valid = true; }
+        bfs_do(A->dev, *AT, n, lo, hi, A->bfs_deg.ptr, A->bfs_edges, comm, src, max_level, dest, d_level, d_parent, &rec);
     } else {
         if (dest >= 0) throw GrbError(GrB_NOT_IMPLEMENTED, "BFS with a destination needs the transpose mirror (B200_Matrix_prepare)");
-        u64 e = 0;
-        bfs_run(A->dev, src, max_level, d_level, d_parent, &e);
-        if (edges) *edges = e;
-        if (info) { memset(info, 0, sizeof(*info)); info->edges = e; }
+        bfs_run(A->dev, src, max_level, d_level, d_parent, &rec.edges);
     }
+    if (location != B200_LOC_DEVICE) {
+        d2h(level, d_level, nloc);
+        if (parent) d2h(parent, d_parent, nloc);
+    }
+    sync_stream();
+    if (info_out) memcpy(info_out, &rec, sizeof(rec));
 }
+// Single-GPU BFS.  With the transpose mirror in place (B200_Matrix_prepare(A, 1), or any earlier pull) the direction-optimising
+// engine runs; without it -- one BFS on a fresh matrix, where building A' would cost more than the search -- the top-down one.
 GrB_Info B200_bfs_ex(GrB_Matrix A, GrB_Index src, int64_t max_level, int64_t dest, int64_t *level, int64_t *parent, int location,
                      B200_BfsInfo *info_out) {
     CHECK_MAT(A); CHECK_PTR(level);
@@ -1828,21 +1840,7 @@ GrB_Info B200_bfs_ex(GrB_Matrix A, GrB_Index src, int64_t max_level, int64_t des
         MultiLock lk{A};
         ensure_init();
         ensure_dev(A);
-        u64 n = A->nrows, edges = 0;
-        BfsInfo rec;
-        memset(&rec, 0, sizeof(rec));
-        if (location == B200_LOC_DEVICE) {
-            bfs_any(A, src, max_level, dest, level, parent, &edges, &rec);
-            sync_stream();
-        } else {
-            DevBuf<i64> dl(n), dp;
-            if (parent) dp.alloc(n);
-            bfs_any(A, src, max_level, dest, dl.ptr, parent ? dp.ptr : nullptr, &edges, &rec);
-            d2h(level, dl.ptr, n);
-            if (parent) d2h(parent, dp.ptr, n);
-            sync_stream();
-        }
-        if (info_out) memcpy(info_out, &rec, sizeof(rec));
+        bfs_staged(A, A->devT_valid ? &A->devT : nullptr, A->nrows, 0, nullptr, src, max_level, dest, level, parent, location, info_out);
         return GrB_SUCCESS;
     });
 }
@@ -1886,23 +1884,7 @@ GrB_Info B200_bfs_partitioned(GrB_Matrix Alocal, GrB_Matrix ATlocal, uint64_t n,
         MultiLock lk{Alocal, ATlocal};
         ensure_init();
         ensure_dev(Alocal); ensure_dev(ATlocal);
-        BfsComm *c = (BfsComm *)comm;
-        const u64 nloc = Alocal->nrows, hi = row_lo + nloc;
-        if (!Alocal->bfs_deg_valid) { bfs_build_degrees(Alocal->dev, n, row_lo, hi, c, Alocal->bfs_deg, &Alocal->bfs_edges); Alocal->bfs_deg_valid = true; }
-        BfsInfo rec;
-        memset(&rec, 0, sizeof(rec));
-        if (location == B200_LOC_DEVICE) {
-            bfs_do(Alocal->dev, ATlocal->dev, n, row_lo, hi, Alocal->bfs_deg.ptr, Alocal->bfs_edges, c, src, max_level, dest, level_local, parent_local, &rec);
-            sync_stream();
-        } else {
-            DevBuf<i64> dl(nloc ? nloc : 1), dp;
-            if (parent_local) dp.alloc(nloc ? nloc : 1);
-            bfs_do(Alocal->dev, ATlocal->dev, n, row_lo, hi, Alocal->bfs_deg.ptr, Alocal->bfs_edges, c, src, max_level, dest, dl.ptr, parent_local ? dp.ptr : nullptr, &rec);
-            d2h(level_local, dl.ptr, nloc);
-            if (parent_local) d2h(parent_local, dp.ptr, nloc);
-            sync_stream();
-        }
-        if (info_out) memcpy(info_out, &rec, sizeof(rec));
+        bfs_staged(Alocal, &ATlocal->dev, n, row_lo, (BfsComm *)comm, src, max_level, dest, level_local, parent_local, location, info_out);
         return GrB_SUCCESS;
     });
 }
@@ -2241,61 +2223,6 @@ GrB_Info B200_Matrix_rmat_block(GrB_Matrix *A, int scale, uint64_t edge_factor, 
         sync_stream();
         set_dev(m, std::move(d));
         *A = mh.release();
-        return GrB_SUCCESS;
-    });
-}
-
-// ---- 1-D row-partitioned BFS steps (all pointers are DEVICE pointers owned by the caller, e.g. torch tensors) ----
-GrB_Info B200_bfs_dist_expand(GrB_Matrix Alocal, uint64_t row_lo, const uint32_t *frontier, uint64_t nf, const uint64_t *visited,
-                              uint64_t *disc, uint64_t nwords, uint64_t *edges_out) {
-    CHECK_MAT(Alocal);
-    return guarded([&]() {
-        GpuLock g;
-        MultiLock lk{Alocal};
-        ensure_init();
-        ensure_dev(Alocal);
-        u64 edges = 0;
-        bfs_dist_expand(Alocal->dev, row_lo, frontier, nf, visited, disc, nwords, &edges);
-        sync_stream();   // the caller hands `disc` to NCCL on another stream next
-        if (edges_out) *edges_out = edges;
-        return GrB_SUCCESS;
-    });
-}
-GrB_Info B200_bfs_dist_merge(const uint64_t *gathered, int nranks, uint64_t nwords, uint64_t *visited, uint64_t row_lo,
-                             uint64_t row_hi, int32_t *level_local, int32_t lvl, uint32_t *next_frontier, uint64_t *counters2,
-                             uint64_t *frontier_bits) {
-    CHECK_PTR(gathered); CHECK_PTR(counters2);
-    return guarded([&]() {
-        GpuLock g;
-        ensure_init();
-        bfs_dist_merge(gathered, nranks, nwords, visited, row_lo, row_hi, level_local, lvl, next_frontier, counters2, frontier_bits);
-        return GrB_SUCCESS;
-    });
-}
-GrB_Info B200_bfs_dist_pull(GrB_Matrix ATlocal, uint64_t row_lo, const uint64_t *frontier_bits, const uint64_t *visited,
-                            uint64_t *disc, uint64_t nwords, uint64_t *scanned_out) {
-    CHECK_MAT(ATlocal);
-    return guarded([&]() {
-        GpuLock g;
-        MultiLock lk{ATlocal};
-        ensure_init();
-        ensure_dev(ATlocal);
-        u64 sc = 0;
-        bfs_dist_pull(ATlocal->dev, row_lo, frontier_bits, visited, disc, nwords, &sc);
-        sync_stream();
-        if (scanned_out) *scanned_out = sc;
-        return GrB_SUCCESS;
-    });
-}
-GrB_Info B200_bfs_dist_parents(GrB_Matrix ATlocal, uint64_t row_lo, const int32_t *level_full, int64_t *parent_local) {
-    CHECK_MAT(ATlocal);
-    return guarded([&]() {
-        GpuLock g;
-        MultiLock lk{ATlocal};
-        ensure_init();
-        ensure_dev(ATlocal);
-        bfs_dist_parents(ATlocal->dev, row_lo, level_full, parent_local);
-        sync_stream();
         return GrB_SUCCESS;
     });
 }

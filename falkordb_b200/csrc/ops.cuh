@@ -71,18 +71,8 @@ void csr_resize(const DevCSR &A, u64 nrows, u64 ncols, DevCSR &out); // grow/shr
 // Z = pattern(A*B) restricted to M's structure (valued mask: entries of M with value 0 excluded unless structural)
 void spgemm_masked(const DevCSR &A, const DevCSR &B, const DevCSR &M, bool structural, DevCSR &out, u64 flops = 0);
 
-// bfs.cu
-void bfs_run(const DevCSR &A, u64 src, i64 max_level, i64 *d_level, i64 *d_parent, u64 *edges_traversed);
-void bfs_dist_expand(const DevCSR &Aloc, u64 row_lo, const u32 *frontier, u64 nf, const u64 *visited, u64 *disc, u64 nwords,
-                     u64 *edges_out);
-void bfs_dist_pull(const DevCSR &ATloc, u64 row_lo, const u64 *frontier, const u64 *visited, u64 *disc, u64 nwords,
-                   u64 *scanned_out);
-void bfs_dist_merge(const u64 *gathered, int P, u64 nwords, u64 *visited, u64 row_lo, u64 row_hi, int *level_local, int lvl,
-                    u32 *next, u64 *host_counters, u64 *frontier_bits);
-void bfs_dist_parents(const DevCSR &ATloc, u64 row_lo, const int *level_full, i64 *parent_local);
-
 void csr_digest(const DevCSR &A, u64 *host_out3);   // {nnz, sum mix(key), sum mix(key + GOLD * (pos + 1))}: see oracle orc_digest
-// bfs_do.cu : direction-optimising BFS, single GPU or 1-D row-block partitioned over NCCL
+// bfs_do.cu : direction-optimising BFS, single GPU or 1-D row-block partitioned over NCCL; top-down BFS without A'
 struct BfsComm;
 struct BfsInfo {          // mirrored by B200_BfsInfo in include/b200grb.h
     u64 depth, edges, td_levels, bu_levels, sparse_levels, exchanges, exchanged_bytes;
@@ -97,6 +87,7 @@ void comm_allgather(BfsComm *c, const void *send, void *recv, size_t bytes_per_r
 void bfs_build_degrees(const DevCSR &Aloc, u64 n, u64 lo, u64 hi, BfsComm *comm, DevBuf<u32> &deg_all, u64 *total_edges);
 void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, const u32 *deg_all, u64 total_edges, BfsComm *comm,
             u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, BfsInfo *info);
+void bfs_run(const DevCSR &A, u64 src, i64 max_level, i64 *d_level, i64 *d_parent, u64 *edges_traversed);
 
 // algo.cu : FP64 mxv (PLUS_TIMES / PLUS_SECOND) and PageRank
 void mxv_fp64(const DevCSR &A, bool use_values, const double *x, const unsigned char *present, double *y, unsigned char *ypresent,

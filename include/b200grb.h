@@ -314,19 +314,6 @@ GrB_Info B200_Matrix_rmat(GrB_Matrix *A, int scale, uint64_t edge_factor, uint64
  * block of the TRANSPOSE, by_col == 2 of the symmetrised strictly-lower-triangular matrix L = tril(A u A') (config 4).  Every rank regenerates the counter-based edge stream and keeps what it owns. */
 GrB_Info B200_Matrix_rmat_block(GrB_Matrix *A, int scale, uint64_t edge_factor, uint64_t seed, uint64_t lo, uint64_t hi,
                                 int by_col);
-/* 1-D row-partitioned BFS building blocks (SURVEY 8e): one level = expand the owned part of the frontier into an
- * n-bit `disc` bitmap; the caller all-gathers the bitmaps (NCCL); merge ORs them, updates `visited`, assigns levels to
- * owned vertices and emits the next owned frontier.  counters2[0] = next owned frontier size, [1] = new vertices
- * globally (0 => done).  Every pointer is a DEVICE pointer except counters2 / edges_out (host). */
-GrB_Info B200_bfs_dist_expand(GrB_Matrix Alocal, uint64_t row_lo, const uint32_t *frontier, uint64_t nf, const uint64_t *visited,
-                              uint64_t *disc, uint64_t nwords, uint64_t *edges_out);
-GrB_Info B200_bfs_dist_merge(const uint64_t *gathered, int nranks, uint64_t nwords, uint64_t *visited, uint64_t row_lo,
-                             uint64_t row_hi, int32_t *level_local, int32_t lvl, uint32_t *next_frontier, uint64_t *counters2,
-                             uint64_t *frontier_bits /* optional: receives the new frontier as an n-bit bitmap */);
-/* bottom-up step: owned unvisited vertices scan their in-neighbours (row block of A') for a frontier member */
-GrB_Info B200_bfs_dist_pull(GrB_Matrix ATlocal, uint64_t row_lo, const uint64_t *frontier_bits, const uint64_t *visited,
-                            uint64_t *disc, uint64_t nwords, uint64_t *scanned_out);
-GrB_Info B200_bfs_dist_parents(GrB_Matrix ATlocal, uint64_t row_lo, const int32_t *level_full, int64_t *parent_local);
 
 /* GRAPH.BULK's edge load into an EMPTY relationship tensor (src/commands/bulk_insert.rs:497 -> graph.rs:2062 ->
  * Tensor::set_all_from_slices, tensor.rs:333-447) as one device-side build: *fwd = the forward UINT64 matrix (value = the pair's
