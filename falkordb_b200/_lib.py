@@ -78,6 +78,7 @@ def lib():
         "LAGr_BreadthFirstSearch_Extended": [C.POINTER(P), C.POINTER(P), P, U64, I64, I64, C.c_bool, C.c_char_p],
         "B200_Matrix_import_CSR": [C.POINTER(P), P, U64, U64, P, P, P, C.c_int],
         "B200_reach_batch": [C.POINTER(P), P, U64, P, I64, C.c_int, C.POINTER(I64)],
+        "B200_reach_batch_delta": [C.POINTER(P), P, U64, P, P, P, C.c_int, I64, C.c_int, C.POINTER(I64)],
         "B200_Tensor_bulk_build": [C.POINTER(P), C.POINTER(C.POINTER(U64)), C.POINTER(C.POINTER(U64)), C.POINTER(U64), U64, U64, P, P, P, U64],
         "B200_Matrix_export_CSR": [P, P, P, P, C.c_int],
         "B200_Matrix_export_bitmap": [P, P, U64, C.POINTER(U64), C.c_int],

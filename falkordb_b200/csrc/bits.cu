@@ -1399,4 +1399,174 @@ u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, con
     }
 }
 
+// ---------------------------------------------------------------------------- exact dirty hop (reach over (m \ dm) u dp)
+// delta_lmxm's AND-NOT term over-masks: it drops (i, j) whenever ANY deleted edge reaches j from row i, even when a remaining edge
+// still reaches it.  A reach over a tensor with pending deletions needs X * (m \ dm) exactly.  Only the columns dm touches can
+// differ from X * m, so those columns are recomputed: Y[pos(j)] = OR of X[pos(k)] over the in-edges k of m'(j, :) that are not in
+// dm'(j, :).  Both rows are sorted, so a lane finds its in-edge in the deleted list with a lower bound that only moves forward.
+// Hub columns are cut into REPAIR_SEG-entry segments, as the pull cuts long rows: a column of several segments is zeroed first and
+// its segments arrive through RED.OR; a column of one segment is stored.  Work is O(W * the repaired columns' in-degrees).
+static const u64 REPAIR_SEG = 1024;
+static const u32 REPAIR_ATOMIC = 0x80000000u, REPAIR_FIRST = 0x40000000u, REPAIR_LEN = 0x3FFFFFFFu;
+
+// segments per column: ceil(indeg_m(j) / REPAIR_SEG) where dm' has a row j, else 0;  st = {repaired columns, their in-edges}
+__global__ void __launch_bounds__(256)
+k_repair_count(const u64 *__restrict__ Dp, const u64 *__restrict__ Tp, u64 n, u32 *__restrict__ cnt, u64 *__restrict__ st) {
+    typedef cub::BlockReduce<u64, 256> Red;
+    __shared__ typename Red::TempStorage ts;
+    u64 c = 0, e = 0;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j <= n; j += stride) {
+        if (j == n) { cnt[j] = 0; continue; }
+        const u64 d = Dp[j + 1] > Dp[j] ? Tp[j + 1] - Tp[j] : 0;
+        cnt[j] = (u32)((d + REPAIR_SEG - 1) / REPAIR_SEG);
+        c += d != 0;
+        e += d;
+    }
+    const u64 tc = Red(ts).Sum(c);
+    __syncthreads();
+    const u64 te = Red(ts).Sum(e);
+    if (threadIdx.x == 0) {
+        if (tc) atomicAdd((unsigned long long *)&st[0], tc);
+        if (te) atomicAdd((unsigned long long *)&st[1], te);
+    }
+}
+__global__ void k_repair_emit(const u64 *__restrict__ Tp, const u32 *__restrict__ cnt, const u64 *__restrict__ pos, u64 n,
+                              u32 *__restrict__ s_col, u64 *__restrict__ s_start, u32 *__restrict__ s_len) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+        const u32 c = cnt[j];
+        if (!c) continue;
+        const u64 t0 = Tp[j], d = Tp[j + 1] - t0, o = pos[j];
+        for (u32 i = 0; i < c; i++) {
+            const u64 s = (u64)i * REPAIR_SEG, len = d - s < REPAIR_SEG ? d - s : REPAIR_SEG;
+            s_col[o + i] = (u32)j;
+            s_start[o + i] = t0 + s;
+            s_len[o + i] = (u32)len | (c > 1 ? (REPAIR_ATOMIC | (i == 0 ? REPAIR_FIRST : 0u)) : 0u);
+        }
+    }
+}
+// the columns merged with RED.OR start from zero (their first segment names them once)
+template <int W>
+__global__ void k_repair_zero(const u32 *__restrict__ s_col, const u32 *__restrict__ s_len, u64 ns, const u32 *__restrict__ yperm,
+                              u64 *__restrict__ Y) {
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += stride) {
+        if (!(s_len[i] & REPAIR_FIRST)) continue;
+        const u64 j = s_col[i], py = yperm ? yperm[j] : j;
+#pragma unroll
+        for (int w = 0; w < W; w++) Y[py * W + w] = 0;
+    }
+}
+// 8 lanes per segment, dealt round-robin; inside a group VG in-edges x SPLIT record parts per unroll step (the pull's lane split).
+template <int W, int U>
+__global__ void __launch_bounds__(256)
+k_bits_repair(const u32 *__restrict__ s_col, const u64 *__restrict__ s_start, const u32 *__restrict__ s_len, u64 ns,
+              const u32 *__restrict__ Tj, const u64 *__restrict__ Dp, const u32 *__restrict__ Dj, const u64 *__restrict__ X,
+              const u32 *__restrict__ xperm, u64 *__restrict__ Y, const u32 *__restrict__ yperm) {
+    constexpr int WL = PullCfg<W>::WL, SPLIT = PullCfg<W>::SPLIT, VG = PullCfg<W>::VG;
+    const u32 lane8 = threadIdx.x & 7;
+    const u32 gmask = 0xFFu << (8 * ((threadIdx.x & 31) >> 3));
+    const u32 vi = lane8 / SPLIT, h = lane8 % SPLIT;
+    const u64 *Xh = X + h * WL;
+    const u64 ngroups = ((u64)gridDim.x * blockDim.x) >> 3;
+    for (u64 i = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < ns; i += ngroups) {   // uniform inside the 8-lane group
+        const u32 j = __ldg(s_col + i), fl = __ldg(s_len + i);
+        const u64 s = __ldg(s_start + i), e = s + (fl & REPAIR_LEN), de = __ldg(Dp + j + 1);
+        u64 d = __ldg(Dp + j);
+        u64 acc[WL];
+#pragma unroll
+        for (int w = 0; w < WL; w++) acc[w] = 0;
+        for (u64 qb = s; qb < e; qb += VG * U) {
+            u32 k[U];
+#pragma unroll
+            for (int u = 0; u < U; u++) { const u64 q = qb + vi + VG * u; k[u] = q < e ? __ldg(Tj + q) : 0xFFFFFFFFu; }
+#pragma unroll
+            for (int u = 0; u < U; u++) {
+                if (k[u] == 0xFFFFFFFFu) continue;
+                u64 lo = d, hi = de;                 // lower bound of k[u] among the deleted sources of j
+                while (lo < hi) {
+                    const u64 mid = (lo + hi) >> 1;
+                    if (__ldg(Dj + mid) < k[u]) lo = mid + 1; else hi = mid;
+                }
+                d = lo;
+                if (d < de && __ldg(Dj + d) == k[u]) continue;   // a deleted edge
+                const u64 px = xperm ? __ldg(xperm + k[u]) : k[u];
+                or_words<WL, false>(acc, Xh + px * W, 0);
+            }
+        }
+#pragma unroll
+        for (int w = 0; w < WL; w++) {
+            u64 a = acc[w];
+#pragma unroll
+            for (int dd = SPLIT; dd < 8; dd <<= 1) a |= __shfl_xor_sync(gmask, a, dd);
+            acc[w] = a;
+        }
+        if (vi == 0) {
+            const u64 py = yperm ? __ldg(yperm + j) : j;
+            u64 *dst = Y + py * W + h * WL;
+            if (fl & REPAIR_ATOMIC) {
+#pragma unroll
+                for (int w = 0; w < WL; w++) if (acc[w]) atomicOr((unsigned long long *)(dst + w), acc[w]);
+            } else store_part<WL>(dst, acc);
+        }
+    }
+}
+
+void bits_repair_plan(const DevCSR &dm, const DevCSR &mT, RepairPlan &rp) {
+    if (dm.nrows != mT.ncols || dm.ncols != mT.nrows) throw GrbError(-6, "reach: delta dimensions differ from the operand");
+    rp.ns = rp.ncols = rp.inedges = 0;
+    rp.s_col.release(); rp.s_len.release(); rp.s_start.release();
+    rp.dmT.clear();
+    const u64 n = mT.nrows;
+    if (!dm.nnz || !n) return;
+    transpose_csr(dm, rp.dmT, false);                  // dm changes with every write: built per call
+    DevBuf<u32> cnt(n + 1);
+    DevBuf<u64> pos(n + 1), st(2);
+    st.zero();
+    LAUNCH(k_repair_count, grid_for(n + 1, 256, (u64)ctx().num_sms * 16), 256, 0, rp.dmT.p.ptr, mT.p.ptr, n, cnt.ptr, st.ptr);
+    exclusive_scan_u32_to_u64(cnt.ptr, pos.ptr, n + 1);
+    u64 h[3];
+    d2h(h, st.ptr, 2);
+    d2h(h + 2, pos.ptr + n, 1);
+    sync_stream();
+    rp.ncols = h[0]; rp.inedges = h[1]; rp.ns = h[2];
+    if (!rp.ns) return;
+    rp.s_col.alloc(rp.ns); rp.s_len.alloc(rp.ns); rp.s_start.alloc(rp.ns);
+    LAUNCH(k_repair_emit, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, mT.p.ptr, cnt.ptr, pos.ptr, n, rp.s_col.ptr,
+           rp.s_start.ptr, rp.s_len.ptr);
+}
+
+template <int W>
+static void repair_impl(const DevBits &X, const DevCSR &mT, const RepairPlan &rp, DevBits &Y) {
+    const u32 *xperm = X.permuted() ? X.pperm->ptr : nullptr, *yperm = Y.permuted() ? Y.pperm->ptr : nullptr;
+    // two row pointers per repaired column, m' and dm' column ids, the gathered records, the stored columns
+    TimedScope ts(TK_BITS_REPAIR, 16 * rp.ncols + 4 * rp.inedges + 4 * rp.dmT.nnz + 8ULL * W * rp.inedges + 8ULL * W * rp.ncols);
+    LAUNCH((k_repair_zero<W>), grid_for(rp.ns, 256, (u64)ctx().num_sms * 16), 256, 0, rp.s_col.ptr, rp.s_len.ptr, rp.ns, yperm, Y.w.ptr);
+    static int per_sm = 0;
+    if (!per_sm) {
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bits_repair<W, 4>, 256, 0));
+        if (per_sm < 1) per_sm = 1;
+    }
+    const u64 need = (rp.ns * 8 + 255) / 256, full = (u64)ctx().num_sms * (u64)per_sm;
+    LAUNCH((k_bits_repair<W, 4>), (u32)(need < full ? need : full), 256, 0, rp.s_col.ptr, rp.s_start.ptr, rp.s_len.ptr, rp.ns, mT.j.ptr,
+           rp.dmT.p.ptr, rp.dmT.j.ptr, X.w.ptr, xperm, Y.w.ptr, yperm);
+}
+
+void bits_repair(const DevBits &X, const DevCSR &mT, const RepairPlan &rp, DevBits &Y) {
+    if (!rp.ns) return;
+    if (X.ncols != mT.ncols || Y.ncols != mT.nrows) throw GrbError(-6, "reach: frontier dimensions differ from the operand");
+    if (X.W != Y.W) throw GrbError(-101, "reach: frontier and product word counts differ");
+    if ((Y.permuted() && !Y.pperm) || (X.permuted() && !X.pperm))
+        throw GrbError(-101, "reach: permuted frontier without its vertex -> position table");
+    switch (Y.W) {
+    case 1: repair_impl<1>(X, mT, rp, Y); break;
+    case 2: repair_impl<2>(X, mT, rp, Y); break;
+    case 4: repair_impl<4>(X, mT, rp, Y); break;
+    case 8: repair_impl<8>(X, mT, rp, Y); break;
+    case 16: repair_impl<16>(X, mT, rp, Y); break;
+    default: throw GrbError(-8, "bit-frontier: unsupported word count");
+    }
+}
+
 } // namespace b200

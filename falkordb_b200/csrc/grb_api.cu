@@ -229,9 +229,10 @@ static GrB_Info guarded(F &&f) {
 
 struct MultiLock {
     uvec<std::unique_lock<std::mutex>> locks;
-    MultiLock(std::initializer_list<GrB_Matrix> ms) {
+    MultiLock(std::initializer_list<GrB_Matrix> ms) : MultiLock(ms.begin(), ms.end()) {}
+    template <class It> MultiLock(It first, It last) {
         uvec<GrB_Matrix> v;
-        for (GrB_Matrix m : ms) if (m) v.push_back(m);
+        for (; first != last; ++first) if (*first) v.push_back(*first);
         std::sort(v.begin(), v.end());
         v.erase(std::unique(v.begin(), v.end()), v.end());
         for (GrB_Matrix m : v) locks.emplace_back(m->mu);
@@ -1025,6 +1026,28 @@ static bool bits_legal(GrB_Matrix C, GrB_Matrix M, GrB_Matrix A, GrB_Matrix B, c
     return true;
 }
 
+// Y = A*B through the frontier dispatch: the push straight from A's entries while A is still a small CSR, the diagonal filter, or
+// the direction-optimising push / pull.  known_flops: flops(A*B) when already counted (~0 otherwise); pt_ok: the CSR push may
+// write Y in B's hot-set order.  Returns true when Y came from A's CSR form (A then has no bit form).
+static bool frontier_product(GrB_Matrix A, GrB_Matrix B, u64 known_flops, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
+    Context &cx = ctx();
+    ensure_dev(B);
+    if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
+    // a frontier that is still a (small) CSR expands straight from its entries; large expansions decline
+    // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
+    const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
+                          A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
+                          !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, fl, (B->devT_valid && pt_ok) ? &B->pt : (const PullTables *)nullptr);
+    if (from_csr) { *path = 7; return true; }
+    if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
+    if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, fl); *path = 5; }
+    else {
+        if (cx.opt_pull_mode != 0) ensure_devT(B);
+        bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, fl, path);
+    }
+    return false;
+}
+
 // The frontier bit-matrix path of GrB_mxm (short-fat A, CondTraverse's F*A): C<!M, RSC> = A*B kept in device frontier form.
 // Returns false when the path does not apply (not legal, switched off, or the automatic choice prefers the general row-wise
 // path); C is then unchanged.  dm / dp (B200_Matrix_delta_lmxm): device-resident deltas of B whose terms are applied to the
@@ -1046,24 +1069,10 @@ static bool frontier_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_Matrix A, GrB_Matrix
         }
     }
     if (!use_bits) return false;
-    ensure_dev(B);
-    if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
     DevBits Y;
     u64 fl = 0;
     int path = 0;
-    // a frontier that is still a (small) CSR expands straight from its entries; large expansions decline
-    // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
-    const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
-                          A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
-                          !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, &fl, (B->devT_valid && !Mask) ? &B->pt : (const PullTables *)nullptr);
-    if (from_csr) path = 7;
-    else if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
-    if (from_csr) {}
-    else if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, &fl); path = 5; }
-    else {
-        if (cx.opt_pull_mode != 0) ensure_devT(B);
-        bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, &fl, &path);
-    }
+    const bool from_csr = frontier_product(A, B, known_flops, !Mask, Y, &fl, &path);
     if (Mask) {
         ensure_bits(Mask);
         bits_andnot(Y, Mask->bits);
@@ -2404,15 +2413,135 @@ GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, con
 // a new vertex); with include_sources the zero-length walk (i, sources[i]) belongs to the result and is never re-discovered.
 // Each level is F<!R, replace, struct> = F*A (GrB_DESC_RSC, matrix.rs:1386) followed by R = R u F (matrix.rs:1398-1400); both stay
 // in device frontier form for <= 1024 sources.  Composed from the public entry points.  *reached is a new nsrc x n BOOL matrix.
-GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, GrB_Matrix A, int64_t max_hops,
-                          int include_sources, int64_t *levels_out) {
-    CHECK_PTR(reached); CHECK_MAT(A);
-    if (nsrc) CHECK_PTR(sources);
-    if (A->nrows != A->ncols) { tl_error = "reach_batch: A must be square"; return GrB_DIMENSION_MISMATCH; }
-    const u64 n = A->ncols;
+//
+// B200_reach_batch_delta walks A = U_t (m[t] \ dm[t]) u dp[t] exactly (no delta_lmxm over-masking).  One operand without deltas
+// (B200_reach_batch) issues the calls above unchanged.  Otherwise a level in frontier form is reach_hop: per operand Y = F*m[t]
+// through the usual dispatch, the columns dm[t] touches recomputed from m[t]'s transpose mirror without the deleted in-edges
+// (bits_repair), then the dp[t] term; the operands' products are ORed, and only then is the reached set masked out, so a dp edge
+// cannot re-add a vertex already reached.  With bits_mode -1 the dirty reach stays in frontier form whenever it is legal (a tiny
+// hop-1 frontier takes the CSR push there): the row-wise path would first need every dirty operand rewritten, O(nnz(m)) per call.
+// Where the frontier path does not apply (bits_mode 0, more than 1024 sources) every dirty operand is materialised once per call
+// with the flush kernels (filter_by_mask, ewise_union) and the level runs the calls above over their union.
+
+struct ReachOperand {
+    GrB_Matrix m = nullptr, dp = nullptr, dm = nullptr;
+    const DevCSR *ddp = nullptr;                 // dp's device form when it holds entries
+    RepairPlan rp;                               // dm's repair plan (rp.ns == 0: nothing to repair)
+};
+
+// One level in frontier form: F <- (OR_t F * E_t) AND NOT R (R only when masked).  F has at most 1024 rows.  Runs under the
+// submission lock.
+static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<ReachOperand> &ops) {
+    Context &cx = ctx();
+    const size_t nops = ops.size();
+    finish_pending(F);
+    DevBits acc, Xcsr;
+    u64 fl = 0;
+    int path = 0;
+    for (ReachOperand &o : ops) {
+        DevBits Y;
+        u64 f = 0;
+        // one operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does
+        const bool from_csr = frontier_product(F, o.m, ~0ULL, nops == 1 && !masked, Y, &f, &path);
+        if (o.rp.ns) {
+            // the repair gathers from F in bit form: a frontier still in CSR form is converted for it
+            if (from_csr && !Xcsr.valid()) bits_from_csr(F->dev, Xcsr);
+            ensure_devT(o.m);
+            bits_repair(from_csr ? Xcsr : F->bits, o.m->devT, o.rp, Y);
+        }
+        if (o.ddp) f += bits_apply_deltas(from_csr ? nullptr : &F->bits, from_csr ? &F->dev : nullptr, nullptr, o.ddp, Y);
+        fl += f;
+        if (nops == 1) { acc = std::move(Y); break; }
+        bits_naturalise(Y);
+        if (!acc.valid()) acc = std::move(Y);
+        else bits_or(acc, Y);
+    }
+    if (masked) {
+        bits_naturalise(acc);
+        ensure_bits(R);
+        bits_andnot(acc, R->bits);
+    }
+    cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
+    set_bits(F, std::move(acc));
+    if (cx.opt_sync_after_op) sync_stream();
+}
+
+// U = the union of every operand's effective pattern (m \ dm) u dp, built once with the flush kernels
+static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<ReachOperand> &ops, u64 n) {
+    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, n, n);
+    if (info) return info;
+    info = guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+        all.push_back(*U);
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        DevCSR S;
+        bool have = false;
+        for (ReachOperand &o : ops) {
+            ensure_dev(o.m);
+            DevCSR E;
+            const DevCSR *e = &o.m->dev;
+            if (o.dm) {
+                ensure_dev(o.dm);
+                if (o.dm->dev.nnz) { filter_by_mask(*e, o.dm->dev, true, true, E); e = &E; }
+            }
+            if (o.dp) {
+                ensure_dev(o.dp);
+                if (o.dp->dev.nnz) { DevCSR T; ewise_union(*e, o.dp->dev, false, T); E = std::move(T); e = &E; }
+            }
+            if (!have) { csr_copy(*e, S, false); have = true; }
+            else { DevCSR T; ewise_union(S, *e, false, T); S = std::move(T); }
+        }
+        set_dev(*U, std::move(S));
+        return GrB_SUCCESS;
+    });
+    if (info) GrB_Matrix_free(U);
+    return info;
+}
+
+static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
+                           const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources, int64_t *levels_out) {
+    const u64 n = m[0]->ncols;
+    std::vector<ReachOperand> ops(nops);
+    bool clean = nops == 1;
+    for (int t = 0; t < nops && clean; t++)
+        for (GrB_Matrix D : {dp ? dp[t] : nullptr, dm ? dm[t] : nullptr}) {
+            GrB_Index nv = 0;
+            if (!D) continue;
+            GrB_Info e = GrB_Matrix_nvals(&nv, D);
+            if (e) return e;
+            if (nv) clean = false;
+        }
+    GrB_Matrix U = nullptr;                      // the materialised union, when a level runs the row-wise calls
+    GrB_Info info = GrB_SUCCESS;
+    for (int t = 0; t < nops; t++) { ops[t].m = m[t]; ops[t].dp = dp ? dp[t] : nullptr; ops[t].dm = dm ? dm[t] : nullptr; }
+    const bool frontier = ctx().opt_bits_mode != 0 && bits_words_for(nsrc) != 0;
+    if (!clean && !frontier) info = reach_materialise(&U, ops, n);
+    else if (!clean) {
+        // per call: deltas' pending tuples finished, dm' and the repaired segments of m' (the base's mirror, built at commit)
+        info = guarded([&]() {
+            GpuLock g;
+            uvec<GrB_Matrix> all;
+            for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+            MultiLock lk(all.begin(), all.end());
+            ensure_init();
+            for (ReachOperand &o : ops) {
+                if (o.dp) { ensure_dev(o.dp); if (o.dp->dev.nnz) o.ddp = &o.dp->dev; }
+                if (!o.dm) continue;
+                ensure_dev(o.dm);
+                if (!o.dm->dev.nnz) continue;
+                ensure_devT(o.m);
+                bits_repair_plan(o.dm->dev, o.m->devT, o.rp);
+            }
+            return GrB_SUCCESS;
+        });
+    }
+    GrB_Matrix A = U ? U : m[0];                 // the operand of the row-wise calls
     GrB_Scalar one = nullptr;
     GrB_Matrix F = nullptr, R = nullptr;
-    GrB_Info info = GrB_Scalar_new(&one, GrB_BOOL);
+    if (!info) info = GrB_Scalar_new(&one, GrB_BOOL);
     if (!info) info = GrB_Scalar_setElement_BOOL(one, true);
     if (!info) info = GrB_Matrix_new(&F, GrB_BOOL, nsrc, n);
     if (!info) info = GrB_Matrix_new(&R, GrB_BOOL, nsrc, n);
@@ -2427,8 +2556,20 @@ GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Ind
         GrB_Index rn = 0, fn = 0;
         info = GrB_Matrix_nvals(&rn, R);
         if (info) break;
-        info = rn ? GrB_mxm(F, R, nullptr, GxB_ANY_PAIR_BOOL, F, A, GrB_DESC_RSC)
-                  : GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, A, nullptr);
+        if (!clean && !U) {
+            info = guarded([&]() {
+                GpuLock g;
+                uvec<GrB_Matrix> all = {F, R};
+                for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+                MultiLock lk(all.begin(), all.end());
+                ensure_init();
+                reach_hop(F, R, rn != 0, ops);
+                return GrB_SUCCESS;
+            });
+        } else {
+            info = rn ? GrB_mxm(F, R, nullptr, GxB_ANY_PAIR_BOOL, F, A, GrB_DESC_RSC)
+                      : GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, A, nullptr);
+        }
         if (!info) info = GrB_Matrix_nvals(&fn, F);
         if (info || fn == 0) break;
         info = GrB_Matrix_eWiseAdd_BinaryOp(R, nullptr, nullptr, GxB_ANY_BOOL, R, F, nullptr);
@@ -2436,10 +2577,43 @@ GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Ind
     }
     GrB_Scalar_free(&one);
     GrB_Matrix_free(&F);
+    GrB_Matrix_free(&U);
+    if (!clean) guarded([&]() { GpuLock g; ops.clear(); return GrB_SUCCESS; });   // the plans' device buffers go back to the pool
     if (info) { GrB_Matrix_free(&R); return info; }
     if (levels_out) *levels_out = level;
     *reached = R;
     return GrB_SUCCESS;
+}
+
+GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, GrB_Matrix A, int64_t max_hops,
+                          int include_sources, int64_t *levels_out) {
+    CHECK_PTR(reached); CHECK_MAT(A);
+    if (nsrc) CHECK_PTR(sources);
+    if (A->nrows != A->ncols) { tl_error = "reach_batch: A must be square"; return GrB_DIMENSION_MISMATCH; }
+    return reach_impl(reached, sources, nsrc, &A, nullptr, nullptr, 1, max_hops, include_sources, levels_out);
+}
+
+GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m,
+                                const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources,
+                                int64_t *levels_out) {
+    CHECK_PTR(reached); CHECK_PTR(m);
+    if (nsrc) CHECK_PTR(sources);
+    if (nops < 1) { tl_error = "reach_batch_delta: nops < 1"; return GrB_INVALID_VALUE; }
+    for (int t = 0; t < nops; t++) {
+        CHECK_MAT(m[t]);
+        if (dp && dp[t]) CHECK_MAT(dp[t]);
+        if (dm && dm[t]) CHECK_MAT(dm[t]);
+    }
+    const u64 n = m[0]->nrows;
+    for (int t = 0; t < nops; t++)
+        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
+            if (X && (X->nrows != n || X->ncols != n)) {
+                tl_error = "reach_batch_delta: operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+            }
+    if (is_huge(m[0])) { tl_error = "reach_batch_delta: host-resident operand"; return GrB_NOT_IMPLEMENTED; }
+    GrB_Info info = guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; });   // no device: fail before any host work
+    if (info) return info;
+    return reach_impl(reached, sources, nsrc, m, dp, dm, nops, max_hops, include_sources, levels_out);
 }
 
 // returns every cached device block to the driver (the caching allocator otherwise keeps freed blocks for reuse)

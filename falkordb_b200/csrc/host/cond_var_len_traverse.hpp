@@ -121,4 +121,36 @@ struct VarLenIter : VarLenIterT<TensorAdjacency> {
         : VarLenIterT<TensorAdjacency>(TensorAdjacency{&t}, min_hops, max_hops, reversed, bidirectional, dest_id, emit_path) {}
 };
 
+// The multiplicity-insensitive fast path of CondVarLenTraverse (emit_path off, a consumer that ignores multiplicity): row i of
+// the result holds the DISTINCT nodes the trail DFS reaches from starts[i] over every type in `types`, as one
+// B200_reach_batch_delta call over the tensors' (m, dp, dm) -- forward layers for Outgoing, the transpose mirror's for Incoming.
+// A shortest walk to v != s is a simple path and a shortest closed walk is a simple cycle, so both are trails and the sets agree.
+// min_hops = 0 adds the start itself; max_hops = UINT64_MAX is unbounded.  Both directions (s -> u -> s may reuse one edge) and
+// min_hops > 1 are refused: such a pattern keeps the DFS (VarLenIter).
+inline Matrix<bool> var_len_reach(const std::vector<const Tensor *> &types, EdgeDirection dir, const std::vector<uint64_t> &starts,
+                                  uint64_t min_hops, uint64_t max_hops) {
+    if (dir == EdgeDirection::Both) throw std::invalid_argument("var_len_reach: a bidirectional pattern is not a reach");
+    if (min_hops > 1) throw std::invalid_argument("var_len_reach: min_hops > 1 is not a reach");
+    if (types.empty()) throw std::invalid_argument("var_len_reach: no relationship type");
+    std::vector<GrB_Matrix> m, dp, dm;
+    for (const Tensor *t : types) {
+        if (dir == EdgeDirection::Outgoing) {
+            t->wait_fwd();
+            t->fwd_m().wait(); t->fwd_dp().wait(); t->fwd_dm().wait();
+            m.push_back(t->fwd_m().inner()); dp.push_back(t->fwd_dp().inner()); dm.push_back(t->fwd_dm().inner());
+        } else {
+            const VersionedMatrix &mt = t->matrix_t();
+            mt.wait();
+            mt.wait_all();
+            m.push_back(mt.m().inner()); dp.push_back(mt.dp().inner()); dm.push_back(mt.dm().inner());
+        }
+    }
+    GrB_Matrix raw = nullptr;
+    int64_t levels = 0;
+    grb_ok(B200_reach_batch_delta(&raw, starts.data(), starts.size(), m.data(), dp.data(), dm.data(), (int)types.size(),
+                                  max_hops > (uint64_t)INT64_MAX ? -1 : (int64_t)max_hops, min_hops == 0 ? 1 : 0, &levels),
+           "B200_reach_batch_delta");
+    return Matrix<bool>::adopt(raw, false);
+}
+
 } // namespace fdb

@@ -60,6 +60,17 @@ void bits_copy(const DevBits &X, DevBits &Y);
 // entries.  The left operand is the bit-matrix Xb, or the CSR Xc when Y came from bits_push_from_csr (Xb null).  dm / dp may be
 // null.  X and Y stay in the vertex order they are stored in.  Returns flops(X * dm) + flops(X * dp).
 u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y);
+// The exact dirty hop's deleted-edge term.  For every column j that dm touches, Y[j] = OR of X[k] over the in-edges k of m(:, j)
+// that are not in dm (Y = X * (m \ dm) on those columns; every other column of X * m is already exact).  The plan is built once
+// per operand and call: dmT = dm', and the repaired columns of m' (m's transpose mirror, natural column ids) cut into segments of
+// at most REPAIR_SEG in-edges; a column of several segments is zeroed and its segments merged with RED.OR.
+struct RepairPlan {
+    DevCSR dmT;                                        // row j = the deleted sources of column j, ascending
+    DevBuf<u32> s_col, s_len; DevBuf<u64> s_start;     // segment -> column, length | flags, first position in m'.col_idx
+    u64 ns = 0, ncols = 0, inedges = 0;                // segments, repaired columns, in-edges of m over them
+};
+void bits_repair_plan(const DevCSR &dm, const DevCSR &mT, RepairPlan &rp);
+void bits_repair(const DevBits &X, const DevCSR &mT, const RepairPlan &rp, DevBits &Y);
 
 // ewise.cu : search-based set algebra on sorted CSR rows
 void csr_copy(const DevCSR &A, DevCSR &out, bool keep_values);

@@ -443,12 +443,24 @@ def traverse_to_host(sources, A, hops, out_bitmap, sub_batches=None):
     return traverse_batch(sources, [A] * hops, OUT_BITMAP, out_bitmap=out_bitmap)[0]
 
 
-def reach_batch(sources, A, max_hops=None, include_sources=False):
-    """B200_reach_batch: `multi_source_reach` below as ONE C-ABI call (what a Rust operator would bind).  Returns (R, levels)."""
+def reach_batch(sources, A, max_hops=None, include_sources=False, deltas=None):
+    """B200_reach_batch: `multi_source_reach` below as ONE C-ABI call (what a Rust operator would bind).  Returns (R, levels).
+    `A` may also be a list of operands (the types of `-[:R1|R2*]->`), and `deltas` one (dp, dm) pair per operand (either may be
+    None): the walked operand is then the union of every (m \\ dm) u dp, exactly, through B200_reach_batch_delta."""
     sources = _u64arr(sources)
     h, lv = P(), I64()
-    check(lib().B200_reach_batch(C.byref(h), sources.ctypes.data, len(sources), A.h, -1 if max_hops is None else int(max_hops),
-                                 1 if include_sources else 0, C.byref(lv)))
+    hops = -1 if max_hops is None else int(max_hops)
+    if deltas is None and isinstance(A, Matrix):
+        check(lib().B200_reach_batch(C.byref(h), sources.ctypes.data, len(sources), A.h, hops, 1 if include_sources else 0,
+                                     C.byref(lv)))
+        return Matrix(0, 0, bool, _handle=h), lv.value
+    ms = [A] if isinstance(A, Matrix) else list(A)
+    n = len(ms)
+    deltas = [(None, None)] * n if deltas is None else list(deltas)
+    assert len(deltas) == n, "one (dp, dm) pair per operand"
+    arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
+    check(lib().B200_reach_batch_delta(C.byref(h), sources.ctypes.data, len(sources), arr(ms), arr([d[0] for d in deltas]),
+                                       arr([d[1] for d in deltas]), n, hops, 1 if include_sources else 0, C.byref(lv)))
     return Matrix(0, 0, bool, _handle=h), lv.value
 
 

@@ -354,6 +354,14 @@ GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, con
  * zero-length walk.  Levels are F<!R,replace,struct> = F*A then R = R u F, in device frontier form; *levels_out = levels run. */
 GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, GrB_Matrix A, int64_t max_hops,
                           int include_sources, int64_t *levels_out);
+/* B200_reach_batch over relationship tensors with pending writes: the walked operand is A = U_t (m[t] \ dm[t]) u dp[t], pattern
+ * only (m / dp may be UINT64, dm BOOL; where dp and dm hold the same entry dp wins; dm entries outside m have no effect).  Exact:
+ * a vertex stays reachable while any remaining edge reaches it (no delta_lmxm over-masking).  dp / dm may be NULL arrays or hold
+ * NULL entries.  Every operand and delta is square of one size n (else GrB_DIMENSION_MISMATCH); nops < 1 is GrB_INVALID_VALUE;
+ * host-resident operands are GrB_NOT_IMPLEMENTED.  One operand without deltas runs exactly B200_reach_batch. */
+GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m,
+                                const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources,
+                                int64_t *levels_out);
 GrB_Info B200_sync(void);
 GrB_Info B200_pool_trim(void); /* hand the caching allocator's free device blocks back to the driver */
 void *B200_stream(void); /* the cudaStream_t every kernel of this library is launched on */
@@ -362,7 +370,7 @@ uint64_t B200_get_stat(const char *name);
 void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
- * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta".  0 on success. */
+ * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
