@@ -551,16 +551,28 @@ k_bits_push(const u32 *__restrict__ act, const u64 *__restrict__ cum, const u64 
 // Early hops of a traversal batch have a tiny frontier (F in CSR form, a few thousand entries).  Going through the
 // bit-matrix there means O(n*W) passes that dwarf the real work (zeroing X, scanning it for flops / active vertices,
 // compacting n flags); this path expands F's entries directly: entry (i, k) ORs bit i into Y[j] for every j in A(k,:).
+// seen (optional, zeroed, one bit per column of F): *edges += deg(k) over the DISTINCT columns k of F, the edges the bit-matrix
+// hop would walk -- the quantity its direction switch compares with nnz(A).
 __global__ void k_csr_entry_info(const u64 *__restrict__ Fp, const u32 *__restrict__ Fj, u64 nrows, const u64 *__restrict__ Ap,
-                                 u32 *__restrict__ erow, u64 *__restrict__ edeg) {
+                                 u32 *__restrict__ erow, u64 *__restrict__ edeg, u32 *__restrict__ seen, u64 *__restrict__ edges) {
     u64 warp = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     u32 lane = threadIdx.x & 31;
     if (warp >= nrows) return;
+    u64 ed = 0;
     for (u64 q = Fp[warp] + lane; q < Fp[warp + 1]; q += 32) {
         u32 k = Fj[q];
         erow[q] = (u32)warp;
-        edeg[q] = Ap[k + 1] - Ap[k];
+        const u64 d = Ap[k + 1] - Ap[k];
+        edeg[q] = d;
+        if (seen) {
+            const u32 bit = 1u << (k & 31);
+            if (!(atomicOr(seen + (k >> 5), bit) & bit)) ed += d;    // the first entry to claim column k counts its degree
+        }
     }
+    if (!seen) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ed += __shfl_xor_sync(0xffffffffu, ed, o);
+    if (lane == 0 && ed) atomicAdd((unsigned long long *)edges, ed);
 }
 // ANDNOT (the dirty hop's deleted-edge term, bits_apply_deltas) clears bit i instead of setting it
 template <int W, bool ANDNOT>
@@ -584,7 +596,9 @@ k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *
             while (e < e1 && cum[e + 1] <= t) e++;
             const u32 i = erow[e];
             u32 col = Aj[Ap[Fj[e]] + (t - cum[e])];
-            if (perm) col = __ldg(perm + col);          // hot-set order: hubs of the next gather become neighbours (64 MB table, L2)
+            // hot-set order through the table (the deltas, which have no relabelled copy); a prepared operand passes its
+            // relabelled col_idx (PullTables::ap) as Aj instead, with perm null
+            if (perm) col = __ldg(perm + col);
             unsigned long long *dst = (unsigned long long *)&Y[(u64)col * W + (i >> 6)];
             if (ANDNOT) atomicAnd(dst, ~(1ULL << (i & 63)));
             else atomicOr(dst, 1ULL << (i & 63));
@@ -592,46 +606,72 @@ k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *
     }
 }
 template <int W>
-static void csr_push_impl(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 flops, const u32 *erow, const u64 *cum, const u32 *perm) {
+static void csr_push_impl(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBits &Y, u64 flops, const u32 *erow, const u64 *cum,
+                          const u32 *perm) {
     u64 nchunks = (flops + PUSH_CHUNK - 1) / PUSH_CHUNK;
     TimedScope ts(TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops);
-    LAUNCH((k_csr_push<W, false>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, A.j.ptr, Y.w.ptr, perm);
+    LAUNCH((k_csr_push<W, false>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, Aj, Y.w.ptr, perm);
 }
-// Y = F * A from the CSR form of F.  Returns false (nothing done) when the expansion is large enough that the
-// direction-optimising bit-matrix hop should take it: flops * 4 > nnz(A), the same switch bits_hop applies to edges.
+// Whether the push straight from F's CSR entries beats the bit-matrix hop.  edges = the out-degrees summed over the DISTINCT
+// columns of F (what the bit-matrix hop walks), flops = over all its entries (one RED each for the CSR push).
+//  * edges * 4 > nnz(A): no -- the bit-matrix hop pulls these frontiers.
+//  * below that the bit-matrix hop pushes too.  It first spends O(n * W) passes that build, count and compact its frontier (and
+//    the next hop packs its natural-order result), then merges the rows that share a column into one RED per word.  So the CSR
+//    push wins while its extra REDs, flops - edges, cost less than those passes.  Measured with scripts/push_gate.py on RMAT-24
+//    (H100 80GB HBM3, 400 W limit; hops 2 + 3 timed; frontiers of 512 and 1,024 rows that repeat hubs 2 to 14 times): the
+//    crossover sits at flops - edges = 0.55, 0.61, 0.70 * n * W at W = 8 and 0.44, 0.48, 0.54 * n * W at W = 16 (edges 15, 30,
+//    60 M).  The bound is n * W / 2: it picks the slower route by at most 0.7 ms of the 4 to 22 ms those hops took.  The bench's
+//    hop-2 frontiers (W = 8) sit at 0.35 to 0.42.
+//  * flops * 4 <= nnz(A) is always taken (it implies the edges bound), as before the bound existed: at W >= 8 that region lies
+//    inside the bound; at W = 1 (64 rows: crossover 1.7 to 1.9 * n * W at 15 and 30 M edges, below 2.5 at 60 M) it keeps some
+//    frontiers that the bit-matrix hop would take up to 0.4 ms faster.
+static bool csr_push_wins(u64 flops, u64 edges, u64 n, u32 W, u64 nnzA) {
+    if (flops * 4 <= nnzA) return true;
+    return edges * 4 <= nnzA && (flops - edges) * 2 <= n * W;
+}
+// Y = F * A from the CSR form of F.  Returns false (nothing done) when the bit-matrix hop should take it (csr_push_wins), unless
+// csr_push = 2.
 bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt) {
     if (F.ncols != A.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
     const u32 W = bits_words_for(F.nrows);
-    u64 flops = 0;
+    u64 flops = 0, edges = 0;
     DevBuf<u32> erow(F.nnz);
-    DevBuf<u64> cum(F.nnz + 1);
+    DevBuf<u64> cum(F.nnz + 2);                  // per-entry degrees -> their prefix sums; [nnz] = flops, [nnz + 1] = edges
     if (F.nnz) {
-        LAUNCH(k_csr_entry_info, grid_for(F.nrows * 32, 256), 256, 0, F.p.ptr, F.j.ptr, F.nrows, A.p.ptr, erow.ptr, cum.ptr);
-        CUDA_TRY(cudaMemsetAsync(cum.ptr + F.nnz, 0, sizeof(u64), stream()));
+        DevBuf<u32> seen((F.ncols + 31) / 32);
+        seen.zero();
+        CUDA_TRY(cudaMemsetAsync(cum.ptr + F.nnz, 0, 2 * sizeof(u64), stream()));
+        LAUNCH(k_csr_entry_info, grid_for(F.nrows * 32, 256), 256, 0, F.p.ptr, F.j.ptr, F.nrows, A.p.ptr, erow.ptr, cum.ptr, seen.ptr,
+               cum.ptr + F.nnz + 1);
         exclusive_scan_u64(cum.ptr, cum.ptr, F.nnz + 1);
-        flops = read_scalar(cum.ptr + F.nnz);
+        u64 h[2];
+        d2h(h, cum.ptr + F.nnz, 2);
+        sync_stream();
+        flops = h[0]; edges = h[1];
     }
-    if (flops * 4 > A.nnz) return false;
+    if (ctx().opt_csr_push != 2 && !csr_push_wins(flops, edges, A.nrows, W, A.nnz)) return false;
     Y.clear();
     Y.nrows = F.nrows; Y.ncols = A.ncols; Y.W = W;
     Y.w.alloc(A.ncols * W);
     Y.w.zero();
     if (flops_out) *flops_out = flops;
-    // a square operand with pull tables: write the result in its hot-set order, the form the next pull gathers from directly
-    const u32 *perm = nullptr;
+    // a square operand with pull tables: write the result in its hot-set order, the form the next pull gathers from directly --
+    // through the operand's relabelled col_idx when the tables have it, else through pperm per flop
+    const u32 *perm = nullptr, *Aj = A.j.ptr;
     if (pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
-        perm = pt->pperm->ptr;
+        if (pt->ap.ptr && pt->ap.n == A.nnz) Aj = pt->ap.ptr;
+        else perm = pt->pperm->ptr;
         Y.pvert = pt->pvert;
         Y.pperm = pt->pperm;
         Y.perm_tag = pt->perm_tag;
     }
     if (flops == 0) return true;
     switch (W) {
-    case 1: csr_push_impl<1>(F, A, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 2: csr_push_impl<2>(F, A, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 4: csr_push_impl<4>(F, A, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 8: csr_push_impl<8>(F, A, Y, flops, erow.ptr, cum.ptr, perm); break;
-    default: csr_push_impl<16>(F, A, Y, flops, erow.ptr, cum.ptr, perm); break;
+    case 1: csr_push_impl<1>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
+    case 2: csr_push_impl<2>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
+    case 4: csr_push_impl<4>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
+    case 8: csr_push_impl<8>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
+    default: csr_push_impl<16>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
     }
     return true;
 }
@@ -1061,7 +1101,7 @@ k_ordered_flops(const u32 *__restrict__ hdeg, u64 n1, const u64 *__restrict__ Xp
 
 static void build_hot_pack(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     u64 n = A.nrows;
-    pt.vert.release(); pt.jp.release(); pt.slot.release(); pt.hdeg.release(); pt.n1 = 0; pt.packed = false;
+    pt.vert.release(); pt.jp.release(); pt.ap.release(); pt.slot.release(); pt.hdeg.release(); pt.n1 = 0; pt.packed = false;
     if (n == 0 || AT.nnz == 0 || n >= 0xFFFFFFFFULL) return;
     DevBuf<u64> keys(n), cnt(1);
     cnt.zero();
@@ -1083,13 +1123,20 @@ static void build_hot_pack(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
 }
 
 // The pull tables of one matrix, built once per immutable base (B200_Matrix_prepare, or the first hop that pulls): the hot-set order
-// when hot_pack is on, A'.col_idx relabelled to it, and the segment list.  Turning hot_pack on after the tables were built without
-// it adds the order and the relabelled col_idx.
+// when hot_pack is on, A'.col_idx and A.col_idx relabelled to it, and the segment list.  Turning hot_pack on after the tables
+// were built without it adds the order and both relabelled col_idx arrays.
 static void build_pull_tables(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     if (!pt.packed && ctx().opt_hot_pack) build_hot_pack(A, AT, pt);
     if (pt.packed && !pt.jp.ptr) {
         pt.jp.alloc(AT.nnz);
         LAUNCH(k_relabel_cols, grid_for(AT.nnz, 256, (u64)ctx().num_sms * 32), 256, 0, AT.j.ptr, AT.nnz, pt.slot.ptr, pt.jp.ptr);
+    }
+    // the CSR push's operand: A.col_idx already in the order it writes Y (4 * nnz(A) bytes), so a pushed flop needs no
+    // dependent pperm[col] read from a table larger than L2.  Only when perm_push can read it; turning perm_push on later adds
+    // it at the next build (until then the push reads pperm[col])
+    if (pt.packed && !pt.ap.ptr && ctx().opt_perm_push && A.nnz && A.nrows == A.ncols) {
+        pt.ap.alloc(A.nnz);
+        LAUNCH(k_relabel_cols, grid_for(A.nnz, 256, (u64)ctx().num_sms * 32), 256, 0, A.j.ptr, A.nnz, pt.pperm->ptr, pt.ap.ptr);
     }
     if (!pt.built) {
         build_seg_list(AT, pt);
@@ -1346,13 +1393,15 @@ static void bits_delta_impl(const DevBits &X, const DevCSR &D, int op, DevBits &
 }
 
 // The first hop: F is still a CSR of <= 1024 rows and Y came from bits_push_from_csr.  Entry (i, k) of F walks delta row k and
-// applies bit i to Y[pos(j)] -- k_csr_push with the delta as its operand.  Returns flops(F * D).
+// applies bit i to Y[pos(j)] -- k_csr_push with the delta as its operand, through pperm per flop (a delta has no relabelled
+// copy of its col_idx).  Returns flops(F * D).
 template <int W>
 static u64 csr_delta_impl(const DevCSR &F, const DevCSR &D, int op, DevBits &Y) {
     if (!F.nnz || !D.nnz) return 0;
     DevBuf<u32> erow(F.nnz);
     DevBuf<u64> cum(F.nnz + 1);
-    LAUNCH(k_csr_entry_info, grid_for(F.nrows * 32, 256), 256, 0, F.p.ptr, F.j.ptr, F.nrows, D.p.ptr, erow.ptr, cum.ptr);
+    LAUNCH(k_csr_entry_info, grid_for(F.nrows * 32, 256), 256, 0, F.p.ptr, F.j.ptr, F.nrows, D.p.ptr, erow.ptr, cum.ptr,
+           (u32 *)nullptr, (u64 *)nullptr);
     CUDA_TRY(cudaMemsetAsync(cum.ptr + F.nnz, 0, sizeof(u64), stream()));
     exclusive_scan_u64(cum.ptr, cum.ptr, F.nnz + 1);
     const u64 flops = read_scalar(cum.ptr + F.nnz);

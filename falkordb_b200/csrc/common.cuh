@@ -61,7 +61,7 @@ struct Context {
     i64 opt_hot_bytes = 64 << 20;  // size of that hot prefix
     i64 opt_hot_pack = 1;          // gather through the degree-sorted, sink-free relabelling of the frontier
     i64 opt_fused_prep = 1;        // pull hops: pack the frontier, count flops / edges and OR it in one pass
-    i64 opt_csr_push = 1;          // tiny CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes)
+    i64 opt_csr_push = 1;          // small CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes); 2 = whatever their size (measurement)
     i64 opt_diag_filter = 1;       // frontier-form mxm by a diagonal (label) matrix runs as an elementwise column filter
     i64 opt_pull_grid = 0;         // CTAs per SM of the segment pull kernel (0 = occupancy: one resident wave)
 };

@@ -1027,16 +1027,16 @@ static bool bits_legal(GrB_Matrix C, GrB_Matrix M, GrB_Matrix A, GrB_Matrix B, c
 }
 
 // Y = A*B through the frontier dispatch: the push straight from A's entries while A is still a small CSR, the diagonal filter, or
-// the direction-optimising push / pull.  known_flops: flops(A*B) when already counted (~0 otherwise); pt_ok: the CSR push may
-// write Y in B's hot-set order.  Returns true when Y came from A's CSR form (A then has no bit form).
-static bool frontier_product(GrB_Matrix A, GrB_Matrix B, u64 known_flops, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
+// the direction-optimising push / pull.  pt_ok: the CSR push may write Y in B's hot-set order.  Returns true when Y came from
+// A's CSR form (A then has no bit form).
+static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
     Context &cx = ctx();
     ensure_dev(B);
     if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
-    // a frontier that is still a (small) CSR expands straight from its entries; large expansions decline
-    // (only worth probing for a small CSR: its preparation is O(nnz(F)); an expansion already known to be large skips it)
+    // a frontier that is still a (small) CSR expands straight from its entries unless it touches enough of B that the pull
+    // should take it (only worth probing for a small CSR: the probe is O(nnz(F)))
     const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
-                          A->dev.nnz <= ((u64)1 << 20) && (known_flops == ~0ULL || known_flops * 4 <= B->dev.nnz) &&
+                          A->dev.nnz <= ((u64)1 << 20) &&
                           !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, fl, (B->devT_valid && pt_ok) ? &B->pt : (const PullTables *)nullptr);
     if (from_csr) { *path = 7; return true; }
     if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
@@ -1057,22 +1057,19 @@ static bool frontier_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_Matrix A, GrB_Matrix
     Context &cx = ctx();
     if (accum || d.t0 || d.t1 || cx.opt_bits_mode == 0 || !bits_legal(C, Mask, A, B, d)) return false;
     bool use_bits = (cx.opt_bits_mode == 1);
-    u64 known_flops = ~0ULL;
     finish_pending(A);
     if (!use_bits) {
         if (A->bits_valid && !A->dev_valid && !A->host_valid) use_bits = true; // stay in frontier form mid-chain
         else {
             ensure_dev(A); ensure_dev(B);
-            u64 fl = spgemm_flops(A->dev, B->dev);
-            known_flops = fl;
-            use_bits = fl >= (u64)cx.opt_bits_min_flops;
+            use_bits = spgemm_flops(A->dev, B->dev) >= (u64)cx.opt_bits_min_flops;
         }
     }
     if (!use_bits) return false;
     DevBits Y;
     u64 fl = 0;
     int path = 0;
-    const bool from_csr = frontier_product(A, B, known_flops, !Mask, Y, &fl, &path);
+    const bool from_csr = frontier_product(A, B, !Mask, Y, &fl, &path);
     if (Mask) {
         ensure_bits(Mask);
         bits_andnot(Y, Mask->bits);
@@ -2442,7 +2439,7 @@ static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<Reach
         DevBits Y;
         u64 f = 0;
         // one operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does
-        const bool from_csr = frontier_product(F, o.m, ~0ULL, nops == 1 && !masked, Y, &f, &path);
+        const bool from_csr = frontier_product(F, o.m, nops == 1 && !masked, Y, &f, &path);
         if (o.rp.ns) {
             // the repair gathers from F in bit form: a frontier still in CSR form is converted for it
             if (from_csr && !Xcsr.valid()) bits_from_csr(F->dev, Xcsr);

@@ -24,8 +24,9 @@ u32 bits_words_for(u64 nrows);
 void bits_from_csr(const DevCSR &F, DevBits &X);
 void bits_to_csr(const DevBits &X, DevCSR &C);
 u64 bits_nvals(const DevBits &X);
-// Y = F * A expanded straight from F's CSR (tiny frontiers); false = too much work for this path, nothing was done
-// pt (optional): A's pull tables; when they carry a vertex order the result is written in it (permuted form)
+// Y = F * A expanded straight from F's CSR (small frontiers); false = the frontier touches enough of A that the pull should take
+// it (edges * 4 > nnz(A)), nothing was done.  pt (optional): A's pull tables; when they carry a vertex order the result is
+// written in it (permuted form)
 bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr);
 void bits_naturalise(DevBits &X);                                // permuted form -> natural vertex order (no-op when natural)
 bool csr_is_diagonal(const DevCSR &A);                          // square, every entry (i,i)
@@ -38,13 +39,14 @@ struct PullTables {   // per-matrix tables of the pull direction, cached with th
     // the same order extended to ALL vertices (sinks follow the n1 slots, by id): a frontier stored in it needs no packing pass
     std::shared_ptr<DevBuf<u32>> pvert, pperm; u64 perm_tag = 0;    // pvert[position] = vertex, pperm[vertex] = position
     DevBuf<u32> jp;                                    // col_idx of A' relabelled to hot-set slots (when packed)
+    DevBuf<u32> ap;                                    // col_idx of A relabelled to positions (pperm[A.j], when packed): the CSR push's operand
     // segment list: rows of A' longer than SMALL_ROW -- whole rows up to LONG_ROW entries, LONG_ROW-entry segments of longer ones --
     // longest first; bit 31 of s_len marks a segment of a long row (merged with RED.OR)
     DevBuf<u32> s_row, s_len; DevBuf<u64> s_start; u64 ns = 0;
     bool built = false;                                // the segment list is built
     void clear() {
         vert.release(); slot.release(); hdeg.release(); n1 = 0; packed = false; pvert.reset(); pperm.reset(); perm_tag = 0;
-        jp.release();
+        jp.release(); ap.release();
         s_row.release(); s_len.release(); s_start.release(); ns = 0;
         built = false;
     }
