@@ -89,6 +89,9 @@ def lib():
         "B200_traverse_batch_delta": [P, U64, P, P, P, C.c_int, C.c_int, P, U64, P, P, U64, C.POINTER(U64), C.POINTER(U64),
                                       C.POINTER(C.c_int)],
         "B200_Matrix_delta_lmxm": [P, P, P, P],
+        "B200_Matrix_union_lmxm": [P, P, P, P, C.c_int],
+        "B200_traverse_batch_union": [P, U64, P, P, C.c_int, P, P, P, C.c_int, P, U64, P, P, U64, C.POINTER(U64), C.POINTER(U64),
+                                      C.POINTER(C.c_int)],
         "B200_set_option": [C.c_char_p, I64],
         "B200_Matrix_extract_pairs": [P, P, P, U64, P, P],
         "B200_Matrix_rmat_block": [C.POINTER(P), C.c_int, U64, U64, U64, U64, C.c_int],

@@ -27,6 +27,11 @@ static const u64 PUSH_CHUNK = 8192;
 static const u64 LONG_ROW = 4096;   // pull: rows longer than this are split into LONG_ROW-entry segments
 
 static void require_natural(const DevBits &X, const char *what);
+// accumulate mode (union hops): the product is ORed into Y, which must already hold a natural-order product of the same shape
+static void require_acc_target(const DevBits &Y, u64 nrows, u64 ncols, u32 W) {
+    require_natural(Y, "accumulating product");
+    if (Y.nrows != nrows || Y.ncols != ncols || Y.W != W) throw GrbError(-6, "accumulating product: target shape differs");
+}
 
 u32 bits_words_for(u64 nrows) {
     if (nrows == 0) return 1;
@@ -607,9 +612,10 @@ k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *
 }
 template <int W>
 static void csr_push_impl(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBits &Y, u64 flops, const u32 *erow, const u64 *cum,
-                          const u32 *perm) {
+                          const u32 *perm, bool acc) {
     u64 nchunks = (flops + PUSH_CHUNK - 1) / PUSH_CHUNK;
-    TimedScope ts(TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops);
+    // col_idx + per-entry (row, column, cum) + one RED per flop; the same bytes when accumulating ("bits_push_acc")
+    TimedScope ts(acc ? TK_BITS_PUSH_ACC : TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops);
     LAUNCH((k_csr_push<W, false>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, Aj, Y.w.ptr, perm);
 }
 // Whether the push straight from F's CSR entries beats the bit-matrix hop.  edges = the out-degrees summed over the DISTINCT
@@ -630,10 +636,11 @@ static bool csr_push_wins(u64 flops, u64 edges, u64 n, u32 W, u64 nnzA) {
     return edges * 4 <= nnzA && (flops - edges) * 2 <= n * W;
 }
 // Y = F * A from the CSR form of F.  Returns false (nothing done) when the bit-matrix hop should take it (csr_push_wins), unless
-// csr_push = 2.
-bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt) {
+// csr_push = 2.  acc: Y |= F * A into a natural-order Y of the product's shape (no zeroing, no vertex order).
+bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt, bool acc) {
     if (F.ncols != A.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
     const u32 W = bits_words_for(F.nrows);
+    if (acc) require_acc_target(Y, F.nrows, A.ncols, W);
     u64 flops = 0, edges = 0;
     DevBuf<u32> erow(F.nnz);
     DevBuf<u64> cum(F.nnz + 2);                  // per-entry degrees -> their prefix sums; [nnz] = flops, [nnz + 1] = edges
@@ -650,15 +657,17 @@ bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops
         flops = h[0]; edges = h[1];
     }
     if (ctx().opt_csr_push != 2 && !csr_push_wins(flops, edges, A.nrows, W, A.nnz)) return false;
-    Y.clear();
-    Y.nrows = F.nrows; Y.ncols = A.ncols; Y.W = W;
-    Y.w.alloc(A.ncols * W);
-    Y.w.zero();
+    if (!acc) {
+        Y.clear();
+        Y.nrows = F.nrows; Y.ncols = A.ncols; Y.W = W;
+        Y.w.alloc(A.ncols * W);
+        Y.w.zero();
+    }
     if (flops_out) *flops_out = flops;
     // a square operand with pull tables: write the result in its hot-set order, the form the next pull gathers from directly --
     // through the operand's relabelled col_idx when the tables have it, else through pperm per flop
     const u32 *perm = nullptr, *Aj = A.j.ptr;
-    if (pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
+    if (!acc && pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
         if (pt->ap.ptr && pt->ap.n == A.nnz) Aj = pt->ap.ptr;
         else perm = pt->pperm->ptr;
         Y.pvert = pt->pvert;
@@ -667,11 +676,11 @@ bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops
     }
     if (flops == 0) return true;
     switch (W) {
-    case 1: csr_push_impl<1>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 2: csr_push_impl<2>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 4: csr_push_impl<4>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
-    case 8: csr_push_impl<8>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
-    default: csr_push_impl<16>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm); break;
+    case 1: csr_push_impl<1>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
+    case 2: csr_push_impl<2>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
+    case 4: csr_push_impl<4>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
+    case 8: csr_push_impl<8>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
+    default: csr_push_impl<16>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
     }
     return true;
 }
@@ -758,6 +767,22 @@ template <int W> __device__ __forceinline__ void store_row(u64 *dst, const u64 (
     }
 }
 template <int WL> __device__ __forceinline__ void store_part(u64 *dst, const u64 (&acc)[WL]) { store_row<WL>(dst, acc); }
+// accumulate mode (union hops): dst |= acc, skipped when acc is empty.  Each record is owned by one lane (k_pull_small) or one
+// 8-lane group (a mid row of k_pull_seg), so a plain read-modify-write is race-free
+template <int WL> __device__ __forceinline__ void or_part(u64 *dst, u64 (&acc)[WL]) {
+    u64 any = 0;
+#pragma unroll
+    for (int w = 0; w < WL; w++) any |= acc[w];
+    if (!any) return;
+    if constexpr (WL == 1) { dst[0] |= acc[0]; }
+    else {
+#pragma unroll
+        for (int w2 = 0; w2 < WL / 2; w2++) {
+            ulonglong2 v = reinterpret_cast<const ulonglong2 *>(dst)[w2];
+            reinterpret_cast<ulonglong2 *>(dst)[w2] = make_ulonglong2(v.x | acc[2 * w2], v.y | acc[2 * w2 + 1]);
+        }
+    }
+}
 
 static const u32 SEG_ATOMIC = 0x80000000u;
 
@@ -829,8 +854,9 @@ static void build_seg_list(const DevCSR &AT, PullTables &pt) {
 // one lane per row, natural order: rows of <= SMALL_ROW entries are finished here, rows longer than LONG_ROW are zero-filled
 // (their segments arrive through RED.OR), everything in between is left to k_pull_seg.  This kernel is latency-bound, not
 // L1TEX-bound: splitting the record across lanes as k_pull_seg does would divide the bytes each warp keeps in flight, so one lane
-// owns the whole record here.
-template <int W, bool HINTS>
+// owns the whole record here.  ACC (union hops): Y already holds earlier operands' products; small rows are ORed into it and long
+// rows are left as they are.
+template <int W, bool HINTS, bool ACC>
 __global__ void __launch_bounds__(256)
 k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
              u64 *__restrict__ Y, u32 hot_bytes, u32 tot_bytes) {
@@ -865,7 +891,8 @@ k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, co
                     if (k[u] != 0xFFFFFFFFu) or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
             }
         }
-        if (e - s <= SMALL_ROW || e - s > LONG_ROW) store_row<W>(Y + j * W, acc);
+        if (ACC) { if (e - s <= SMALL_ROW) or_part<W>(Y + j * W, acc); }
+        else if (e - s <= SMALL_ROW || e - s > LONG_ROW) store_row<W>(Y + j * W, acc);
 #pragma unroll
         for (int u = 0; u < 4; u++) k[u] = kn[u];
         s = s1; e = e1; s1 = s2; e1 = e2;
@@ -875,8 +902,9 @@ k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, co
 // 8 lanes per list entry (a mid row, or one LONG_ROW-entry segment of a long row); entries sorted by length, descending.
 // Three-stage software pipeline: list entry two steps ahead, col_idx batch one step ahead, gathers now.  Step t of group g
 // handles list entry t * ngroups + g on even steps and t * ngroups + (ngroups - 1 - g) on odd ones, which evens out the totals per
-// group.  The 8 lanes cover VG vertices x SPLIT record parts per unroll step.
-template <int W, bool HINTS, int U, bool EARLY>
+// group.  The 8 lanes cover VG vertices x SPLIT record parts per unroll step.  ACC (union hops): a mid row is ORed into the stored
+// record instead of replacing it (long-row segments merge with RED.OR either way).
+template <int W, bool HINTS, int U, bool EARLY, bool ACC>
 __global__ void __launch_bounds__(256)
 k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const u32 *__restrict__ s_len, u64 ns,
            const u32 *__restrict__ ATj, const u64 *__restrict__ X, u64 *__restrict__ Y, const u64 *__restrict__ Gp,
@@ -963,7 +991,8 @@ k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const
             if (s_len[i] & SEG_ATOMIC) {
 #pragma unroll
                 for (int w = 0; w < WL; w++) if (acc[w]) atomicOr((unsigned long long *)(dst + w), acc[w]);
-            } else store_part<WL>(dst, acc);
+            } else if (ACC) or_part<WL>(dst, acc);
+            else store_part<WL>(dst, acc);
         }
         s0 = s1; e0 = e1; s1 = s2; e1 = e2;
     }
@@ -1147,11 +1176,11 @@ static void build_pull_tables(const DevCSR &A, const DevCSR &AT, PullTables &pt)
 // k_pull_small over every row of A', then k_pull_seg over the segment list.  The segment kernel's grid is every CTA resident at
 // once (occupancy x SMs) unless pull_grid overrides it: entries are dealt round-robin to 8-lane groups, so one full wave keeps all
 // SMs busy to the end.
-template <int W, bool HINTS>
+template <int W, bool HINTS, bool ACC>
 static void launch_pull(const DevCSR &AT, const PullTables &pt, u64 m, const u32 *gj, const u64 *gx, u64 *Y, const u64 *Gp,
                         u32 hot_bytes, u32 tot_bytes) {
     Context &cx = ctx();
-    LAUNCH((k_pull_small<W, HINTS>), grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT.p.ptr, gj, m, gx, Y, hot_bytes, tot_bytes);
+    LAUNCH((k_pull_small<W, HINTS, ACC>), grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT.p.ptr, gj, m, gx, Y, hot_bytes, tot_bytes);
     if (!pt.ns) return;
     auto seg = [&](auto kern) {
         int per_sm = 0;
@@ -1161,13 +1190,13 @@ static void launch_pull(const DevCSR &AT, const PullTables &pt, u64 m, const u32
         LAUNCH(kern, (u32)cx.num_sms * (u32)per_sm, 256, 0, pt.s_row.ptr, pt.s_start.ptr, pt.s_len.ptr, pt.ns, gj, gx, Y, Gp, hot_bytes,
                tot_bytes);
     };
-    if (Gp) seg(k_pull_seg<W, HINTS, 4, true>);
-    else seg(k_pull_seg<W, HINTS, 4, false>);
+    if (Gp) seg(k_pull_seg<W, HINTS, 4, true, ACC>);
+    else seg(k_pull_seg<W, HINTS, 4, false, ACC>);
 }
 
 template <int W>
 static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y,
-                     u64 *flops_out, int *path_out) {
+                     u64 *flops_out, int *path_out, bool acc) {
     Context &cx = ctx();
     u64 n = A.nrows, m = A.ncols;
     // X in permuted form: usable as it stands only by the pull through the tables it was ordered for; anything else works on a
@@ -1178,9 +1207,11 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
     const DevBits *Xuse = &Xin;
     if (Xin.permuted() && !ordered) { bits_copy(Xin, Xnat); bits_naturalise(Xnat); Xuse = &Xnat; }
     const DevBits &X = *Xuse;
-    Y.clear();
-    Y.nrows = X.nrows; Y.ncols = m; Y.W = W;
-    Y.w.alloc(m * W);
+    if (!acc) {
+        Y.clear();
+        Y.nrows = X.nrows; Y.ncols = m; Y.W = W;
+        Y.w.alloc(m * W);
+    }
     DevBuf<u32> flag(n + 1);
     DevBuf<u64> st(2);
     st.zero();
@@ -1210,12 +1241,12 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
         else if (cx.opt_pull_mode == 0) pull = false;
         else pull = edges * 4 > A.nnz; // direction switch: frontier touches > 1/4 of the edges
     }
-    if (edges == 0) { Y.w.zero(); if (path_out) *path_out = 0; return; }
+    if (edges == 0) { if (!acc) Y.w.zero(); if (path_out) *path_out = 0; return; }
     if (ordered && !pull) {                     // the push direction works on natural order: undo the frontier's order and start over
         DevBits Xn;
         bits_copy(Xin, Xn);
         bits_naturalise(Xn);
-        hop_impl<W>(Xn, A, AT, pt, Y, flops_out, path_out);
+        hop_impl<W>(Xn, A, AT, pt, Y, flops_out, path_out, acc);
         return;
     }
     if (!pull) {
@@ -1224,7 +1255,7 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
             st2.zero();
             LAUNCH(k_bits_flops, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, X.w.ptr, (u32)W, n, A.p.ptr, flag.ptr, st2.ptr);
         }
-        Y.w.zero();
+        if (!acc) Y.w.zero();                   // accumulate: the REDs OR into the earlier operands' product
         CUDA_TRY(cudaMemsetAsync(flag.ptr + n, 0, sizeof(u32), stream()));
         DevBuf<u64> pos(n + 1);
         exclusive_scan_u32_to_u64(flag.ptr, pos.ptr, n + 1);
@@ -1236,8 +1267,8 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
         exclusive_scan_u64(cum.ptr, cum.ptr, nact + 1);
         u64 nchunks = (edges + PUSH_CHUNK - 1) / PUSH_CHUNK;
         {
-            // col_idx segments + per-active (id,cum,start) + X words + one RED per (edge, word)
-            TimedScope ts(TK_BITS_PUSH, 4 * edges + 20 * nact + 8ULL * W * nact + 8ULL * W * edges);
+            // col_idx segments + per-active (id,cum,start) + X words + one RED per (edge, word); the same bytes when accumulating
+            TimedScope ts(acc ? TK_BITS_PUSH_ACC : TK_BITS_PUSH, 4 * edges + 20 * nact + 8ULL * W * nact + 8ULL * W * edges);
             LAUNCH((k_bits_push<W>), (u32)nchunks, 256, 0, act.ptr, cum.ptr, astart.ptr, nact, edges, A.j.ptr, X.w.ptr, Y.w.ptr);
         }
         if (path_out) *path_out = 2;
@@ -1269,13 +1300,18 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
         Gp = Gd.ptr;
     }
     {
-        // compulsory traffic: stream A' col_idx + rowptr, read X once, write Y once (X gathers hit L2)
-        TimedScope ts(TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + 8ULL * W * m);
+        // compulsory traffic: stream A' col_idx + rowptr, read X once, write Y once (X gathers hit L2).  Accumulating ("bits_pull_acc"),
+        // Y is also read once: an upper bound, rows with nothing to add skip the read and the write.
+        TimedScope ts(acc ? TK_BITS_PULL_ACC : TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + (acc ? 16ULL : 8ULL) * W * m);
         u64 totb = gn * W * 8;
         const u32 tot_bytes = totb > 0xFFFFFFF0ULL ? 0xFFFFFFF0u : (u32)totb;
         const u32 hot_bytes = (u64)cx.opt_hot_bytes < tot_bytes ? (u32)cx.opt_hot_bytes : tot_bytes;
-        if (cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2)) launch_pull<W, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-        else launch_pull<W, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+        const bool hints = cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2);
+        if (acc) {
+            if (hints) launch_pull<W, true, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+            else launch_pull<W, false, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+        } else if (hints) launch_pull<W, true, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+        else launch_pull<W, false, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
     }
     if (path_out) *path_out = 3;
 }
@@ -1287,14 +1323,15 @@ void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
 }
 
 void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y, u64 *flops_out,
-              int *path_out) {
+              int *path_out, bool acc) {
     if (X.ncols != A.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
+    if (acc) require_acc_target(Y, X.nrows, A.ncols, X.W);
     switch (X.W) {
-    case 1: hop_impl<1>(X, A, AT, pt, Y, flops_out, path_out); break;
-    case 2: hop_impl<2>(X, A, AT, pt, Y, flops_out, path_out); break;
-    case 4: hop_impl<4>(X, A, AT, pt, Y, flops_out, path_out); break;
-    case 8: hop_impl<8>(X, A, AT, pt, Y, flops_out, path_out); break;
-    case 16: hop_impl<16>(X, A, AT, pt, Y, flops_out, path_out); break;
+    case 1: hop_impl<1>(X, A, AT, pt, Y, flops_out, path_out, acc); break;
+    case 2: hop_impl<2>(X, A, AT, pt, Y, flops_out, path_out, acc); break;
+    case 4: hop_impl<4>(X, A, AT, pt, Y, flops_out, path_out, acc); break;
+    case 8: hop_impl<8>(X, A, AT, pt, Y, flops_out, path_out, acc); break;
+    case 16: hop_impl<16>(X, A, AT, pt, Y, flops_out, path_out, acc); break;
     default: throw GrbError(-8, "bit-frontier: unsupported word count");
     }
 }

@@ -1028,8 +1028,8 @@ static bool bits_legal(GrB_Matrix C, GrB_Matrix M, GrB_Matrix A, GrB_Matrix B, c
 
 // Y = A*B through the frontier dispatch: the push straight from A's entries while A is still a small CSR, the diagonal filter, or
 // the direction-optimising push / pull.  pt_ok: the CSR push may write Y in B's hot-set order.  Returns true when Y came from
-// A's CSR form (A then has no bit form).
-static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
+// A's CSR form (A then has no bit form).  acc (union hops): Y |= A*B into a natural-order Y that holds earlier operands' products.
+static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y, u64 *fl, int *path, bool acc = false) {
     Context &cx = ctx();
     ensure_dev(B);
     if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
@@ -1037,13 +1037,18 @@ static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y,
     // should take it (only worth probing for a small CSR: the probe is O(nnz(F)))
     const bool from_csr = cx.opt_csr_push && A->dev_valid && !A->bits_valid && cx.opt_pull_mode != 1 &&
                           A->dev.nnz <= ((u64)1 << 20) &&
-                          !(B->diag_state == 1 && cx.opt_diag_filter) && bits_push_from_csr(A->dev, B->dev, Y, fl, (B->devT_valid && pt_ok) ? &B->pt : (const PullTables *)nullptr);
+                          !(B->diag_state == 1 && cx.opt_diag_filter) &&
+                          bits_push_from_csr(A->dev, B->dev, Y, fl, (B->devT_valid && pt_ok) ? &B->pt : (const PullTables *)nullptr, acc);
     if (from_csr) { *path = 7; return true; }
     if (!(A->bits_valid && A->pending.empty())) ensure_bits(A);   // an existing frontier keeps its vertex order for the hop
-    if (B->diag_state == 1 && cx.opt_diag_filter) { natural_bits(A); bits_diag(A->bits, B->dev, Y, fl); *path = 5; }
-    else {
+    if (B->diag_state == 1 && cx.opt_diag_filter) {
+        natural_bits(A);
+        if (acc) { DevBits Z; bits_diag(A->bits, B->dev, Z, fl); bits_or(Y, Z); }   // a diagonal type: a column filter, then OR
+        else bits_diag(A->bits, B->dev, Y, fl);
+        *path = 5;
+    } else {
         if (cx.opt_pull_mode != 0) ensure_devT(B);
-        bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, fl, path);
+        bits_hop(A->bits, B->dev, B->devT_valid ? &B->devT : nullptr, B->devT_valid ? &B->pt : (PullTables *)nullptr, Y, fl, path, acc);
     }
     return false;
 }
@@ -2233,6 +2238,216 @@ GrB_Info B200_Matrix_rmat_block(GrB_Matrix *A, int scale, uint64_t edge_factor, 
     });
 }
 
+// ---- unions of relationship operands with pending writes: E = U_t (m[t] \ dm[t]) u dp[t], pattern only ----
+// What the reference builds for a hop or a var-len walk over several relationship types (build_relationship_matrix_unrestricted,
+// graph.rs:2520-2550: extract(T_1), then set_pattern(<!dm_t> m_t) and set_pattern(dp_t) per further type).  The union is exact:
+// an entry that one type contributes survives another type's dm, and within a type dp wins over dm.  Walked by
+// B200_reach_batch_delta and multiplied by the union hops of B200_Matrix_union_lmxm / B200_traverse_batch_union.
+struct UnionOperand {
+    GrB_Matrix m = nullptr, dp = nullptr, dm = nullptr;
+    const DevCSR *ddp = nullptr;                 // dp's device form when it holds entries
+    RepairPlan rp;                               // dm's repair plan (rp.ns == 0: nothing to repair)
+};
+
+static std::vector<UnionOperand> union_operands(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
+    std::vector<UnionOperand> ops(nops);
+    for (int t = 0; t < nops; t++) { ops[t].m = m[t]; ops[t].dp = dp ? dp[t] : nullptr; ops[t].dm = dm ? dm[t] : nullptr; }
+    return ops;
+}
+
+// Y = F * E in frontier form (F at most 1024 rows), under the submission lock; *fl += sum_t flops(F * m[t]) + flops(F * dp[t]).
+// The first operand with a repair plan goes first: it writes Y fresh and has the columns its dm touches recomputed in place
+// (bits_repair overwrites columns, so it cannot accumulate).  Every further clean operand ORs into the same natural-order Y: the
+// pushes skip zeroing Y and the pull ORs each row into the stored record.  A further operand with a repair plan (or every further
+// operand with union_accum = 0) gets a bit-matrix of its own that is repaired, naturalised and ORed in.  pt_ok applies to a single
+// operand only: the CSR push may then leave Y in the operand's hot-set order, as GrB_mxm does.
+static void union_product(GrB_Matrix F, std::vector<UnionOperand> &ops, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
+    Context &cx = ctx();
+    const size_t nops = ops.size();
+    finish_pending(F);
+    std::vector<UnionOperand *> order;
+    for (UnionOperand &o : ops) if (o.rp.ns) { order.push_back(&o); break; }
+    for (UnionOperand &o : ops) if (order.empty() || &o != order[0]) order.push_back(&o);
+    DevBits Xcsr;
+    for (size_t i = 0; i < nops; i++) {
+        UnionOperand &o = *order[i];
+        const bool own = i > 0 && (o.rp.ns || !cx.opt_union_accum);
+        DevBits Z;
+        DevBits &T = own ? Z : Y;
+        u64 f = 0;
+        const bool from_csr = frontier_product(F, o.m, nops == 1 && pt_ok, T, &f, path, i > 0 && !own);
+        if (o.rp.ns) {
+            // the repair gathers from F in bit form: a frontier still in CSR form is converted for it
+            if (from_csr && !Xcsr.valid()) bits_from_csr(F->dev, Xcsr);
+            ensure_devT(o.m);
+            bits_repair(from_csr ? Xcsr : F->bits, o.m->devT, o.rp, T);
+        }
+        if (o.ddp) f += bits_apply_deltas(from_csr ? nullptr : &F->bits, from_csr ? &F->dev : nullptr, nullptr, o.ddp, T);
+        *fl += f;
+        if (own) { bits_naturalise(Z); bits_or(Y, Z); }
+    }
+}
+
+// U = the union of every operand's effective pattern (m \ dm) u dp, built once with the flush kernels
+static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<UnionOperand> &ops, u64 n) {
+    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, n, n);
+    if (info) return info;
+    info = guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+        all.push_back(*U);
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        DevCSR S;
+        bool have = false;
+        for (UnionOperand &o : ops) {
+            ensure_dev(o.m);
+            DevCSR E;
+            const DevCSR *e = &o.m->dev;
+            if (o.dm) {
+                ensure_dev(o.dm);
+                if (o.dm->dev.nnz) { filter_by_mask(*e, o.dm->dev, true, true, E); e = &E; }
+            }
+            if (o.dp) {
+                ensure_dev(o.dp);
+                if (o.dp->dev.nnz) { DevCSR T; ewise_union(*e, o.dp->dev, false, T); E = std::move(T); e = &E; }
+            }
+            if (!have) { csr_copy(*e, S, false); have = true; }
+            else { DevCSR T; ewise_union(S, *e, false, T); S = std::move(T); }
+        }
+        set_dev(*U, std::move(S));
+        return GrB_SUCCESS;
+    });
+    if (info) GrB_Matrix_free(U);
+    return info;
+}
+
+// per call, for the frontier form: deltas' pending tuples finished, dp's device form, and dm's repair plan (dm' and the repaired
+// segments of m', the base's mirror built at commit)
+static GrB_Info union_plan(std::vector<UnionOperand> &ops) {
+    return guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        for (UnionOperand &o : ops) {
+            if (o.dp) { ensure_dev(o.dp); if (o.dp->dev.nnz) o.ddp = &o.dp->dev; }
+            if (!o.dm) continue;
+            ensure_dev(o.dm);
+            if (!o.dm->dev.nnz) continue;
+            ensure_devT(o.m);
+            bits_repair_plan(o.dm->dev, o.m->devT, o.rp);
+        }
+        return GrB_SUCCESS;
+    });
+}
+
+// the plans' device buffers go back to the pool
+static void union_release(std::vector<UnionOperand> &ops) { guarded([&]() { GpuLock g; ops.clear(); return GrB_SUCCESS; }); }
+
+// ---- union hops: F <- F * E, exact (no delta_lmxm over-masking) ----
+// A union hop is prepared once per call: with F in frontier form (a BOOL F of at most 1024 rows and bits_mode != 0) the operands'
+// repair plans, otherwise the union materialised once (reach_materialise) for the general GrB_mxm -- the reference's cost, paid
+// per call rather than per hop.  last_flops of a union hop = sum_t flops(F * m[t]) + flops(F * dp[t]) on either path: the work
+// the frontier form does, independent of how the operands overlap.
+struct UnionHop {
+    std::vector<UnionOperand> ops;
+    GrB_Matrix U = nullptr;                      // the materialised union (row-wise path)
+};
+
+static bool union_frontier(u64 rows, u64 n) {
+    return ctx().opt_bits_mode != 0 && bits_words_for(rows) != 0 && n < ((u64)1 << 32);
+}
+
+static GrB_Info union_hop_prepare(UnionHop &uh, bool frontier, u64 n) {
+    return frontier ? union_plan(uh.ops) : reach_materialise(&uh.U, uh.ops, n);
+}
+
+static void union_hop_release(UnionHop &uh) {
+    GrB_Matrix_free(&uh.U);
+    union_release(uh.ops);
+}
+
+static GrB_Info union_hop_apply(GrB_Matrix F, UnionHop &uh) {
+    uvec<GrB_Matrix> all = {F};
+    for (UnionOperand &o : uh.ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+    if (uh.U) {
+        u64 fl = 0;
+        GrB_Info info = guarded([&]() {
+            GpuLock g;
+            MultiLock lk(all.begin(), all.end());
+            ensure_init();
+            ensure_dev(F);
+            for (UnionOperand &o : uh.ops) {
+                ensure_dev(o.m);
+                fl += spgemm_flops(F->dev, o.m->dev);
+                if (o.dp) { ensure_dev(o.dp); fl += spgemm_flops(F->dev, o.dp->dev); }
+            }
+            return GrB_SUCCESS;
+        });
+        if (!info) info = GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, uh.U, nullptr);
+        if (!info) { Context &cx = ctx(); cx.total_flops -= cx.last_flops.load(); cx.total_flops += fl; cx.last_flops = fl; }
+        return info;
+    }
+    return guarded([&]() {
+        GpuLock g;
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        Context &cx = ctx();
+        DevBits Y;
+        u64 fl = 0;
+        int path = 0;
+        union_product(F, uh.ops, true, Y, &fl, &path);
+        cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
+        set_bits(F, std::move(Y));
+        if (cx.opt_sync_after_op) sync_stream();
+        return GrB_SUCCESS;
+    });
+}
+
+// nops >= 1 operands and their deltas: square, of one size, device-resident
+static GrB_Info union_check(const char *what, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
+    CHECK_PTR(m);
+    if (nops < 1) { tl_error = std::string(what) + ": nops < 1"; return GrB_INVALID_VALUE; }
+    for (int t = 0; t < nops; t++) {
+        CHECK_MAT(m[t]);
+        if (dp && dp[t]) CHECK_MAT(dp[t]);
+        if (dm && dm[t]) CHECK_MAT(dm[t]);
+    }
+    const u64 n = m[0]->nrows;
+    for (int t = 0; t < nops; t++)
+        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
+            if (X && (X->nrows != n || X->ncols != n)) {
+                tl_error = std::string(what) + ": operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+            }
+    for (int t = 0; t < nops; t++)
+        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
+            if (X && is_huge(X)) { tl_error = std::string(what) + ": host-resident operand"; return GrB_NOT_IMPLEMENTED; }
+    return GrB_SUCCESS;
+}
+
+static GrB_Info device_ready() { return guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; }); }
+
+// The union hop as one call, the counterpart of B200_Matrix_delta_lmxm: F <- F * U_t (m[t] \ dm[t]) u dp[t].
+GrB_Info B200_Matrix_union_lmxm(GrB_Matrix F, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
+    CHECK_MAT(F);
+    GrB_Info info = union_check("union_lmxm", m, dp, dm, nops);
+    if (info) return info;
+    const u64 n = m[0]->nrows;
+    if (F->ncols != n) { tl_error = "union_lmxm: F * m does not fit F"; return GrB_DIMENSION_MISMATCH; }
+    if (is_huge(F)) { tl_error = "union_lmxm: host-resident frontier"; return GrB_NOT_IMPLEMENTED; }
+    info = device_ready();                       // no device: fail before any host work
+    if (info) return info;
+    UnionHop uh;
+    uh.ops = union_operands(m, dp, dm, nops);
+    info = union_hop_prepare(uh, F->type == T_BOOL && union_frontier(F->nrows, n), n);
+    if (!info) info = union_hop_apply(F, uh);
+    union_hop_release(uh);
+    return info;
+}
+
 // ---- delta_lmxm as ONE C call (matrix.rs:1317-1402): F <- (F*m AND NOT F*dm) OR F*dp over GxB_ANY_PAIR_BOOL ----
 // The reference composes three GrB_mxm calls and an eWiseAdd, each of which builds or rewrites a whole |F| x n bit-matrix.  In
 // frontier form only the deltas' entries are touched here: F*m runs through GrB_mxm's frontier path unchanged, then the dm and dp
@@ -2302,29 +2517,51 @@ GrB_Info B200_Matrix_delta_lmxm(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_M
 //   B200_OUT_AUTO   : bitmap when the result holds more than one entry per 32 slots (fewer bytes over PCIe), else CSR; the choice
 //                     is reported in *format_out.  Needs both output buffers.
 // Composed from the public entry points (each takes the submission lock for its own duration), so other threads' calls interleave.
-// Hop h is B200_Matrix_delta_lmxm(F, hops[h], dp[h], dm[h]); dp / dm NULL (B200_traverse_batch) or holding NULL entries: clean hops.
-static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, const GrB_Matrix *dp,
-                              const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p,
-                              uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
+// Operands are hop-major: hop h owns hop_nops[h] consecutive entries of hops / dp / dm (hop_nops NULL: one each).  A delta hop
+// (hop_union NULL or hop_union[h] == 0, one operand k) is B200_Matrix_delta_lmxm(F, hops[k], dp[k], dm[k]); a union hop is
+// B200_Matrix_union_lmxm over its operands, prepared once per call (union_hop_prepare).  dp / dm NULL (B200_traverse_batch) or
+// holding NULL entries: clean operands.
+static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const int *hop_nops, const int *hop_union,
+                              const GrB_Matrix *hops, const GrB_Matrix *dp, const GrB_Matrix *dm, int nhops, int format,
+                              uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
+                              uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
     CHECK_PTR(hops);
     if (nsrc) CHECK_PTR(sources);
     if (nhops < 1) { tl_error = "traverse_batch: nhops < 1"; return GrB_INVALID_VALUE; }
-    for (int h = 0; h < nhops; h++) {
-        CHECK_MAT(hops[h]);
-        if (dp && dp[h]) CHECK_MAT(dp[h]);
-        if (dm && dm[h]) CHECK_MAT(dm[h]);
+    std::vector<int> first(nhops + 1, 0);        // hop h's operands: [first[h], first[h + 1]) (hop_nops checked by the caller)
+    for (int h = 0; h < nhops; h++) first[h + 1] = first[h] + (hop_nops ? hop_nops[h] : 1);
+    const int nopd = first[nhops];
+    for (int k = 0; k < nopd; k++) {
+        CHECK_MAT(hops[k]);
+        if (dp && dp[k]) CHECK_MAT(dp[k]);
+        if (dm && dm[k]) CHECK_MAT(dm[k]);
     }
     if (format != B200_OUT_BITMAP && format != B200_OUT_CSR && format != B200_OUT_AUTO) { tl_error = "traverse_batch: unknown format"; return GrB_INVALID_VALUE; }
     if ((format != B200_OUT_CSR && !out_bits) || (format != B200_OUT_BITMAP && (!out_p || (!out_j && out_j_capacity)))) {
         tl_error = "traverse_batch: output buffer missing for the requested format"; return GrB_NULL_POINTER;
     }
-    const u64 inner = hops[0]->nrows, ncols = hops[nhops - 1]->ncols;
+    const u64 inner = hops[0]->nrows, ncols = hops[nopd - 1]->ncols;
     const u64 wpr = (ncols + 63) / 64;
     if (format != B200_OUT_CSR && words_per_row != wpr) { tl_error = "traverse_batch: words_per_row must be ceil(ncols / 64)"; return GrB_DIMENSION_MISMATCH; }
+    // GrB_mxm(C = F, A = F, B) needs C's dimensions to match the product: a chain over square n x n operands (what the reference
+    // stores, graph.rs:1191, 1211) keeps them; rectangular chains are rejected up front
+    for (int k = 0; k < nopd; k++) {
+        if (hops[k]->nrows != inner || hops[k]->ncols != inner) { tl_error = "traverse_batch: operands must be square and equally sized"; return GrB_DIMENSION_MISMATCH; }
+        for (GrB_Matrix D : {dp ? dp[k] : nullptr, dm ? dm[k] : nullptr})
+            if (D && (D->nrows != inner || D->ncols != inner)) { tl_error = "traverse_batch: delta dimensions differ from the hop's"; return GrB_DIMENSION_MISMATCH; }
+    }
     GrB_Scalar one = nullptr;
     GrB_Info info = GrB_Scalar_new(&one, GrB_BOOL);
     if (info) return info;
     GrB_Scalar_setElement_BOOL(one, true);
+    // union hops: plans (frontier form, for the rows of one F: a 128-row slice or the whole batch) or the materialised union
+    std::vector<UnionHop> uhops(hop_union ? nhops : 0);
+    const bool ufrontier = union_frontier(format == B200_OUT_BITMAP ? std::min<u64>(nsrc, 128) : nsrc, inner);
+    for (int h = 0; h < (int)uhops.size() && !info; h++)
+        if (hop_union[h]) {
+            uhops[h].ops = union_operands(hops + first[h], dp ? dp + first[h] : nullptr, dm ? dm + first[h] : nullptr, first[h + 1] - first[h]);
+            info = union_hop_prepare(uhops[h], ufrontier, inner);
+        }
     u64 flops = 0, nvals = 0;
     int chosen = format;
     std::vector<B200_Ticket> tickets;
@@ -2333,9 +2570,11 @@ static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const Gr
         for (u64 i = 0; i < r1 - r0; i++) rows[i] = i;
         GrB_Info e = GxB_Matrix_build_Scalar(F, rows.data(), sources + r0, one, r1 - r0);
         for (int h = 0; h < nhops && !e; h++) {
-            e = B200_Matrix_delta_lmxm(F, hops[h], dp ? dp[h] : nullptr, dm ? dm[h] : nullptr);
+            const int k = first[h];
+            e = (hop_union && hop_union[h]) ? union_hop_apply(F, uhops[h])
+                                            : B200_Matrix_delta_lmxm(F, hops[k], dp ? dp[k] : nullptr, dm ? dm[k] : nullptr);
             if (!e) flops += ctx().last_flops.load();
-            if (!e && h + 1 < nhops && F->ncols != hops[h + 1]->nrows) { tl_error = "traverse_batch: hop dimensions do not chain"; e = GrB_DIMENSION_MISMATCH; }
+            if (!e && h + 1 < nhops && F->ncols != hops[first[h + 1]]->nrows) { tl_error = "traverse_batch: hop dimensions do not chain"; e = GrB_DIMENSION_MISMATCH; }
         }
         return e;
     };
@@ -2343,14 +2582,7 @@ static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const Gr
         // the frontier's column dimension follows the hops: n0 x n1 x ... (rectangular label ranges are n x n in the reference)
         return GrB_Matrix_new(F, GrB_BOOL, rows, inner);
     };
-    // GrB_mxm(C = F, A = F, B) needs C's dimensions to match the product: a chain over square n x n operands (what the reference
-    // stores, graph.rs:1191, 1211) keeps them; rectangular chains are rejected up front
-    for (int h = 0; h < nhops; h++) {
-        if (hops[h]->nrows != inner || hops[h]->ncols != inner) { GrB_Scalar_free(&one); tl_error = "traverse_batch: operands must be square and equally sized"; return GrB_DIMENSION_MISMATCH; }
-        for (GrB_Matrix D : {dp ? dp[h] : nullptr, dm ? dm[h] : nullptr})
-            if (D && (D->nrows != inner || D->ncols != inner)) { GrB_Scalar_free(&one); tl_error = "traverse_batch: delta dimensions differ from the hop's"; return GrB_DIMENSION_MISMATCH; }
-    }
-    if (format == B200_OUT_AUTO || format == B200_OUT_CSR) {
+    if (!info && (format == B200_OUT_AUTO || format == B200_OUT_CSR)) {
         // density is known only after the hops: run the whole batch once, then pick the hand-off
         GrB_Matrix F = nullptr;
         info = fresh(&F, nsrc);
@@ -2366,7 +2598,7 @@ static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const Gr
             }
         }
         GrB_Matrix_free(&F);
-    } else {
+    } else if (!info) {
         const u64 per = 128;
         for (u64 r0 = 0; r0 < nsrc && !info; r0 += per) {
             const u64 r1 = std::min<u64>(nsrc, r0 + per);
@@ -2381,6 +2613,7 @@ static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const Gr
         for (B200_Ticket &t : tickets) { GrB_Info e = B200_Ticket_wait(&t); if (!info) info = e; }
         nvals = ~0ULL;       // not counted on this path (a popcount pass per slice would only serve this number)
     }
+    for (UnionHop &uh : uhops) union_hop_release(uh);
     GrB_Scalar_free(&one);
     if (nvals_out) *nvals_out = nvals;
     if (flops_out) *flops_out = flops;
@@ -2391,8 +2624,8 @@ static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const Gr
 GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, int nhops, int format,
                              uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
                              uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
-    return traverse_impl(sources, nsrc, hops, nullptr, nullptr, nhops, format, out_bits, words_per_row, out_p, out_j, out_j_capacity,
-                         nvals_out, flops_out, format_out);
+    return traverse_impl(sources, nsrc, nullptr, nullptr, hops, nullptr, nullptr, nhops, format, out_bits, words_per_row, out_p, out_j,
+                         out_j_capacity, nvals_out, flops_out, format_out);
 }
 
 // The same traversal over operands with pending writes: hop h is (m[h], dp[h], dm[h]) through B200_Matrix_delta_lmxm.
@@ -2400,8 +2633,30 @@ GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, con
                                    const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row,
                                    uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out,
                                    int *format_out) {
-    return traverse_impl(sources, nsrc, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j, out_j_capacity, nvals_out,
-                         flops_out, format_out);
+    return traverse_impl(sources, nsrc, nullptr, nullptr, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j,
+                         out_j_capacity, nvals_out, flops_out, format_out);
+}
+
+// The same traversal over hop groups: hop h is a delta hop (hop_union[h] == 0, hop_nops[h] == 1) or a union hop over its
+// hop_nops[h] operands (B200_Matrix_union_lmxm).  Operands, validation and errors as B200_Matrix_union_lmxm.
+GrB_Info B200_traverse_batch_union(const GrB_Index *sources, GrB_Index nsrc, const int *hop_nops, const int *hop_union, int nhops,
+                                   const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int format, uint64_t *out_bits,
+                                   uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
+                                   uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
+    CHECK_PTR(hop_nops); CHECK_PTR(hop_union);
+    if (nsrc) CHECK_PTR(sources);
+    if (nhops < 1) { tl_error = "traverse_batch: nhops < 1"; return GrB_INVALID_VALUE; }
+    int nopd = 0;
+    for (int h = 0; h < nhops; h++) {
+        if (hop_nops[h] < 1) { tl_error = "traverse_batch: a hop has no operand"; return GrB_INVALID_VALUE; }
+        if (hop_nops[h] > 1 && !hop_union[h]) { tl_error = "traverse_batch: a delta hop takes one operand"; return GrB_INVALID_VALUE; }
+        nopd += hop_nops[h];
+    }
+    GrB_Info info = union_check("traverse_batch_union", m, dp, dm, nopd);
+    if (!info) info = device_ready();           // no device: fail before any host work
+    if (info) return info;
+    return traverse_impl(sources, nsrc, hop_nops, hop_union, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j,
+                         out_j_capacity, nvals_out, flops_out, format_out);
 }
 
 // ---- multi-source reachability as ONE C call (SURVEY 8f-1: the multiplicity-insensitive core of CondVarLenTraverse with
@@ -2412,47 +2667,22 @@ GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, con
 // in device frontier form for <= 1024 sources.  Composed from the public entry points.  *reached is a new nsrc x n BOOL matrix.
 //
 // B200_reach_batch_delta walks A = U_t (m[t] \ dm[t]) u dp[t] exactly (no delta_lmxm over-masking).  One operand without deltas
-// (B200_reach_batch) issues the calls above unchanged.  Otherwise a level in frontier form is reach_hop: per operand Y = F*m[t]
-// through the usual dispatch, the columns dm[t] touches recomputed from m[t]'s transpose mirror without the deleted in-edges
-// (bits_repair), then the dp[t] term; the operands' products are ORed, and only then is the reached set masked out, so a dp edge
-// cannot re-add a vertex already reached.  With bits_mode -1 the dirty reach stays in frontier form whenever it is legal (a tiny
+// (B200_reach_batch) issues the calls above unchanged.  Otherwise a level in frontier form is reach_hop: Y = F * A through
+// union_product (per operand Y = F*m[t] through the usual dispatch, the columns dm[t] touches recomputed from m[t]'s transpose
+// mirror without the deleted in-edges (bits_repair), then the dp[t] term, the operands' products ORed into one Y), and only then is
+// the reached set masked out, so a dp edge cannot re-add a vertex already reached.  With bits_mode -1 the dirty reach stays in frontier form whenever it is legal (a tiny
 // hop-1 frontier takes the CSR push there): the row-wise path would first need every dirty operand rewritten, O(nnz(m)) per call.
 // Where the frontier path does not apply (bits_mode 0, more than 1024 sources) every dirty operand is materialised once per call
 // with the flush kernels (filter_by_mask, ewise_union) and the level runs the calls above over their union.
 
-struct ReachOperand {
-    GrB_Matrix m = nullptr, dp = nullptr, dm = nullptr;
-    const DevCSR *ddp = nullptr;                 // dp's device form when it holds entries
-    RepairPlan rp;                               // dm's repair plan (rp.ns == 0: nothing to repair)
-};
-
-// One level in frontier form: F <- (OR_t F * E_t) AND NOT R (R only when masked).  F has at most 1024 rows.  Runs under the
-// submission lock.
-static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<ReachOperand> &ops) {
+// One level in frontier form: F <- (F * A) AND NOT R (R only when masked).  F has at most 1024 rows.  Runs under the submission
+// lock.  One operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does.
+static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<UnionOperand> &ops) {
     Context &cx = ctx();
-    const size_t nops = ops.size();
-    finish_pending(F);
-    DevBits acc, Xcsr;
+    DevBits acc;
     u64 fl = 0;
     int path = 0;
-    for (ReachOperand &o : ops) {
-        DevBits Y;
-        u64 f = 0;
-        // one operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does
-        const bool from_csr = frontier_product(F, o.m, nops == 1 && !masked, Y, &f, &path);
-        if (o.rp.ns) {
-            // the repair gathers from F in bit form: a frontier still in CSR form is converted for it
-            if (from_csr && !Xcsr.valid()) bits_from_csr(F->dev, Xcsr);
-            ensure_devT(o.m);
-            bits_repair(from_csr ? Xcsr : F->bits, o.m->devT, o.rp, Y);
-        }
-        if (o.ddp) f += bits_apply_deltas(from_csr ? nullptr : &F->bits, from_csr ? &F->dev : nullptr, nullptr, o.ddp, Y);
-        fl += f;
-        if (nops == 1) { acc = std::move(Y); break; }
-        bits_naturalise(Y);
-        if (!acc.valid()) acc = std::move(Y);
-        else bits_or(acc, Y);
-    }
+    union_product(F, ops, !masked, acc, &fl, &path);
     if (masked) {
         bits_naturalise(acc);
         ensure_bits(R);
@@ -2463,45 +2693,9 @@ static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<Reach
     if (cx.opt_sync_after_op) sync_stream();
 }
 
-// U = the union of every operand's effective pattern (m \ dm) u dp, built once with the flush kernels
-static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<ReachOperand> &ops, u64 n) {
-    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, n, n);
-    if (info) return info;
-    info = guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-        all.push_back(*U);
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        DevCSR S;
-        bool have = false;
-        for (ReachOperand &o : ops) {
-            ensure_dev(o.m);
-            DevCSR E;
-            const DevCSR *e = &o.m->dev;
-            if (o.dm) {
-                ensure_dev(o.dm);
-                if (o.dm->dev.nnz) { filter_by_mask(*e, o.dm->dev, true, true, E); e = &E; }
-            }
-            if (o.dp) {
-                ensure_dev(o.dp);
-                if (o.dp->dev.nnz) { DevCSR T; ewise_union(*e, o.dp->dev, false, T); E = std::move(T); e = &E; }
-            }
-            if (!have) { csr_copy(*e, S, false); have = true; }
-            else { DevCSR T; ewise_union(S, *e, false, T); S = std::move(T); }
-        }
-        set_dev(*U, std::move(S));
-        return GrB_SUCCESS;
-    });
-    if (info) GrB_Matrix_free(U);
-    return info;
-}
-
 static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
                            const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources, int64_t *levels_out) {
     const u64 n = m[0]->ncols;
-    std::vector<ReachOperand> ops(nops);
     bool clean = nops == 1;
     for (int t = 0; t < nops && clean; t++)
         for (GrB_Matrix D : {dp ? dp[t] : nullptr, dm ? dm[t] : nullptr}) {
@@ -2513,28 +2707,10 @@ static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_In
         }
     GrB_Matrix U = nullptr;                      // the materialised union, when a level runs the row-wise calls
     GrB_Info info = GrB_SUCCESS;
-    for (int t = 0; t < nops; t++) { ops[t].m = m[t]; ops[t].dp = dp ? dp[t] : nullptr; ops[t].dm = dm ? dm[t] : nullptr; }
+    std::vector<UnionOperand> ops = union_operands(m, dp, dm, nops);
     const bool frontier = ctx().opt_bits_mode != 0 && bits_words_for(nsrc) != 0;
     if (!clean && !frontier) info = reach_materialise(&U, ops, n);
-    else if (!clean) {
-        // per call: deltas' pending tuples finished, dm' and the repaired segments of m' (the base's mirror, built at commit)
-        info = guarded([&]() {
-            GpuLock g;
-            uvec<GrB_Matrix> all;
-            for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-            MultiLock lk(all.begin(), all.end());
-            ensure_init();
-            for (ReachOperand &o : ops) {
-                if (o.dp) { ensure_dev(o.dp); if (o.dp->dev.nnz) o.ddp = &o.dp->dev; }
-                if (!o.dm) continue;
-                ensure_dev(o.dm);
-                if (!o.dm->dev.nnz) continue;
-                ensure_devT(o.m);
-                bits_repair_plan(o.dm->dev, o.m->devT, o.rp);
-            }
-            return GrB_SUCCESS;
-        });
-    }
+    else if (!clean) info = union_plan(ops);
     GrB_Matrix A = U ? U : m[0];                 // the operand of the row-wise calls
     GrB_Scalar one = nullptr;
     GrB_Matrix F = nullptr, R = nullptr;
@@ -2557,7 +2733,7 @@ static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_In
             info = guarded([&]() {
                 GpuLock g;
                 uvec<GrB_Matrix> all = {F, R};
-                for (ReachOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+                for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
                 MultiLock lk(all.begin(), all.end());
                 ensure_init();
                 reach_hop(F, R, rn != 0, ops);
@@ -2575,7 +2751,7 @@ static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_In
     GrB_Scalar_free(&one);
     GrB_Matrix_free(&F);
     GrB_Matrix_free(&U);
-    if (!clean) guarded([&]() { GpuLock g; ops.clear(); return GrB_SUCCESS; });   // the plans' device buffers go back to the pool
+    if (!clean) union_release(ops);
     if (info) { GrB_Matrix_free(&R); return info; }
     if (levels_out) *levels_out = level;
     *reached = R;
@@ -2682,6 +2858,7 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "csr_push") c.opt_csr_push = value;
     else if (n == "fused_prep") c.opt_fused_prep = value;
     else if (n == "perm_push") c.opt_perm_push = value;
+    else if (n == "union_accum") c.opt_union_accum = value;
     // retired: the pull, the count pass and the fill have a single kernel each now, and there is no persisting-L2 window; the
     // names stay accepted so callers that set them keep working
     else if (n == "fill_kernel" || n == "fill_cap" || n == "pull_kernel" || n == "unroll" || n == "small_split" ||

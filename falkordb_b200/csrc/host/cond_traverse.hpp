@@ -21,38 +21,90 @@ struct ExpandResult {
 
 static const size_t BATCH_SIZE = 1024; // graph/src/runtime/batch.rs:81
 
-// TraversalMatrix (cond_traverse.rs:64-90): the adjacency VersionedMatrix<bool>, or one relationship type's Tensor
+// Graph::build_relationship_matrix_unrestricted (graph.rs:2520-2550), statement for statement: the exact union of several
+// relationship types' forward layers, U_t (m_t \ dm_t) u dp_t, as a fresh delta-free matrix.  set_pattern has no replace, so an
+// entry an earlier type contributed survives a later type's dm.  What CondTraverseOp multiplies by for -[:R1|R2]-> before the
+// union hop; tests compare the union hop against it.
+inline VersionedMatrix union_by_extract(const std::vector<const Tensor *> &types) {
+    Matrix<bool> m = types[0]->extract();
+    for (size_t k = 1; k < types.size(); k++) {
+        const Tensor *t = types[k];
+        t->wait_fwd();
+        m.set_pattern<uint64_t>(&t->fwd_dm(), t->fwd_m(), Descriptor::C);
+        m.set_pattern<uint64_t>(nullptr, t->fwd_dp());
+    }
+    return VersionedMatrix::from_matrix(m);
+}
+
+// TraversalMatrix (cond_traverse.rs:64-90): the adjacency VersionedMatrix<bool>, one relationship type's Tensor, or several types'
+// Tensors (-[:R1|R2]->, cond_traverse.rs:493, 523): the union hop over their forward layers (B200_Matrix_union_lmxm) in place of
+// the reference's build_relationship_matrix_unrestricted plus a hop by the fresh matrix.  A one-type list is still a union hop.
 struct TraversalMatrix {
     const VersionedMatrix *vm = nullptr;
     const Tensor *t = nullptr;
+    std::vector<const Tensor *> ts;
     TraversalMatrix(const VersionedMatrix *v) : vm(v) {}
     TraversalMatrix(const Tensor *x) : t(x) {}
-    uint64_t ncols() const { return vm ? vm->ncols() : t->fwd_m().ncols(); }
+    TraversalMatrix(std::vector<const Tensor *> xs) : ts(std::move(xs)) {
+        if (ts.empty()) throw std::invalid_argument("TraversalMatrix: a multi-type hop needs at least one type");
+    }
+    bool is_union() const { return !ts.empty(); }
+    uint64_t ncols() const { return vm ? vm->ncols() : (t ? t : ts[0])->fwd_m().ncols(); }
     void delta_lmxm_into(Matrix<bool> &f) const {                // cond_traverse.rs:77-85
         if (vm) f.delta_lmxm(vm->m(), vm->dp(), vm->dm());
-        else f.delta_lmxm(t->fwd_m(), t->fwd_dp(), t->fwd_dm());
+        else if (t) f.delta_lmxm(t->fwd_m(), t->fwd_dp(), t->fwd_dm());
+        else {
+            std::vector<GrB_Matrix> m, dp, dm;
+            operands(m, dp, dm);
+            f.union_lmxm(m, dp, dm);
+        }
     }
-    // the (m, dp, dm) handles delta_lmxm_into multiplies by, for B200_traverse_batch_delta
-    void operands(GrB_Matrix *m, GrB_Matrix *dp, GrB_Matrix *dm) const {
-        if (vm) { vm->dp().wait(); vm->dm().wait(); *m = vm->m().inner(); *dp = vm->dp().inner(); *dm = vm->dm().inner(); }
-        else { t->fwd_dp().wait(); t->fwd_dm().wait(); *m = t->fwd_m().inner(); *dp = t->fwd_dp().inner(); *dm = t->fwd_dm().inner(); }
+    // the (m, dp, dm) handles delta_lmxm_into multiplies by, appended: one triple, or one per type of a union hop
+    void operands(std::vector<GrB_Matrix> &m, std::vector<GrB_Matrix> &dp, std::vector<GrB_Matrix> &dm) const {
+        if (vm) {
+            vm->dp().wait(); vm->dm().wait();
+            m.push_back(vm->m().inner()); dp.push_back(vm->dp().inner()); dm.push_back(vm->dm().inner());
+            return;
+        }
+        if (t) {
+            t->fwd_dp().wait(); t->fwd_dm().wait();
+            m.push_back(t->fwd_m().inner()); dp.push_back(t->fwd_dp().inner()); dm.push_back(t->fwd_dm().inner());
+            return;
+        }
+        for (const Tensor *x : ts) {                             // as build_relationship_matrix_unrestricted: wait_fwd per type
+            x->wait_fwd();
+            x->fwd_m().wait(); x->fwd_dp().wait(); x->fwd_dm().wait();
+            m.push_back(x->fwd_m().inner()); dp.push_back(x->fwd_dp().inner()); dm.push_back(x->fwd_dm().inner());
+        }
     }
 };
 
-// Every hop of a batch in one library call (B200_traverse_batch_delta, CSR hand-off): (row, dest) pairs of F * hops, in
-// ascending order.  The batch rows are the surviving sources' positions in the input batch.
+// Every hop of a batch in one library call (CSR hand-off): (row, dest) pairs of F * hops, in ascending order.  The batch rows are
+// the surviving sources' positions in the input batch.  Hops of one operand each go to B200_traverse_batch_delta; with a union hop
+// among them the hop groups go to B200_traverse_batch_union.
 inline void traverse_coalesced(const std::vector<uint64_t> &rows, const std::vector<uint64_t> &srcs,
                                const std::vector<TraversalMatrix> &hops, std::vector<uint64_t> &out_row, std::vector<uint64_t> &out_dest) {
-    std::vector<GrB_Matrix> m(hops.size()), dp(hops.size()), dm(hops.size());
-    for (size_t h = 0; h < hops.size(); h++) hops[h].operands(&m[h], &dp[h], &dm[h]);
+    std::vector<GrB_Matrix> m, dp, dm;
+    std::vector<int> nops, uni;
+    bool any_union = false;
+    for (const TraversalMatrix &h : hops) {
+        const size_t before = m.size();
+        h.operands(m, dp, dm);
+        nops.push_back((int)(m.size() - before));
+        uni.push_back(h.is_union() ? 1 : 0);
+        any_union = any_union || h.is_union();
+    }
     std::vector<uint64_t> p(srcs.size() + 1);
     std::vector<uint32_t> j(std::max<size_t>(1024, 16 * srcs.size()));
     uint64_t nv = 0;
     for (int attempt = 0; attempt < 2; attempt++) {              // a result larger than the first guess is rerun into its size
-        GrB_Info info = B200_traverse_batch_delta(srcs.data(), srcs.size(), m.data(), dp.data(), dm.data(), (int)hops.size(),
-                                                  B200_OUT_CSR, nullptr, 0, p.data(), j.data(), j.size(), &nv, nullptr, nullptr);
+        GrB_Info info = any_union
+            ? B200_traverse_batch_union(srcs.data(), srcs.size(), nops.data(), uni.data(), (int)hops.size(), m.data(), dp.data(),
+                                        dm.data(), B200_OUT_CSR, nullptr, 0, p.data(), j.data(), j.size(), &nv, nullptr, nullptr)
+            : B200_traverse_batch_delta(srcs.data(), srcs.size(), m.data(), dp.data(), dm.data(), (int)hops.size(),
+                                        B200_OUT_CSR, nullptr, 0, p.data(), j.data(), j.size(), &nv, nullptr, nullptr);
         if (info == GrB_INSUFFICIENT_SPACE && attempt == 0) { j.resize(nv); continue; }
-        grb_ok(info, "B200_traverse_batch_delta");
+        grb_ok(info, any_union ? "B200_traverse_batch_union" : "B200_traverse_batch_delta");
         break;
     }
     for (size_t r = 0; r < srcs.size(); r++)

@@ -584,6 +584,47 @@ static void t_coalesced_traverse_over_tensor_operand() {
     }
 }
 
+// multi-type hops (-[:R1|R2]->): expand_batch over a union TraversalMatrix, per hop (B200_Matrix_union_lmxm) and coalesced
+// (B200_traverse_batch_union), gives the pairs of the reference's route, union_by_extract plus a hop by the fresh matrix
+static void t_union_traverse_over_tensor_types() {   // device
+    auto pairs = [](const ExpandResult &r) {
+        std::vector<std::pair<uint64_t, uint64_t>> v;
+        for (size_t k = 0; k < r.dest.size(); k++) v.push_back({r.row_idx[k], r.dest[k]});
+        return v;
+    };
+    const uint64_t n = 64;
+    auto make = [&](uint64_t mul, uint64_t add, uint64_t id, uint64_t del) {
+        Tensor t(n, n);
+        std::vector<uint64_t> S, D, I;
+        for (uint64_t i = 0; i < 280; i++) { S.push_back((i * mul) % n); D.push_back((i * add + 7 + i / n) % n); I.push_back(id++); }
+        t.set_all_from_slices(S, D, I);
+        t.wait();
+        t.fold_oversized();                                       // the first batch becomes the committed base
+        std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> gone;
+        for (uint64_t i = del; i < 280; i += 4) gone.push_back(std::make_tuple(I[i], S[i], D[i]));
+        t.remove_all(gone);                                       // tombstones over the base
+        t.set_all_from_slices({1, 2, 3, S[0]}, {50, 51, 52, D[0]}, {id, id + 1, id + 2, id + 3});   // adds, one re-add
+        return t;
+    };
+    // c holds a's pairs but deletes others: a pair deleted in one type stays through the other, in both directions
+    Tensor a = make(37, 101, 0, 0), b = make(53, 89, 10000, 1), c = make(37, 101, 20000, 2);
+    VersionedMatrix lab(n, n);
+    for (uint64_t v = 0; v < n; v += 3) lab.set(v, v);
+    std::vector<uint64_t> src = {0, 1, 5, 9, 17, 40, 63};
+    for (const std::vector<const Tensor *> &types : {std::vector<const Tensor *>{&a}, std::vector<const Tensor *>{&a, &b},
+                                                     std::vector<const Tensor *>{&a, &b, &c}}) {
+        VersionedMatrix u = union_by_extract(types);
+        std::vector<TraversalMatrix> hops = {TraversalMatrix(&a), TraversalMatrix(types), TraversalMatrix(&lab), TraversalMatrix(types)};
+        std::vector<TraversalMatrix> ref = {TraversalMatrix(&a), TraversalMatrix(&u), TraversalMatrix(&lab), TraversalMatrix(&u)};
+        for (bool fuse : {false, true}) {
+            ExpandResult want = expand_batch(src, ref, {}, {&lab}, fuse);
+            REQUIRE(!want.dest.empty(), "test setup: the traversal finds nothing");
+            REQUIRE(pairs(expand_batch(src, hops, {}, {&lab}, fuse)) == pairs(want), "per-hop union traversal differs from union_by_extract");
+            REQUIRE(pairs(expand_batch(src, hops, {}, {&lab}, fuse, true)) == pairs(want), "coalesced union traversal differs from union_by_extract");
+        }
+    }
+}
+
 // var_len_reach (one B200_reach_batch_delta call) against the DISTINCT nodes the trail DFS reaches, over tensors whose inserts,
 // deletes, re-adds, multi-edges and self-loops still sit in the deltas.  The graphs are sparse so that the DFS stays small.
 struct TensorsAdjacency {       // get_node_relationships_by_type over several types
@@ -901,6 +942,7 @@ static TestEntry TESTS[] = {
     {"traverse_over_tensor_operand", t_traverse_over_tensor_operand},
     {"coalesced_traverse_over_tensor_operand", t_coalesced_traverse_over_tensor_operand},
     {"var_len_reach_matches_trails", t_var_len_reach_matches_trails},
+    {"union_traverse_over_tensor_types", t_union_traverse_over_tensor_types},
     {"repack_output_batches", t_repack_output_batches},
     {"repack_logic", t_repack_logic},
     {"var_len_trails", t_var_len_trails},

@@ -239,6 +239,13 @@ class Matrix {
         grb_ok(B200_Matrix_delta_lmxm(h->m, m.inner(), dp.inner(), dm.inner()), "B200_Matrix_delta_lmxm");
         mark_pending();
     }
+    // the union hop over several relationship types as one library call (B200_Matrix_union_lmxm):
+    // self <- self * U_t (m[t] \ dm[t]) u dp[t], exact; the deltas' pending tuples must be finished by the caller
+    void union_lmxm(const std::vector<GrB_Matrix> &m, const std::vector<GrB_Matrix> &dp, const std::vector<GrB_Matrix> &dm) {
+        static_assert(std::is_same<T, bool>::value, "union_lmxm is defined on Matrix<bool>");
+        grb_ok(B200_Matrix_union_lmxm(h->m, m.data(), dp.data(), dm.data(), (int)m.size()), "B200_Matrix_union_lmxm");
+        mark_pending();
+    }
 
     // ---- iteration: the reference's loop over the C row iterator (matrix.rs:1471-1605) ----
     class Iter {

@@ -26,8 +26,9 @@ void bits_to_csr(const DevBits &X, DevCSR &C);
 u64 bits_nvals(const DevBits &X);
 // Y = F * A expanded straight from F's CSR (small frontiers); false = the frontier touches enough of A that the pull should take
 // it (edges * 4 > nnz(A)), nothing was done.  pt (optional): A's pull tables; when they carry a vertex order the result is
-// written in it (permuted form)
-bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr);
+// written in it (permuted form).  acc: Y |= F * A, Y holding a natural-order product of the same shape (pt is then ignored)
+bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr,
+                        bool acc = false);
 void bits_naturalise(DevBits &X);                                // permuted form -> natural vertex order (no-op when natural)
 bool csr_is_diagonal(const DevCSR &A);                          // square, every entry (i,i)
 void bits_diag(const DevBits &X, const DevCSR &A, DevBits &Y, u64 *flops_out);   // Y = X * A for diagonal A
@@ -51,9 +52,10 @@ struct PullTables {   // per-matrix tables of the pull direction, cached with th
         built = false;
     }
 };
-// Y = X * A.  AT (= A') and its pull tables enable the pull direction; may be null (push only).
+// Y = X * A.  AT (= A') and its pull tables enable the pull direction; may be null (push only).  acc: Y |= X * A into a
+// natural-order Y of the product's shape (the push skips zeroing Y, the pull ORs each row into the stored record).
 void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y, u64 *flops_out,
-              int *path_out);
+              int *path_out, bool acc = false);
 void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt);   // square A: build the pull tables now
 void bits_andnot(DevBits &Y, const DevBits &M); // Y &= ~M
 void bits_or(DevBits &Y, const DevBits &Z);     // Y |= Z

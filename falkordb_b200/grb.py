@@ -272,6 +272,15 @@ class Matrix:
         are applied to F*m in place, touching only the deltas' entries.  dp / dm may be None."""
         check(lib().B200_Matrix_delta_lmxm(self.h, m.h, None if dp is None else dp.h, None if dm is None else dm.h))
 
+    def union_lmxm(self, ms, deltas=None):
+        """B200_Matrix_union_lmxm: the union hop of `-[:R1|R2]->`, self <- self * U_t (ms[t] \\ dm_t) u dp_t, exact (no
+        delta_lmxm over-masking, also for one operand).  `deltas`: one (dp, dm) pair per operand, either may be None."""
+        n = len(ms)
+        deltas = [(None, None)] * n if deltas is None else list(deltas)
+        assert len(deltas) == n, "one (dp, dm) pair per operand"
+        arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
+        check(lib().B200_Matrix_union_lmxm(self.h, arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), n))
+
     def element_wise_add(self, mask=None, a=None, b=None, descriptor=None):
         op = obj("GxB_ANY_BOOL") if self.dtype is bool else obj("GrB_SECOND_UINT64")
         check(lib().GrB_Matrix_eWiseAdd_BinaryOp(self.h, mask.h if mask is not None else None, None, op,
@@ -414,21 +423,40 @@ def traverse_batch(sources, hop_matrices, fmt=OUT_AUTO, out_bitmap=None, out_p=N
     F(i, sources[i]) = 1, F <- F * hop_matrices[0] * ... ; the result lands in `out_bitmap` (uint64[nsrc, ceil(n/64)], pinned for
     overlapped copies) and / or (`out_p` uint64[nsrc+1], `out_j` uint32[capacity]).  Returns (flops, nvals or None, format).
     `deltas`: one (dp, dm) pair per hop (either may be None) -- hop h is then delta_lmxm by (hop_matrices[h], dp, dm), through
-    B200_traverse_batch_delta."""
+    B200_traverse_batch_delta.
+    A hop given as a LIST of operands is a union hop (the types of `-[:R1|R2]->`, Matrix.union_lmxm), and its entry of `deltas`
+    (if given) a list with one (dp, dm) pair per operand; any such hop sends the call through B200_traverse_batch_union."""
     sources = _u64arr(sources)
     nh = len(hop_matrices)
-    hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
     nv, fl, chosen = U64(0), U64(0), C.c_int(0)
     wpr = out_bitmap.shape[1] if out_bitmap is not None else 0
     outs = (fmt, None if out_bitmap is None else out_bitmap.ctypes.data, wpr,
             None if out_p is None else out_p.ctypes.data, None if out_j is None else out_j.ctypes.data,
             0 if out_j is None else len(out_j), C.byref(nv), C.byref(fl), C.byref(chosen))
-    if deltas is None:
+    if any(isinstance(h, (list, tuple)) for h in hop_matrices):
+        assert deltas is None or len(deltas) == nh, "one deltas entry per hop"
+        ms, pairs, nops, union = [], [], [], []
+        for k, h in enumerate(hop_matrices):
+            group = list(h) if isinstance(h, (list, tuple)) else [h]
+            d = (None, None) if deltas is None else deltas[k]
+            d = ([(None, None)] * len(group) if d is None else list(d)) if isinstance(h, (list, tuple)) else [d]
+            assert len(d) == len(group), "one (dp, dm) pair per operand of a union hop"
+            ms += group
+            pairs += d
+            nops.append(len(group))
+            union.append(1 if isinstance(h, (list, tuple)) else 0)
+        n = len(ms)
+        arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
+        info = lib().B200_traverse_batch_union(sources.ctypes.data, len(sources), (C.c_int * nh)(*nops), (C.c_int * nh)(*union), nh,
+                                               arr(ms), arr([d[0] for d in pairs]), arr([d[1] for d in pairs]), *outs)
+    elif deltas is None:
+        hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
         info = lib().B200_traverse_batch(sources.ctypes.data, len(sources), hs, nh, *outs)
     else:
         assert len(deltas) == nh, "one (dp, dm) pair per hop"
         dps = (C.c_void_p * nh)(*[None if d[0] is None else d[0].h for d in deltas])
         dms = (C.c_void_p * nh)(*[None if d[1] is None else d[1].h for d in deltas])
+        hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
         info = lib().B200_traverse_batch_delta(sources.ctypes.data, len(sources), hs, dps, dms, nh, *outs)
     if info == -103:                     # GrB_INSUFFICIENT_SPACE: nv holds the entries needed
         raise BufferError(f"out_j holds {0 if out_j is None else len(out_j)} entries, the result has {nv.value}")

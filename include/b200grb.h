@@ -348,6 +348,22 @@ GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, con
                                    const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row,
                                    uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out,
                                    int *format_out);
+/* The union hop of a fixed-length hop over several relationship types (MATCH (a)-[:R1|R2]->(b); CondTraverseOp's
+ * build_relationship_matrix_unrestricted, graph.rs:2520-2550): F <- F * U_t (m[t] \ dm[t]) u dp[t] over GxB_ANY_PAIR_BOOL, exact
+ * (no delta_lmxm over-masking), also for nops == 1.  Pattern only (m / dp may be UINT64, dm BOOL; within a type dp wins over dm; an
+ * entry one type contributes survives another type's dm).  dp / dm may be NULL arrays or hold NULL entries.  Every operand and delta
+ * is square of one size n = ncols(F) (else GrB_DIMENSION_MISMATCH); nops < 1 is GrB_INVALID_VALUE; host-resident operands are
+ * GrB_NOT_IMPLEMENTED; with no device GxB_GPU_ERROR comes back before any host work.
+ * last_flops = sum_t flops(F*m[t]) + flops(F*dp[t]). */
+GrB_Info B200_Matrix_union_lmxm(GrB_Matrix F, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops);
+/* B200_traverse_batch over hop groups.  Operands are hop-major: hop h owns hop_nops[h] consecutive entries of m / dp / dm.
+ * hop_union[h] == 0: a delta hop (hop_nops[h] must be 1), B200_Matrix_delta_lmxm; else a union hop, B200_Matrix_union_lmxm over
+ * its operands.  Outputs, formats, GrB_INSUFFICIENT_SPACE and flops as B200_traverse_batch; operand errors as
+ * B200_Matrix_union_lmxm.  hop_nops == 1 and hop_union == 0 everywhere is B200_traverse_batch_delta. */
+GrB_Info B200_traverse_batch_union(const GrB_Index *sources, GrB_Index nsrc, const int *hop_nops, const int *hop_union, int nhops,
+                                   const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int format, uint64_t *out_bits,
+                                   uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
+                                   uint64_t *nvals_out, uint64_t *flops_out, int *format_out);
 /* Multi-source reachability in one call (SURVEY 8f-1: CondVarLenTraverse with emit_path = false, cond_var_len_traverse.rs:196;
  * AllShortestPaths' BFS phase, all_shortest_paths.rs:7-25): row i of *reached (new nsrc x n BOOL matrix) = the vertices reachable
  * from sources[i] by 1..max_hops edges of the square matrix A (max_hops < 0: to the fixed point); include_sources adds the
@@ -370,7 +386,8 @@ uint64_t B200_get_stat(const char *name);
 void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
- * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair".  0 on success. */
+ * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", and the accumulating
+ * products of union hops, "bits_pull_acc" and "bits_push_acc".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
