@@ -92,6 +92,7 @@ def lib():
         "B200_Matrix_union_lmxm": [P, P, P, P, C.c_int],
         "B200_traverse_batch_union": [P, U64, P, P, C.c_int, P, P, P, C.c_int, P, U64, P, P, U64, C.POINTER(U64), C.POINTER(U64),
                                       C.POINTER(C.c_int)],
+        "B200_expand_edges": [P, P, U64, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, U64, C.POINTER(U64)],
         "B200_set_option": [C.c_char_p, I64],
         "B200_Matrix_extract_pairs": [P, P, P, U64, P, P],
         "B200_Matrix_rmat_block": [C.POINTER(P), C.c_int, U64, U64, U64, U64, C.c_int],

@@ -1,0 +1,328 @@
+// edges.cu -- relationship ids of named-edge, incoming and bidirectional hops (B200_expand_edges): the edges CondTraverse's
+// expand_row / bind_edge and ExpandInto read one Tensor::get at a time (cond_traverse.rs:663-702, 844-935, expand_into.rs:121-258),
+// for a whole batch of rows in one pass over the tensors' live layers.
+//
+// Lists.  Row i, block b (forward: out-neighbours; reverse: in-neighbours), type t and layer l (0 = the base m / mt, 1 = the
+// delta-plus dp / mt_dp) own one list: the layer's row sources[i], or with targets only its entry at targets[i] (0 or 1 entry).
+// Lists are laid out flat in (row, block, type, layer) order behind an exclusive scan of their lengths, and every pass runs one
+// thread per list entry, so a hub row is spread over the whole grid like any other.
+// Count.  A base entry shadowed by its delta-minus or delta-plus layer counts 0.  A forward entry's value is its layer value; a
+// reverse entry (k in row s of mt) looks its value up at forward (k, s) with Tensor::eff_get's rule.  The count is 1, or for a
+// MULTI_EDGE value the size of the key's merged id list (me \ me_dm) u me_dp.  EDGES_FIRST keeps 1 for the first type present
+// at a neighbour and 0 for the others.
+// Place.  Lists are sorted by neighbour, so an entry's output position is the block's offset plus, per list of its block, the
+// counts of the entries ahead of it -- smaller neighbours, and the same neighbour in a lower-index type -- read from the scan of
+// the counts with one binary search per list (2T per entry; ewise.cu's rank sums).  No sort and no merge loop.
+// Fill.  node, id, type and direction of every output entry; a MULTI_EDGE entry writes its merged id list.
+// The me layers are host-resident (2^60 x 2^60); their sorted (key, ids) stores are uploaded once and cached on the handle.
+#include "common.cuh"
+#include "ops.cuh"
+
+namespace b200 {
+
+static const u64 EE_MULTI = ~0ULL;   // Tensor's MULTI_EDGE value (tensor.rs:206)
+
+struct ECsr { const u64 *p; const u32 *j; const u64 *x; };          // p null: the layer is absent
+struct EStore { const u64 *key; const u64 *ptr; const u64 *id; u64 nkey; };
+struct EType { ECsr m, dp, dm, mt, mtdp, mtdm; EStore me, medp, medm; };
+struct EArgs {
+    const u64 *src, *tgt;            // tgt null: every neighbour
+    const EType *types;
+    u64 n, G, E;                     // rows, lists, list entries
+    u32 T, nb;                       // types, blocks per row
+    int dir;
+};
+
+static ECsr ecsr(const DevCSR *A) {
+    if (!A || !A->nnz) return ECsr{nullptr, nullptr, nullptr};
+    return ECsr{A->p.ptr, A->j.ptr, A->x.ptr};
+}
+static EStore estore(const DevIdStore *S) {
+    if (!S || !S->nkey) return EStore{nullptr, nullptr, nullptr, 0};
+    return EStore{S->key.ptr, S->ptr.ptr, S->id.ptr, S->nkey};
+}
+
+__device__ __forceinline__ u64 lb32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
+    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] < c) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+__device__ __forceinline__ u64 ub32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
+    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] <= c) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+// position of (r, c) in A, or ~0
+__device__ __forceinline__ u64 find_rc(const ECsr &A, u64 r, u32 c) {
+    if (!A.p) return ~0ULL;
+    const u64 e = A.p[r + 1], q = lb32(A.j, A.p[r], e, c);
+    return q < e && A.j[q] == c ? q : ~0ULL;
+}
+// Tensor::eff_get (tensor.rs:290-303): dp if present, else nothing if dm holds it, else m
+__device__ __forceinline__ bool eff_get(const EType &t, u64 r, u32 c, u64 *v) {
+    u64 q = find_rc(t.dp, r, c);
+    if (q != ~0ULL) { *v = t.dp.x[q]; return true; }
+    if (find_rc(t.dm, r, c) != ~0ULL) return false;
+    q = find_rc(t.m, r, c);
+    if (q == ~0ULL) return false;
+    *v = t.m.x[q];
+    return true;
+}
+__device__ __forceinline__ void key_range(const EStore &S, u64 key, u64 *lo, u64 *hi) {
+    *lo = *hi = 0;
+    if (!S.nkey) return;
+    u64 a = 0, b = S.nkey;
+    while (a < b) { u64 mid = (a + b) >> 1; if (S.key[mid] < key) a = mid + 1; else b = mid; }
+    if (a < S.nkey && S.key[a] == key) { *lo = S.ptr[a]; *hi = S.ptr[a + 1]; }
+}
+// the key's ids in (me \ me_dm) u me_dp, ascending, handed to f until it returns false; returns how many were handed
+template <class F>
+__device__ u64 merged_ids(const EType &t, u64 key, F f) {
+    u64 a, ae, d, de, p, pe;
+    key_range(t.me, key, &a, &ae);
+    key_range(t.medm, key, &d, &de);
+    key_range(t.medp, key, &p, &pe);
+    u64 k = 0;
+    while (true) {
+        while (a < ae) {                                     // skip deleted base ids
+            const u64 va = t.me.id[a];
+            while (d < de && t.medm.id[d] < va) d++;
+            if (d < de && t.medm.id[d] == va) a++; else break;
+        }
+        const bool ha = a < ae, hp = p < pe;
+        if (!ha && !hp) break;
+        const u64 va = ha ? t.me.id[a] : 0, vp = hp ? t.medp.id[p] : 0;
+        u64 v;
+        if (ha && (!hp || va <= vp)) { v = va; a++; if (hp && vp == va) p++; }
+        else { v = vp; p++; }
+        k++;
+        if (!f(k - 1, v)) break;
+    }
+    return k;
+}
+
+struct ListId { u64 i; u32 b, t, l; bool rev; };
+__device__ __forceinline__ ListId list_of(const EArgs &A, u64 g) {
+    ListId r;
+    r.l = (u32)(g & 1);
+    u64 q = g >> 1;
+    r.t = (u32)(q % A.T); q /= A.T;
+    r.b = (u32)(q % A.nb);
+    r.i = q / A.nb;
+    r.rev = A.dir == 1 || (A.dir == 2 && r.b == 1);
+    return r;
+}
+__device__ __forceinline__ const ECsr &layer_of(const EType &t, bool rev, u32 l) { return rev ? (l ? t.mtdp : t.mt) : (l ? t.dp : t.m); }
+// largest g with lstart[g] <= e (lstart ascending, lstart[0] = 0)
+__device__ __forceinline__ u64 list_at(const u64 *__restrict__ lstart, u64 G, u64 e) {
+    u64 lo = 0, hi = G - 1;
+    while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (lstart[mid] <= e) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
+// per list: its first position in the layer's col_idx and its length.  stat[0] += forward entries, stat[1] += reverse entries,
+// stat[2] += entries of the delta-minus rows the count pass searches (the byte formula)
+__global__ void k_ee_lists(EArgs A, u64 *__restrict__ lo, u64 *__restrict__ len, u64 *__restrict__ stat) {
+    for (u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x; g < A.G; g += (u64)gridDim.x * blockDim.x) {
+        const ListId L = list_of(A, g);
+        const EType &t = A.types[L.t];
+        const ECsr &X = layer_of(t, L.rev, L.l);
+        const u64 s = A.src[L.i];
+        u64 a = 0, n = 0;
+        if (X.p) {
+            a = X.p[s];
+            u64 e = X.p[s + 1];
+            if (A.tgt) { const u32 c = (u32)A.tgt[L.i]; a = lb32(X.j, a, e, c); e = a < e && X.j[a] == c ? a + 1 : a; }
+            n = e - a;
+        }
+        lo[g] = a; len[g] = n;
+        if (n) atomicAdd((unsigned long long *)&stat[L.rev ? 1 : 0], (unsigned long long)n);
+        const ECsr &D = L.rev ? t.mtdm : t.dm;
+        if (L.l == 0 && D.p && D.p[s + 1] > D.p[s]) atomicAdd((unsigned long long *)&stat[2], (unsigned long long)(D.p[s + 1] - D.p[s]));
+    }
+}
+
+// per entry: value and count (ALL semantics)
+__global__ void k_ee_count(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo, u64 *__restrict__ val,
+                           u32 *__restrict__ cnt) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < A.E; e += (u64)gridDim.x * blockDim.x) {
+        const u64 g = list_at(lstart, A.G, e);
+        const ListId L = list_of(A, g);
+        const EType &t = A.types[L.t];
+        const ECsr &X = layer_of(t, L.rev, L.l);
+        const u64 s = A.src[L.i], q = lo[g] + (e - lstart[g]);
+        const u32 x = X.j[q];
+        u32 c = 0;
+        u64 v = 0;
+        bool live = !(A.dir == 2 && L.rev && x == s);                         // BOTH: a self-loop once, in the forward block
+        if (live && L.l == 0)                                                  // a base entry the deltas shadow
+            live = find_rc(L.rev ? t.mtdm : t.dm, s, x) == ~0ULL && find_rc(L.rev ? t.mtdp : t.dp, s, x) == ~0ULL;
+        if (live) {
+            if (!L.rev) v = X.x[q];
+            else live = eff_get(t, x, (u32)s, &v);                             // in-neighbour x: the forward pair (x, s)
+        }
+        if (live) {
+            if (v != EE_MULTI) c = 1;
+            else {
+                const u64 key = L.rev ? ((u64)x << 32 | s) : (s << 32 | x);
+                c = (u32)merged_ids(t, key, [](u64, u64) { return true; });
+            }
+        }
+        val[e] = v; cnt[e] = c;
+    }
+}
+
+// entry e of list g: where neighbour x sits in list g2 of the same block -- the entries ahead of it (< x, or <= x for a
+// lower-index type) as a flat position
+__device__ __forceinline__ u64 rank_in(const EArgs &A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo,
+                                       const u64 *__restrict__ len, u64 g2, bool rev, u32 x, bool upper) {
+    const ListId L2 = list_of(A, g2);
+    const ECsr &X = layer_of(A.types[L2.t], rev, L2.l);
+    const u64 a = lo[g2], b = a + len[g2];
+    if (a == b) return lstart[g2];
+    const u64 k = upper ? ub32(X.j, a, b, x) : lb32(X.j, a, b, x);
+    return lstart[g2] + (k - a);
+}
+
+// EDGES_FIRST: an entry keeps 1 when no lower-index type of its block holds a counted entry at the same neighbour
+__global__ void k_ee_first(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo, const u64 *__restrict__ len,
+                           const u32 *__restrict__ cnt, u32 *__restrict__ first) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < A.E; e += (u64)gridDim.x * blockDim.x) {
+        u32 keep = 0;
+        if (cnt[e]) {
+            const u64 g = list_at(lstart, A.G, e);
+            const ListId L = list_of(A, g);
+            const u32 x = layer_of(A.types[L.t], L.rev, L.l).j[lo[g] + (e - lstart[g])];
+            const u64 blk = g - (g % (2 * (u64)A.T));
+            keep = 1;
+            for (u32 t2 = 0; t2 < L.t && keep; t2++)
+                for (u32 l2 = 0; l2 < 2; l2++) {
+                    const u64 g2 = blk + 2 * t2 + l2;
+                    const u64 e2 = rank_in(A, lstart, lo, len, g2, L.rev, x, false);
+                    const ListId M = list_of(A, g2);
+                    const ECsr &X = layer_of(A.types[M.t], L.rev, M.l);
+                    if (e2 < lstart[g2] + len[g2] && X.j[lo[g2] + (e2 - lstart[g2])] == x && cnt[e2]) { keep = 0; break; }
+                }
+        }
+        first[e] = keep;
+    }
+}
+
+// out_p[i] = the output position of row i's first list (i = n: the total)
+__global__ void k_ee_rowptr(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ pos, u64 *__restrict__ out_p) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= A.n; i += (u64)gridDim.x * blockDim.x)
+        out_p[i] = pos[lstart[i * A.nb * 2 * A.T]];
+}
+
+__global__ void k_ee_fill(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo, const u64 *__restrict__ len,
+                          const u64 *__restrict__ val, const u32 *__restrict__ cnt, const u64 *__restrict__ pos,
+                          u32 *__restrict__ node, u64 *__restrict__ edge, uint16_t *__restrict__ type, uint8_t *__restrict__ rev) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < A.E; e += (u64)gridDim.x * blockDim.x) {
+        const u32 c = cnt[e];
+        if (!c) continue;
+        const u64 g = list_at(lstart, A.G, e);
+        const ListId L = list_of(A, g);
+        const EType &t = A.types[L.t];
+        const u32 x = layer_of(t, L.rev, L.l).j[lo[g] + (e - lstart[g])];
+        const u64 blk = g - (g % (2 * (u64)A.T));
+        u64 o = pos[lstart[blk]];                                              // row offset + the blocks before this one
+        for (u32 t2 = 0; t2 < A.T; t2++)
+            for (u32 l2 = 0; l2 < 2; l2++) {
+                const u64 g2 = blk + 2 * t2 + l2;
+                const u64 e2 = g2 == g ? e : rank_in(A, lstart, lo, len, g2, L.rev, x, t2 < L.t);
+                o += pos[e2] - pos[lstart[g2]];
+            }
+        const u64 v = val[e];
+        auto put = [&](u64 k, u64 id) {
+            node[o + k] = x;
+            edge[o + k] = id;
+            if (type) type[o + k] = (uint16_t)L.t;
+            if (rev) rev[o + k] = L.rev ? 1 : 0;
+            return k + 1 < c;
+        };
+        if (v != EE_MULTI) put(0, v);
+        else {
+            const u64 s = A.src[L.i];
+            merged_ids(t, L.rev ? ((u64)x << 32 | s) : (s << 32 | x), put);
+        }
+    }
+}
+
+void DevIdStore::upload(const u64 *hkey, const u64 *hptr, const u64 *hid, u64 nk) {
+    clear();
+    nkey = nk;
+    if (nk) {
+        key.alloc(nk); ptr.alloc(nk + 1); id.alloc(hptr[nk]);
+        h2d(key.ptr, hkey, nk); h2d(ptr.ptr, hptr, nk + 1); h2d(id.ptr, hid, hptr[nk]);
+        sync_stream();                                   // the host vectors are pageable
+    }
+    valid = true;
+}
+
+u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<EdgeTypeDev> &types, int dir, int mode, u64 *out_p,
+                u32 *out_node, u64 *out_edge, uint16_t *out_type, uint8_t *out_rev, u64 capacity) {
+    const u32 T = (u32)types.size(), nb = dir == 2 ? 2 : 1;
+    std::vector<EType> ht(T);
+    for (u32 t = 0; t < T; t++) {
+        const EdgeTypeDev &x = types[t];
+        ht[t] = EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
+                      estore(x.me_dm)};
+    }
+    DevBuf<EType> dt(T);
+    h2d(dt.ptr, ht.data(), T);
+    EArgs A{d_src, d_tgt, dt.ptr, n, n * nb * T * 2, 0, T, nb, dir};
+    const u32 grid = (u32)ctx().num_sms * 8;
+    DevBuf<u64> out(n + 1);
+    if (n == 0) {
+        out.zero();
+        d2h(out_p, out.ptr, 1);
+        sync_stream();
+        return 0;
+    }
+    DevBuf<u64> lo(A.G), llen(A.G + 1), lstart(A.G + 1), stat(3);
+    stat.zero();
+    // Compulsory bytes ("edge_expand"): 16 per list (its row pointers), 12 per forward entry (column + value), 28 per reverse
+    // entry (column 4, plus its forward point lookup: row pointers 16, value 8), 4 per entry of the delta-minus rows searched,
+    // and 14 per output entry (node 4, id 8, type 2), 15 with the direction.
+    TimedScope ts(TK_EDGE_EXPAND, 0);
+    CUDA_TRY(cudaMemsetAsync(llen.ptr + A.G, 0, sizeof(u64), stream()));
+    LAUNCH(k_ee_lists, grid_for(A.G, 256, grid), 256, 0, A, lo.ptr, llen.ptr, stat.ptr);
+    exclusive_scan_u64(llen.ptr, lstart.ptr, A.G + 1);
+    u64 h[4];
+    d2h(h, stat.ptr, 3);
+    d2h(h + 3, lstart.ptr + A.G, 1);
+    sync_stream();
+    A.E = h[3];
+    DevBuf<u64> val(A.E), pos(A.E + 1);
+    DevBuf<u32> cnt(A.E + 1), first;
+    u32 *fin = cnt.ptr;
+    CUDA_TRY(cudaMemsetAsync(cnt.ptr + A.E, 0, sizeof(u32), stream()));
+    if (A.E) LAUNCH(k_ee_count, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, val.ptr, cnt.ptr);
+    if (mode == 1 && A.E) {
+        first.alloc(A.E + 1);
+        CUDA_TRY(cudaMemsetAsync(first.ptr + A.E, 0, sizeof(u32), stream()));
+        LAUNCH(k_ee_first, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, llen.ptr, cnt.ptr, first.ptr);
+        fin = first.ptr;
+    }
+    exclusive_scan_u32_to_u64(fin, pos.ptr, A.E + 1);
+    LAUNCH(k_ee_rowptr, grid_for(n + 1, 256, grid), 256, 0, A, lstart.ptr, pos.ptr, out.ptr);
+    d2h(out_p, out.ptr, n + 1);
+    sync_stream();
+    const u64 total = out_p[n];
+    ts.bytes = 16 * A.G + 12 * h[0] + 28 * h[1] + 4 * h[2] + (out_rev ? 15 : 14) * total;
+    if (total > capacity || total == 0) return total;
+    DevBuf<u32> dnode(total);
+    DevBuf<u64> dedge(total);
+    DevBuf<uint16_t> dtype;
+    DevBuf<uint8_t> drev;
+    if (out_type) dtype.alloc(total);
+    if (out_rev) drev.alloc(total);
+    LAUNCH(k_ee_fill, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, llen.ptr, val.ptr, fin, pos.ptr, dnode.ptr, dedge.ptr,
+           dtype.ptr, drev.ptr);
+    d2h(out_node, dnode.ptr, total);
+    d2h(out_edge, dedge.ptr, total);
+    if (out_type) d2h(out_type, dtype.ptr, total);
+    if (out_rev) d2h(out_rev, drev.ptr, total);
+    sync_stream();
+    return total;
+}
+
+} // namespace b200

@@ -141,6 +141,7 @@ struct GB_Matrix_opaque : UObject {
     DevCSR devT;
     PullTables pt;   // pull-direction tables of devT (bits.cu)
     DevBuf<u32> bfs_deg; u64 bfs_edges = 0; bool bfs_deg_valid = false;   // out-degree table of the BFS engine (bfs_do.cu)
+    DevIdStore ids;  // device copy of the host store, for a Tensor's multi-edge layers (B200_expand_edges)
     int sparsity_control = GxB_HYPERSPARSE | GxB_SPARSE | GxB_BITMAP | GxB_FULL;
     int hyper_hash = 1;
     int orientation = GrB_ROWMAJOR;
@@ -246,6 +247,9 @@ static void invalidate_aux(GrB_Matrix A) {
     A->devT_valid = false;
     A->devT.clear();
     A->pt.clear();
+    // every change of the stored entries passes through here: set_dev / set_bits / set_empty (clear, build, element-wise
+    // results, container load / unload), finish_pending (setElement / removeElement) and resize
+    A->ids.clear();
 }
 
 static void set_dev(GrB_Matrix A, DevCSR &&d) {
@@ -2787,6 +2791,78 @@ GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, G
     GrB_Info info = guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; });   // no device: fail before any host work
     if (info) return info;
     return reach_impl(reached, sources, nsrc, m, dp, dm, nops, max_hops, include_sources, levels_out);
+}
+
+// ---- relationship ids of a batch of rows (expand_row / bind_edge / ExpandInto's Tensor::get, cond_traverse.rs:663-702, 844-935,
+// expand_into.rs:121-258) in one call: edges.cu.  The me layers stay host-resident; their stores go to the device once per handle
+// and change (GB_Matrix_opaque::ids, dropped by invalidate_aux).
+static const DevIdStore *id_store(GrB_Matrix A) {
+    if (!A) return nullptr;
+    ensure_host(A);
+    if (!A->ids.valid) {
+        const HostStore &h = A->host;
+        A->ids.upload(h.hrow.data(), h.hptr.data(), h.hcol.data(), h.hrow.size());
+    }
+    return &A->ids;
+}
+
+GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, GrB_Index n, const B200_TensorLayers *types,
+                           int ntypes, int dir, int mode, uint64_t *out_p, uint32_t *out_node, uint64_t *out_edge,
+                           uint16_t *out_type, uint8_t *out_rev, uint64_t out_capacity, uint64_t *nout) {
+    CHECK_PTR(types); CHECK_PTR(out_p); CHECK_PTR(nout);
+    if (n) CHECK_PTR(sources);
+    if (out_capacity) { CHECK_PTR(out_node); CHECK_PTR(out_edge); }
+    if (ntypes < 1 || ntypes > 65536 || dir < B200_DIR_OUT || dir > B200_DIR_BOTH || mode < B200_EDGES_ALL || mode > B200_EDGES_FIRST) {
+        tl_error = "expand_edges: ntypes outside 1 .. 65536 (out_type is 16 bits), or dir / mode out of range"; return GrB_INVALID_VALUE;
+    }
+    for (int t = 0; t < ntypes; t++) {
+        const B200_TensorLayers &L = types[t];
+        CHECK_MAT(L.m);
+        for (GrB_Matrix X : {L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) if (X) CHECK_MAT(X);
+        if (dir != B200_DIR_OUT && !L.mt) { tl_error = "expand_edges: incoming edges need the transpose mt"; return GrB_NULL_POINTER; }
+        if (L.m->type != T_UINT64 || (L.dp && L.dp->type != T_UINT64)) {
+            tl_error = "expand_edges: the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
+        }
+    }
+    const u64 nv = types[0].m->nrows;
+    for (int t = 0; t < ntypes; t++) {
+        const B200_TensorLayers &L = types[t];
+        for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm})
+            if (X && (X->nrows != nv || X->ncols != nv)) {
+                tl_error = "expand_edges: forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+            }
+    }
+    if (is_huge(types[0].m)) { tl_error = "expand_edges: host-resident forward or transpose layers"; return GrB_NOT_IMPLEMENTED; }
+    for (u64 i = 0; i < n; i++)
+        if (sources[i] >= nv || (targets && targets[i] >= nv)) { tl_error = "expand_edges: vertex id out of range"; return GrB_INVALID_INDEX; }
+    GrB_Info info = device_ready();             // no device: fail before any host work
+    if (info) return info;
+    return guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (int t = 0; t < ntypes; t++) {
+            const B200_TensorLayers &L = types[t];
+            for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) all.push_back(X);
+        }
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
+        std::vector<EdgeTypeDev> td(ntypes);
+        for (int t = 0; t < ntypes; t++) {
+            const B200_TensorLayers &L = types[t];
+            const bool rev = dir != B200_DIR_OUT;
+            td[t] = EdgeTypeDev{dev(L.m), dev(L.dp), dev(L.dm), rev ? dev(L.mt) : nullptr, rev ? dev(L.mt_dp) : nullptr,
+                                rev ? dev(L.mt_dm) : nullptr, id_store(L.me), id_store(L.me_dp), id_store(L.me_dm)};
+        }
+        DevBuf<u64> ds(n), dtg(targets ? n : 0);
+        h2d(ds.ptr, (const u64 *)sources, n);
+        if (targets) h2d(dtg.ptr, (const u64 *)targets, n);
+        const u64 total = edge_expand(ds.ptr, targets ? dtg.ptr : nullptr, n, td, dir, mode, out_p, out_node, out_edge, out_type,
+                                      out_rev, out_capacity);
+        *nout = total;
+        if (total > out_capacity) { tl_error = "expand_edges: output capacity too small (*nout = entries needed)"; return GrB_INSUFFICIENT_SPACE; }
+        return GrB_SUCCESS;
+    });
 }
 
 // returns every cached device block to the driver (the caching allocator otherwise keeps freed blocks for reuse)

@@ -111,6 +111,128 @@ inline void traverse_coalesced(const std::vector<uint64_t> &rows, const std::vec
         for (uint64_t q = p[r]; q < p[r + 1]; q++) { out_row.push_back(rows[r]); out_dest.push_back(j[q]); }
 }
 
+// ---- relationship ids: named-edge, incoming and bidirectional hops (B200_expand_edges) ----
+// Row i of a batch covers p[i] .. p[i+1]: the neighbour, the edge id, the type index and whether the entry belongs to the reverse
+// block; forward block first, inside a block neighbour, type index, id ascending.
+struct EdgeExpansion {
+    std::vector<uint64_t> p{0};
+    std::vector<uint32_t> node;
+    std::vector<uint64_t> edge;
+    std::vector<uint16_t> type;
+    std::vector<uint8_t> rev;
+    void push(uint64_t d, uint64_t id, size_t t, bool r) { node.push_back((uint32_t)d); edge.push_back(id); type.push_back((uint16_t)t); rev.push_back(r); }
+    void end_row() { p.push_back(edge.size()); }
+};
+
+// every row's relationships in one library call, each type's layers passed after Tensor::wait()
+inline EdgeExpansion expand_edges(const std::vector<uint64_t> &srcs, const std::vector<uint64_t> *targets,
+                                  const std::vector<const Tensor *> &types, int dir, int mode) {
+    std::vector<B200_TensorLayers> ls;
+    for (const Tensor *t : types) {
+        t->wait();
+        t->fwd_m().wait(); t->fwd_dp().wait(); t->fwd_dm().wait();
+        const VersionedMatrix &mt = t->matrix_t(), &me = t->edge_versioned();
+        mt.wait_all(); me.wait_all();
+        ls.push_back(B200_TensorLayers{t->fwd_m().inner(), t->fwd_dp().inner(), t->fwd_dm().inner(), mt.m().inner(), mt.dp().inner(),
+                                       mt.dm().inner(), me.m().inner(), me.dp().inner(), me.dm().inner()});
+    }
+    EdgeExpansion r;
+    const size_t n = srcs.size();
+    r.p.assign(n + 1, 0);
+    r.node.resize(std::max<size_t>(1024, 4 * n));
+    uint64_t nv = 0;
+    for (int attempt = 0; attempt < 2; attempt++) {              // a result larger than the first guess is rerun into its size
+        r.edge.resize(r.node.size()); r.type.resize(r.node.size()); r.rev.resize(r.node.size());
+        GrB_Info info = B200_expand_edges(srcs.data(), targets ? targets->data() : nullptr, n, ls.data(), (int)ls.size(), dir, mode,
+                                          r.p.data(), r.node.data(), r.edge.data(), r.type.data(), r.rev.data(), r.node.size(), &nv);
+        if (info == GrB_INSUFFICIENT_SPACE && attempt == 0) { r.node.resize(nv); continue; }
+        grb_ok(info, "B200_expand_edges");
+        break;
+    }
+    r.node.resize(nv); r.edge.resize(nv); r.type.resize(nv); r.rev.resize(nv);
+    return r;
+}
+
+// process_pairs' edge loop for one (src, dst) pair of a block (cond_traverse.rs:1084-1113 emit_relationship, :676-687 bind_edge):
+// the pair's ids per type in edge_type_indices order, all of them or the first
+inline void emit_pair_edges(const std::vector<const Tensor *> &types, uint64_t src, uint64_t dst, uint64_t nbr, bool rev, bool first,
+                            EdgeExpansion &r) {
+    for (size_t t = 0; t < types.size(); t++) {
+        for (uint64_t id : types[t]->get(src, dst)) {
+            r.push(nbr, id, t, rev);
+            if (first) return;
+        }
+    }
+}
+
+// the neighbours a seeked structural iterator over the types yields for `row`, ascending: the forward layers (fwd_iter) or the
+// maintained transpose (build_transposed_iter, cond_traverse.rs:221-235)
+inline std::vector<uint64_t> row_neighbours(const std::vector<const Tensor *> &types, uint64_t row, bool transposed) {
+    std::vector<uint64_t> out;
+    for (const Tensor *t : types) {
+        if (transposed) {
+            auto it = t->matrix_t().iter(row, row);
+            std::tuple<uint64_t, uint64_t> e;
+            while (it.next(e)) out.push_back(std::get<1>(e));
+        } else {
+            auto it = t->fwd_iter(row, row);
+            std::tuple<uint64_t, uint64_t, uint64_t> e;
+            while (it.next(e)) out.push_back(std::get<1>(e));
+        }
+    }
+    std::sort(out.begin(), out.end());
+    out.erase(std::unique(out.begin(), out.end()), out.end());
+    return out;
+}
+
+// expand_row's edge loops restated statement for statement (cond_traverse.rs:844-935): forward pairs from the structural iterator
+// seeked at the source, reverse pairs from matrix_t()'s iterator (self-loops skipped under BOTH), ids by Tensor::get.  The route
+// B200_expand_edges replaces; tests compare against it.
+inline EdgeExpansion expand_edges_by_get(const std::vector<uint64_t> &srcs, const std::vector<const Tensor *> &types, int dir, int mode) {
+    EdgeExpansion r;
+    const bool first = mode == B200_EDGES_FIRST;
+    for (uint64_t s : srcs) {
+        if (dir != B200_DIR_IN)
+            for (uint64_t d : row_neighbours(types, s, false)) emit_pair_edges(types, s, d, d, false, first, r);
+        if (dir != B200_DIR_OUT)
+            for (uint64_t k : row_neighbours(types, s, true)) {
+                if (dir == B200_DIR_BOTH && k == s) continue;
+                emit_pair_edges(types, k, s, k, true, first, r);
+            }
+        r.end_row();
+    }
+    return r;
+}
+
+// ExpandInto with the edge bound (expand_into.rs:121-258): Tensor::get on (src, dst), and under BOTH on (dst, src) when they differ
+inline EdgeExpansion expand_into_by_get(const std::vector<uint64_t> &srcs, const std::vector<uint64_t> &dsts,
+                                        const std::vector<const Tensor *> &types, int dir, int mode) {
+    EdgeExpansion r;
+    const bool first = mode == B200_EDGES_FIRST;
+    for (size_t i = 0; i < srcs.size(); i++) {
+        const uint64_t s = srcs[i], d = dsts[i];
+        if (dir != B200_DIR_IN) emit_pair_edges(types, s, d, d, false, first, r);
+        if (dir == B200_DIR_IN || (dir == B200_DIR_BOTH && d != s)) emit_pair_edges(types, d, s, d, true, first, r);
+        r.end_row();
+    }
+    return r;
+}
+
+// today's bind_edge route on the batched path (cond_traverse.rs:600-608, 663-702): the (row, dest) pairs of one union hop over
+// the types (B200_traverse_batch_union), then one Tensor::get per pair for its first id
+inline EdgeExpansion bind_edge_after_traverse(const std::vector<uint64_t> &srcs, const std::vector<const Tensor *> &types) {
+    std::vector<uint64_t> rows(srcs.size()), out_row, out_dest;
+    for (size_t i = 0; i < rows.size(); i++) rows[i] = i;
+    traverse_coalesced(rows, srcs, {TraversalMatrix(types)}, out_row, out_dest);
+    EdgeExpansion r;
+    size_t q = 0;
+    for (size_t i = 0; i < srcs.size(); i++) {
+        for (; q < out_row.size() && out_row[q] == i; q++) emit_pair_edges(types, srcs[i], out_dest[q], out_dest[q], false, true, r);
+        r.end_row();
+    }
+    return r;
+}
+
 // fuse_dst_labels (SURVEY 8f-2): label matrices are diagonal (graph.rs:1191), so the destination filter F*A*L_dst
 // (graph.rs:2600-2626) is one more delta_lmxm against the label's VersionedMatrix -- a column filter in frontier form on
 // the device -- instead of a node_has_label probe (1-3 extractElement calls) per output pair on the host.

@@ -1045,4 +1045,68 @@ int fdbh_var_len_reach(void **tensors, uint64_t ntypes, int dir, const uint64_t 
 }
 void fdbh_free(void *p) { free(p); }
 
+// ---- a relationship Tensor for the edge-id routes: GRAPH.BULK's load, batched inserts and deletes with pending writes ----
+void *fdbh_tensor_bulk_load(uint64_t n, const uint64_t *srcs, const uint64_t *dsts, const uint64_t *ids, uint64_t k) {
+    try {
+        return new Tensor(Tensor::bulk_load(n, n, std::vector<uint64_t>(srcs, srcs + k), std::vector<uint64_t>(dsts, dsts + k),
+                                            std::vector<uint64_t>(ids, ids + k)));
+    } catch (const std::exception &e) { g_msg = e.what(); return nullptr; }
+}
+void fdbh_tensor_free(void *t) { delete (Tensor *)t; }
+int fdbh_tensor_set_all(void *t, const uint64_t *srcs, const uint64_t *dsts, const uint64_t *ids, uint64_t k) {
+    try {
+        ((Tensor *)t)->set_all_from_slices(std::vector<uint64_t>(srcs, srcs + k), std::vector<uint64_t>(dsts, dsts + k),
+                                           std::vector<uint64_t>(ids, ids + k));
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+int fdbh_tensor_remove_all(void *t, const uint64_t *ids, const uint64_t *srcs, const uint64_t *dsts, uint64_t k) {
+    try {
+        std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rels;
+        for (uint64_t q = 0; q < k; q++) rels.push_back(std::make_tuple(ids[q], srcs[q], dsts[q]));
+        ((Tensor *)t)->remove_all(rels);
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+// the nine layer handles (B200_TensorLayers order) after Tensor::wait(); borrowed, valid until the tensor changes
+int fdbh_tensor_layers(void *tp, void **out9) {
+    try {
+        const Tensor *t = (const Tensor *)tp;
+        t->wait();
+        const VersionedMatrix &mt = t->matrix_t(), &me = t->edge_versioned();
+        mt.wait_all(); me.wait_all();
+        GrB_Matrix h[9] = {t->fwd_m().inner(), t->fwd_dp().inner(), t->fwd_dm().inner(), mt.m().inner(), mt.dp().inner(),
+                           mt.dm().inner(), me.m().inner(), me.dp().inner(), me.dm().inner()};
+        for (int k = 0; k < 9; k++) out9[k] = h[k];
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+// The relationships of a batch of rows over Tensor pointers.  route 0: B200_expand_edges (expand_edges); 1: Tensor::get per pair
+// (expand_edges_by_get, or expand_into_by_get with targets); 2: B200_traverse_batch_union then a get per pair (bind_edge's route:
+// dir OUT, mode FIRST, no targets).  Outputs are malloc'ed; free with fdbh_free.
+int fdbh_expand_edges(void **tensors, uint64_t ntypes, const uint64_t *srcs, const uint64_t *tgts, uint64_t n, int dir, int mode,
+                      int route, uint64_t **out_p, uint32_t **out_node, uint64_t **out_edge, uint16_t **out_type, uint8_t **out_rev,
+                      uint64_t *nout) {
+    try {
+        std::vector<const Tensor *> types;
+        for (uint64_t k = 0; k < ntypes; k++) types.push_back((const Tensor *)tensors[k]);
+        std::vector<uint64_t> s(srcs, srcs + n), d;
+        if (tgts) d.assign(tgts, tgts + n);
+        EdgeExpansion r;
+        if (route == 0) r = expand_edges(s, tgts ? &d : nullptr, types, dir, mode);
+        else if (route == 1) r = tgts ? expand_into_by_get(s, d, types, dir, mode) : expand_edges_by_get(s, types, dir, mode);
+        else if (route == 2 && !tgts && dir == B200_DIR_OUT && mode == B200_EDGES_FIRST) r = bind_edge_after_traverse(s, types);
+        else throw std::invalid_argument("expand_edges: unknown route, or route 2 outside dir OUT / mode FIRST without targets");
+        const uint64_t m = r.edge.size();
+        *nout = m;
+        auto out = [](auto **dst, const auto &v) {
+            *dst = (std::remove_reference_t<decltype(**dst)> *)malloc(sizeof(**dst) * (v.size() + 1));
+            if (!*dst) throw std::bad_alloc();
+            memcpy(*dst, v.data(), sizeof(**dst) * v.size());
+        };
+        out(out_p, r.p); out(out_node, r.node); out(out_edge, r.edge); out(out_type, r.type); out(out_rev, r.rev);
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
 } // extern "C"

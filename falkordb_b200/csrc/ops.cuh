@@ -113,6 +113,23 @@ int cdlp(const DevCSR &A, int itermax, u64 *d_label);         // synchronous lab
 
 void probe_pairs(const DevCSR &A, const u64 *dI, const u64 *dJ, u64 n, unsigned char *d_found, u64 *d_val);
 
+// edges.cu : relationship ids of the rows of a batch over relationship tensors' live layers (B200_expand_edges)
+struct DevIdStore {   // a host-resident matrix's sorted store on the device: key[k] = a non-empty row, its columns id[ptr[k] .. ptr[k+1])
+    DevBuf<u64> key, ptr, id;
+    u64 nkey = 0;
+    bool valid = false;
+    void upload(const u64 *hkey, const u64 *hptr, const u64 *hid, u64 nk);
+    void clear() { key.release(); ptr.release(); id.release(); nkey = 0; valid = false; }
+};
+struct EdgeTypeDev {  // one relationship type: forward m / dp (u64 values) / dm, the transpose's layers, the multi-edge store's
+    const DevCSR *m, *dp, *dm, *mt, *mt_dp, *mt_dm;   // null or empty: absent
+    const DevIdStore *me, *me_dp, *me_dm;
+};
+// dir 0 out / 1 in / 2 both, mode 0 every id / 1 the first id per (row, block, neighbour).  d_tgt null: every neighbour.  Writes
+// out_p[0..n] and returns the number of output entries; the entries themselves only when they fit in capacity.
+u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<EdgeTypeDev> &types, int dir, int mode, u64 *out_p,
+                u32 *out_node, u64 *out_edge, uint16_t *out_type, uint8_t *out_rev, u64 capacity);
+
 // hypersparse host form <-> dense device rowptr (ewise.cu)
 void rowptr_from_hyper(const u64 *d_hrow, const u64 *d_hptr, u64 nvec, u64 nrows, u64 *d_p);
 u64 hyper_from_rowptr(const u64 *d_p, u64 nrows, u64 nnz, DevBuf<u64> &d_hrow, DevBuf<u64> &d_hptr);

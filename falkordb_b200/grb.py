@@ -520,3 +520,50 @@ def multi_source_reach(sources, A, max_hops=None, include_sources=False):
         level += 1
     return R, level
 
+
+
+DIR_OUT, DIR_IN, DIR_BOTH = 0, 1, 2
+EDGES_ALL, EDGES_FIRST = 0, 1
+TENSOR_LAYERS = ("m", "dp", "dm", "mt", "mt_dp", "mt_dm", "me", "me_dp", "me_dm")
+
+
+class TensorLayers(C.Structure):
+    """B200_TensorLayers (include/b200grb.h): one relationship type's nine layer handles"""
+    _fields_ = [(k, P) for k in TENSOR_LAYERS]
+
+
+def _handle(x):
+    return None if x is None else (x.h if isinstance(x, Matrix) else x)
+
+
+def expand_edges(sources, types, dir=DIR_OUT, mode=EDGES_ALL, targets=None, capacity=None):
+    """B200_expand_edges: the relationships of a batch of rows over relationship types, in one call.  `types`: one entry per type,
+    a sequence or dict of the nine layers in TENSOR_LAYERS order (Matrix, raw handle or None; m required, mt for DIR_IN / DIR_BOTH).
+    `targets` (same length as `sources`): row i covers only the neighbour targets[i] (ExpandInto).  Returns numpy arrays
+    (p uint64[n+1], node uint32, edge uint64, type uint16, rev uint8); a result larger than `capacity` (default: a guess) is run
+    once more into its size."""
+    sources = _u64arr(sources)
+    n = len(sources)
+    if targets is not None:
+        targets = _u64arr(targets)
+        assert len(targets) == n, "one target per source"
+    ls = (TensorLayers * max(1, len(types)))()
+    for k, t in enumerate(types):
+        vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
+        for name, x in zip(TENSOR_LAYERS, vals):
+            setattr(ls[k], name, _handle(x))
+    cap = max(1024, 4 * n) if capacity is None else int(capacity)
+    p, nv = np.zeros(n + 1, np.uint64), U64(0)
+    for attempt in (0, 1):
+        node, edge = np.zeros(max(cap, 1), np.uint32), np.zeros(max(cap, 1), np.uint64)
+        typ, rev = np.zeros(max(cap, 1), np.uint16), np.zeros(max(cap, 1), np.uint8)
+        info = lib().B200_expand_edges(sources.ctypes.data if n else None, None if targets is None else targets.ctypes.data, n, ls,
+                                       len(types), dir, mode, p.ctypes.data, node.ctypes.data, edge.ctypes.data, typ.ctypes.data,
+                                       rev.ctypes.data, cap, C.byref(nv))
+        if info == -103 and attempt == 0:        # GrB_INSUFFICIENT_SPACE: nv holds the entries needed
+            cap = nv.value
+            continue
+        check(info)
+        break
+    m = nv.value
+    return p, node[:m], edge[:m], typ[:m], rev[:m]

@@ -1,0 +1,93 @@
+"""ctypes binding of libfdbhost.so, the C++ host mirror of the reference's Tensor and CondTraverse (csrc/host): a relationship
+Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending, and the routes that read its
+relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get)."""
+import ctypes as C
+import os
+
+import numpy as np
+
+from ._lib import U64
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_L = None
+
+ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
+
+
+def host():
+    global _L
+    if _L is not None:
+        return _L
+    L = C.CDLL(os.path.join(_HERE, "libfdbhost.so"))
+    P = C.c_void_p
+    L.fdbh_tensor_bulk_load.argtypes = [U64, P, P, P, U64]
+    L.fdbh_tensor_bulk_load.restype = P
+    L.fdbh_tensor_free.argtypes = [P]
+    L.fdbh_tensor_set_all.argtypes = [P, P, P, P, U64]
+    L.fdbh_tensor_remove_all.argtypes = [P, P, P, P, U64]
+    L.fdbh_tensor_layers.argtypes = [P, P]
+    L.fdbh_expand_edges.argtypes = [P, U64, P, P, U64, C.c_int, C.c_int, C.c_int] + [P] * 5 + [C.POINTER(U64)]
+    L.fdbh_free.argtypes = [P]
+    L.fdbh_last_message.restype = C.c_char_p
+    _L = L
+    return L
+
+
+def _u64(*xs):
+    return [np.ascontiguousarray(x, dtype=np.uint64) for x in xs]
+
+
+class Tensor:
+    """csrc/host/tensor.hpp's Tensor over n vertices, loaded with the edges (src[k], dst[k], ids[k]) by Tensor::bulk_load"""
+
+    def __init__(self, n, src, dst, ids):
+        self.L = host()
+        a = _u64(src, dst, ids)
+        self.h = self.L.fdbh_tensor_bulk_load(n, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0]))
+        if not self.h:
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.L.fdbh_tensor_free(self.h)
+            self.h = None
+
+    def add(self, src, dst, ids):
+        """Tensor::set_all_from_slices"""
+        a = _u64(src, dst, ids)
+        if self.L.fdbh_tensor_set_all(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0])):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def remove(self, ids, src, dst):
+        """Tensor::remove_all"""
+        a = _u64(ids, src, dst)
+        if self.L.fdbh_tensor_remove_all(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0])):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def layers(self):
+        """the nine layer handles in B200_TensorLayers order, after Tensor::wait(); valid until the tensor changes"""
+        out = (C.c_void_p * 9)()
+        if self.L.fdbh_tensor_layers(self.h, out):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+        return [out[k] for k in range(9)]
+
+
+def expand_edges(tensors, sources, dir, mode, targets=None, route=ROUTE_BY_GET):
+    """fdbh_expand_edges over Tensor objects: (p, node, edge, type, rev) as numpy arrays"""
+    L = host()
+    (src,) = _u64(sources)
+    tg = None if targets is None else _u64(targets)[0]
+    ts = (C.c_void_p * len(tensors))(*[t.h for t in tensors])
+    ptrs = [C.c_void_p() for _ in range(5)]
+    nv = U64(0)
+    rc = L.fdbh_expand_edges(ts, len(tensors), src.ctypes.data, None if tg is None else tg.ctypes.data, len(src), dir, mode, route,
+                             *[C.byref(x) for x in ptrs], C.byref(nv))
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    m = nv.value
+    out = []
+    for x, dt, k in zip(ptrs, (np.uint64, np.uint32, np.uint64, np.uint16, np.uint8), (len(src) + 1, m, m, m, m)):
+        nbytes = k * np.dtype(dt).itemsize
+        out.append(np.frombuffer((C.c_char * nbytes).from_address(x.value), dt).copy() if k else np.zeros(0, dt))
+        L.fdbh_free(x)
+    return tuple(out)

@@ -378,6 +378,37 @@ GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Ind
 GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m,
                                 const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources,
                                 int64_t *levels_out);
+/* The layers of one relationship type's Tensor (tensor.rs:184-259), as B200_expand_edges reads them.  m / dp: forward UINT64 layers
+ * (value = the pair's edge id, or UINT64_MAX = MULTI_EDGE), dm BOOL; mt / mt_dp / mt_dm: the maintained transpose, BOOL; me / me_dp
+ * / me_dm: the multi-edge store (2^60 x 2^60 BOOL, row = src << 32 | dst, column = edge id).  Every layer but m may be NULL. */
+typedef struct {
+    GrB_Matrix m, dp, dm;
+    GrB_Matrix mt, mt_dp, mt_dm;
+    GrB_Matrix me, me_dp, me_dm;
+} B200_TensorLayers;
+#define B200_DIR_OUT 0
+#define B200_DIR_IN 1
+#define B200_DIR_BOTH 2
+#define B200_EDGES_ALL 0   /* one entry per relationship (emit_relationship) */
+#define B200_EDGES_FIRST 1 /* one entry per (row, direction, neighbour): the first id (bind_edge) */
+/* The relationships of a batch of rows over ntypes relationship types, in one call (CondTraverse's expand_row / bind_edge,
+ * ExpandInto's Tensor::get probes).  The value of a pair in one type is Tensor::eff_get's: dp if present, else none if dm holds
+ * it, else m; a MULTI_EDGE value stands for the key's ids in (me \ me_dm) u me_dp, ascending.
+ * Row i covers out_p[i] .. out_p[i+1] of out_node (the neighbour), out_edge (the id), out_type (index into types) and out_rev:
+ *  - B200_DIR_OUT: the effective out-neighbours d of sources[i] over the types;
+ *  - B200_DIR_IN: the in-neighbours k from each type's effective transpose row, ids looked up at forward (k, sources[i]);
+ *  - B200_DIR_BOTH: the forward block, then the reverse block without k == sources[i] (out_rev = 1 marks reverse entries);
+ *  - inside a block: neighbour ascending, then type index, then id.
+ * targets non-NULL: row i covers only the neighbour targets[i] (ExpandInto).  B200_EDGES_FIRST keeps, per (row, block,
+ * neighbour), the first entry of that order.  out_type / out_rev may be NULL.  out_p (n + 1 entries) is written in every case;
+ * the entries only when they fit out_capacity, else GrB_INSUFFICIENT_SPACE with *nout = the entries needed.
+ * Errors: ntypes outside 1 .. 65536, dir or mode out of range GrB_INVALID_VALUE; m not UINT64 (or dp not UINT64) GrB_DOMAIN_MISMATCH; forward and
+ * transpose layers not square of one size n GrB_DIMENSION_MISMATCH; an id >= n GrB_INVALID_INDEX; mt NULL under DIR_IN / DIR_BOTH
+ * GrB_NULL_POINTER; host-resident forward or transpose layers GrB_NOT_IMPLEMENTED (the me layers are host-resident: their stores
+ * are uploaded once and cached with the handle until it changes); with no device GxB_GPU_ERROR before any host work. */
+GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, GrB_Index n, const B200_TensorLayers *types,
+                           int ntypes, int dir, int mode, uint64_t *out_p, uint32_t *out_node, uint64_t *out_edge,
+                           uint16_t *out_type, uint8_t *out_rev, uint64_t out_capacity, uint64_t *nout);
 GrB_Info B200_sync(void);
 GrB_Info B200_pool_trim(void); /* hand the caching allocator's free device blocks back to the driver */
 void *B200_stream(void); /* the cudaStream_t every kernel of this library is launched on */
