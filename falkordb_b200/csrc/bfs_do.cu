@@ -18,6 +18,13 @@
 //
 // Without A' (one BFS on a fresh matrix, where building the mirror would cost more than the search) bfs_run runs a plain
 // top-down BFS on one GPU with the same level and min-id parent; it has no dest early exit.
+//
+// Over relationship operands with pending writes (one GPU) the same loop walks A = U_t (m_t \ dm_t) u dp_t without building it:
+// the kernels read a small array of operands {m, m', dp, dp', dm, dm'} (the DIRTY instantiations; DIRTY = false is the clean
+// engine above).  Top-down expands one list per (frontier vertex, operand, layer m / dp) and skips an m entry found in the
+// vertex's dm row; the parent and the bottom-up step take the minimum over the operands of the first frontier member in
+// m'(v,:) \ dm'(v,:) and in dp'(v,:).  The switch reads sum_t deg(m_t) + deg(dp_t), an upper bound of the effective out-degree:
+// it steers the direction only, levels and parents do not depend on it.
 #include "common.cuh"
 #include "ops.cuh"
 #include <nccl.h>
@@ -106,10 +113,62 @@ __device__ __forceinline__ u64 do_find_le(const u64 *__restrict__ a, u64 lo, u64
 }
 __device__ __forceinline__ bool bit_of(const u64 *__restrict__ b, u64 v) { return (b[v >> 6] >> (v & 63)) & 1ULL; }
 
+// one operand of the dirty BFS on the device: the base m and its transpose mirror, dp and dm and their transposes (p null: empty)
+struct BfsOpDev {
+    const u64 *mp, *mtp, *dpp, *dptp, *dmp, *dmtp;
+    const u32 *mj, *mtj, *dpj, *dptj, *dmj, *dmtj;
+};
+
+// the minimum-id frontier member of v's effective in-row, -1 if none, for one 8-lane group (every lane gets it).  Per operand
+// m'(v,:) minus dm'(v,:) -- both rows ascend, so each lane's lower bound in dm' only moves forward -- then dp'(v,:).  Rows
+// ascend, so a list stops at its first hit or once its entries pass the best hit so far.
+__device__ __forceinline__ i64 do_first_parent(const BfsOpDev *__restrict__ ops, u32 nops, u64 v, const u64 *__restrict__ frontier,
+                                               u32 lane8, u32 gmask) {
+    u64 best = ~0ULL;
+    for (u32 t = 0; t < nops; t++) {
+        for (int layer = 0; layer < 2; layer++) {
+            const u64 *Tp = layer ? ops[t].dptp : ops[t].mtp;
+            const u32 *Tj = layer ? ops[t].dptj : ops[t].mtj;
+            if (!Tp) continue;
+            const u64 s = Tp[v], e = Tp[v + 1];
+            u64 d = 0, de = 0;
+            const u32 *Dj = ops[t].dmtj;
+            if (!layer && ops[t].dmtp) { d = ops[t].dmtp[v]; de = ops[t].dmtp[v + 1]; }
+            for (u64 qb = s; qb < e && Tj[qb] < best; qb += 8) {
+                const u64 q = qb + lane8;
+                u32 u = 0;
+                bool hit = false;
+                if (q < e) {
+                    u = Tj[q];
+                    hit = u < best && bit_of(frontier, u);
+                    if (hit && d < de) {
+                        u64 lo = d, hi = de;
+                        while (lo < hi) { const u64 mid = (lo + hi) >> 1; if (Dj[mid] < u) lo = mid + 1; else hi = mid; }
+                        d = lo;
+                        if (d < de && Dj[d] == u) hit = false;      // a deleted edge
+                    }
+                }
+                const u32 m = __ballot_sync(gmask, hit) & gmask;
+                if (m) { best = __shfl_sync(gmask, u, __ffs(m) - 1); break; }
+            }
+        }
+    }
+    return best == ~0ULL ? -1 : (i64)best;
+}
+
 __global__ void k_do_deg32(const u64 *__restrict__ p, u64 nloc, u32 *__restrict__ deg) {
     u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
     for (; t < nloc; t += stride) { u64 d = p[t + 1] - p[t]; deg[t] = d > 0xFFFFFFFFULL ? 0xFFFFFFFFu : (u32)d; }
+}
+// deg += base (a base's cached table) + the row lengths of p (may be null), saturating
+__global__ void k_do_deg_add(const u32 *__restrict__ base, const u64 *__restrict__ p, u64 n, u32 *__restrict__ deg) {
+    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 stride = (u64)gridDim.x * blockDim.x;
+    for (; t < n; t += stride) {
+        const u64 d = (u64)deg[t] + base[t] + (p ? p[t + 1] - p[t] : 0);
+        deg[t] = d > 0xFFFFFFFFULL ? 0xFFFFFFFFu : (u32)d;
+    }
 }
 __global__ void k_do_init(i64 *__restrict__ level, i64 *__restrict__ parent, u64 nloc, u64 lo, u64 src) {
     u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -152,10 +211,28 @@ __global__ void k_do_frontier_deg(const u32 *__restrict__ fr, u64 nf, u64 lo, co
         start[t] = s;
     }
 }
-// top-down: every out-edge of the owned frontier vertices marks its unvisited target in `disc`
+// dirty top-down lists: list s = (frontier vertex s / nops2, operand (s % nops2) / 2, layer m / dp by s & 1)
+__global__ void k_do_frontier_deg_delta(const u32 *__restrict__ fr, u64 nseg, const BfsOpDev *__restrict__ ops, u32 nops2,
+                                        u64 *__restrict__ deg, u64 *__restrict__ start) {
+    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    u64 stride = (u64)gridDim.x * blockDim.x;
+    for (; t <= nseg; t += stride) {
+        if (t == nseg) { deg[t] = 0; break; }
+        const u32 r = (u32)(t % nops2);
+        const u64 *p = (r & 1) ? ops[r >> 1].dpp : ops[r >> 1].mp;
+        const u64 u = fr[t / nops2];
+        const u64 s = p ? p[u] : 0;
+        deg[t] = p ? p[u + 1] - s : 0;
+        start[t] = s;
+    }
+}
+// top-down: every out-edge of the owned frontier vertices marks its unvisited target in `disc`.  DIRTY: the lists of
+// k_do_frontier_deg_delta over the frontier `fr`; an m entry (u, v) in dm's row u is skipped (only a non-empty row searches).
+template <bool DIRTY>
 __global__ void __launch_bounds__(256)
 k_do_expand(const u64 *__restrict__ cum, const u64 *__restrict__ start, u64 nf, u64 total, const u32 *__restrict__ Aj,
-            const u64 *__restrict__ visited, u32 *__restrict__ disc) {
+            const u64 *__restrict__ visited, u32 *__restrict__ disc, const u32 *__restrict__ fr, const BfsOpDev *__restrict__ ops,
+            u32 nops2) {
     __shared__ u64 s_e0, s_e1;
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (u64 chunk = blockIdx.x; chunk * DO_CHUNK < total; chunk += gridDim.x) {
@@ -170,8 +247,24 @@ k_do_expand(const u64 *__restrict__ cum, const u64 *__restrict__ start, u64 nf, 
             const u64 t = t0 + lane;
             if (t < hi) {
                 while (e < e1 && cum[e + 1] <= t) e++;
-                const u32 v = Aj[start[e] + (t - cum[e])];
-                if (!bit_of(visited, v)) atomicOr(&disc[v >> 5], 1u << (v & 31));
+                if constexpr (DIRTY) {
+                    const u32 r = (u32)(e % nops2);
+                    const BfsOpDev &o = ops[r >> 1];
+                    const u32 v = ((r & 1) ? o.dpj : o.mj)[start[e] + (t - cum[e])];
+                    if (bit_of(visited, v)) continue;
+                    if (!(r & 1) && o.dmp) {
+                        const u64 u = fr[e / nops2];
+                        u64 lo = o.dmp[u], hi = o.dmp[u + 1];
+                        if (lo < hi) {
+                            while (lo < hi) { const u64 mid = (lo + hi) >> 1; if (o.dmj[mid] < v) lo = mid + 1; else hi = mid; }
+                            if (lo < o.dmp[u + 1] && o.dmj[lo] == v) continue;   // a deleted edge
+                        }
+                    }
+                    atomicOr(&disc[v >> 5], 1u << (v & 31));
+                } else {
+                    const u32 v = Aj[start[e] + (t - cum[e])];
+                    if (!bit_of(visited, v)) atomicOr(&disc[v >> 5], 1u << (v & 31));
+                }
             }
         }
     }
@@ -196,9 +289,12 @@ __global__ void k_do_scatter_lists(const u32 *__restrict__ lists, u64 total, con
     }
 }
 // top-down epilogue: each owned new vertex takes the level and its minimum-id parent = first frontier member of its A' row
+// (DIRTY: do_first_parent over the operands)
+template <bool DIRTY>
 __global__ void __launch_bounds__(256)
 k_do_assign(const u32 *__restrict__ list, u64 cnt, u64 lo, const u64 *__restrict__ ATp, const u32 *__restrict__ ATj,
-            const u64 *__restrict__ frontier, i64 *__restrict__ level, i64 *__restrict__ parent, i64 lvl) {
+            const u64 *__restrict__ frontier, i64 *__restrict__ level, i64 *__restrict__ parent, i64 lvl,
+            const BfsOpDev *__restrict__ ops, u32 nops) {
     const u32 lane8 = threadIdx.x & 7, sub = (threadIdx.x & 31) >> 3;
     const u32 gmask = 0xFFu << (8 * sub);
     u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
@@ -208,7 +304,9 @@ k_do_assign(const u32 *__restrict__ list, u64 cnt, u64 lo, const u64 *__restrict
         if (i >= cnt) continue;                      // uniform inside the 8-lane group
         const u64 r = list[i] - lo;
         i64 par = -1;
-        if (parent) {
+        if constexpr (DIRTY) {
+            if (parent) par = do_first_parent(ops, nops, r + lo, frontier, lane8, gmask);
+        } else if (parent) {
             const u64 s = ATp[r], e = ATp[r + 1];
             for (u64 qb = s; qb < e; qb += 8) {
                 const u64 q = qb + lane8;
@@ -223,9 +321,12 @@ k_do_assign(const u32 *__restrict__ list, u64 cnt, u64 lo, const u64 *__restrict
     }
 }
 // bottom-up: owned unvisited vertices look for a frontier in-neighbour; first hit in ascending order = minimum-id parent
+// (DIRTY: do_first_parent over the operands)
+template <bool DIRTY>
 __global__ void __launch_bounds__(256)
 k_do_pull(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 nloc, u64 lo, const u64 *__restrict__ frontier,
-          const u64 *__restrict__ visited, u32 *__restrict__ newb32, i64 *__restrict__ level, i64 *__restrict__ parent, i64 lvl) {
+          const u64 *__restrict__ visited, u32 *__restrict__ newb32, i64 *__restrict__ level, i64 *__restrict__ parent, i64 lvl,
+          const BfsOpDev *__restrict__ ops, u32 nops) {
     const u32 lane8 = threadIdx.x & 7, sub = (threadIdx.x & 31) >> 3;
     const u32 gmask = 0xFFu << (8 * sub);
     u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
@@ -235,6 +336,15 @@ k_do_pull(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 nloc, u6
         if (r >= nloc) continue;
         const u64 v = lo + r;
         if (bit_of(visited, v)) continue;
+        if constexpr (DIRTY) {
+            const i64 par = do_first_parent(ops, nops, v, frontier, lane8, gmask);
+            if (par >= 0 && lane8 == 0) {
+                atomicOr(&newb32[v >> 5], 1u << (v & 31));
+                level[r] = lvl;
+                if (parent) parent[r] = par;
+            }
+            continue;
+        }
         const u64 s = ATp[r], e = ATp[r + 1];
         for (u64 qb = s; qb < e; qb += 8) {
             const u64 q = qb + lane8;
@@ -348,10 +458,41 @@ void bfs_build_degrees(const DevCSR &Aloc, u64 n, u64 lo, u64 hi, BfsComm *comm,
     *total_edges = local;
 }
 
+// the switch's table over dirty operands, per call: sum_t deg(m_t) (each base's cached table) + deg(dp_t)
+void bfs_delta_degrees(const std::vector<BfsOperand> &ops, u64 n, DevBuf<u32> &deg, u64 *total_edges) {
+    deg.alloc(n ? n : 1);
+    deg.zero();
+    u64 total = 0;
+    for (const BfsOperand &o : ops) {
+        if (n) LAUNCH(k_do_deg_add, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, o.deg, o.dp ? o.dp->p.ptr : (const u64 *)nullptr, n, deg.ptr);
+        total += o.edges + (o.dp ? o.dp->nnz : 0);
+    }
+    *total_edges = total;
+}
+
+static const u64 *csr_p(const DevCSR *A) { return A ? A->p.ptr : nullptr; }
+static const u32 *csr_j(const DevCSR *A) { return A ? A->j.ptr : nullptr; }
+
 void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, const u32 *deg_all, u64 total_edges, BfsComm *comm,
-            u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, BfsInfo *info) {
+            u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, BfsInfo *info, const std::vector<BfsOperand> *dirty) {
     if (src >= n) throw GrbError(-4, "BFS source out of range");
     const int P = comm_world(comm), rank = comm_rank(comm);
+    if (dirty && (P > 1 || dirty->empty())) throw GrbError(-3, "BFS over operands with deltas: one GPU and at least one operand");
+    // the dirty operands on the device; layers: transposed rows a parent search reads per vertex (for the byte counts)
+    const u32 nops = dirty ? (u32)dirty->size() : 0;
+    DevBuf<BfsOpDev> dops;
+    std::vector<BfsOpDev> h(nops);
+    u64 layers = 0;
+    if (dirty) {
+        for (u32 t = 0; t < nops; t++) {
+            const BfsOperand &o = (*dirty)[t];
+            h[t] = BfsOpDev{csr_p(o.m), csr_p(o.mT), csr_p(o.dp), csr_p(o.dpT), csr_p(o.dm), csr_p(o.dmT),
+                            csr_j(o.m), csr_j(o.mT), csr_j(o.dp), csr_j(o.dpT), csr_j(o.dm), csr_j(o.dmT)};
+            layers += 1 + (o.dpT != nullptr) + (o.dmT != nullptr);
+        }
+        dops.alloc(nops);
+        h2d(dops.ptr, h.data(), nops);
+    }
     const u64 block = P > 1 ? (n + P - 1) / P : n;          // vertices per rank (multiple of 64 when P > 1)
     const u64 nwl = P > 1 ? block / 64 : (n + 63) / 64;     // words per owned slice
     const u64 nw = nwl * P;                                 // words of a replicated bitmap (padded)
@@ -366,7 +507,7 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
     u32 dsrc = 0;
     d2h(&dsrc, deg_all + src, 1);
     sync_stream();
-    u64 nf = 1, mf = dsrc, explored = dsrc, edges = dsrc;
+    u64 nf = 1, mf = dsrc, explored = dsrc, edges = dsrc, reached = 1;
     const u64 udest = dest >= 0 ? (u64)dest : ~0ULL;
     bool bottom_up = false;
     i64 lvl = 0;
@@ -396,7 +537,21 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
             LAUNCH(k_do_compact, grid_for(w1 - w0, 256, (u64)ctx().num_sms * 8), 256, 0, frontier, w0, w1, list.ptr, cnt.ptr);
             const u64 nfl = read_scalar(cnt.ptr);
             disc.zero();
-            if (nfl) {
+            if (nfl && dirty) {
+                // one list per (frontier vertex, operand, layer m / dp)
+                const u64 nseg = nfl * 2 * nops;
+                DevBuf<u64> cum(nseg + 1), start(nseg);
+                LAUNCH(k_do_frontier_deg_delta, grid_for(nseg + 1, 256, (u64)ctx().num_sms * 16), 256, 0, list.ptr, nseg, dops.ptr, 2 * nops, cum.ptr, start.ptr);
+                exclusive_scan_u64(cum.ptr, cum.ptr, nseg + 1);
+                const u64 total = read_scalar(cum.ptr + nseg);
+                if (total) {
+                    // column ids of every listed entry, each list's offset and start, each (vertex, operand)'s dm row pointers
+                    TimedScope ts(TK_BFS_DELTA, 4 * total + 16 * nseg + 16 * nfl * nops);
+                    const u32 grid = (u32)std::min<u64>((total + DO_CHUNK - 1) / DO_CHUNK, (u64)cx.num_sms * 16);
+                    LAUNCH(k_do_expand<true>, grid, 256, 0, cum.ptr, start.ptr, nseg, total, (const u32 *)nullptr, visited.ptr, (u32 *)disc.ptr,
+                           list.ptr, dops.ptr, 2 * nops);
+                }
+            } else if (nfl) {
                 DevBuf<u64> cum(nfl + 1), start(nfl);
                 LAUNCH(k_do_frontier_deg, grid_for(nfl + 1, 256, (u64)ctx().num_sms * 16), 256, 0, list.ptr, nfl, lo, Aloc.p.ptr, cum.ptr, start.ptr);
                 exclusive_scan_u64(cum.ptr, cum.ptr, nfl + 1);
@@ -404,7 +559,8 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
                 if (total) {
                     TimedScope ts(TK_BFS_EXPAND, 4 * total + 20 * nfl);
                     const u32 grid = (u32)std::min<u64>((total + DO_CHUNK - 1) / DO_CHUNK, (u64)cx.num_sms * 16);
-                    LAUNCH(k_do_expand, grid, 256, 0, cum.ptr, start.ptr, nfl, total, Aloc.j.ptr, visited.ptr, (u32 *)disc.ptr);
+                    LAUNCH(k_do_expand<false>, grid, 256, 0, cum.ptr, start.ptr, nfl, total, Aloc.j.ptr, visited.ptr, (u32 *)disc.ptr,
+                           (const u32 *)nullptr, (const BfsOpDev *)nullptr, 0u);
                 }
             }
             if (P == 1) {
@@ -435,15 +591,28 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
             cnt.zero();
             LAUNCH(k_do_compact, grid_for(w1 - w0, 256, (u64)ctx().num_sms * 8), 256, 0, newb, w0, w1, list.ptr, cnt.ptr);
             const u64 nnew = read_scalar(cnt.ptr);
-            if (nnew) LAUNCH(k_do_assign, grid_for(nnew * 8, 256, (u64)ctx().num_sms * 16), 256, 0, list.ptr, nnew, lo, ATloc.p.ptr, ATloc.j.ptr, frontier, d_level, d_parent, lvl);
+            if (nnew && dirty) {
+                // the new vertices' list entries, levels and parents, and the transposed rows' pointers they read
+                TimedScope ts(TK_BFS_DELTA, 20 * nnew + 16 * nnew * layers);
+                LAUNCH(k_do_assign<true>, grid_for(nnew * 8, 256, (u64)ctx().num_sms * 16), 256, 0, list.ptr, nnew, lo, (const u64 *)nullptr,
+                       (const u32 *)nullptr, frontier, d_level, d_parent, lvl, dops.ptr, nops);
+            } else if (nnew) {
+                LAUNCH(k_do_assign<false>, grid_for(nnew * 8, 256, (u64)ctx().num_sms * 16), 256, 0, list.ptr, nnew, lo, ATloc.p.ptr, ATloc.j.ptr,
+                       frontier, d_level, d_parent, lvl, (const BfsOpDev *)nullptr, 0u);
+            }
             rec.td_levels++;
         } else {
             // ---- bottom-up ----
             CUDA_TRY(cudaMemsetAsync(newb, 0, nw * sizeof(u64), stream()));
-            if (nloc) {
+            if (nloc && dirty) {
+                // the visited bitmap, and the transposed rows' pointers of every unvisited vertex
+                TimedScope ts(TK_BFS_DELTA, 8 * nw + 16 * (n - reached) * layers);
+                LAUNCH(k_do_pull<true>, grid_for(nloc * 8, 256, (u64)cx.num_sms * 32), 256, 0, (const u64 *)nullptr, (const u32 *)nullptr, nloc, lo,
+                       frontier, visited.ptr, (u32 *)newb, d_level, d_parent, lvl, dops.ptr, nops);
+            } else if (nloc) {
                 TimedScope ts(TK_BFS_EXPAND, 0);
-                LAUNCH(k_do_pull, grid_for(nloc * 8, 256, (u64)cx.num_sms * 32), 256, 0, ATloc.p.ptr, ATloc.j.ptr, nloc, lo, frontier, visited.ptr,
-                       (u32 *)newb, d_level, d_parent, lvl);
+                LAUNCH(k_do_pull<false>, grid_for(nloc * 8, 256, (u64)cx.num_sms * 32), 256, 0, ATloc.p.ptr, ATloc.j.ptr, nloc, lo, frontier, visited.ptr,
+                       (u32 *)newb, d_level, d_parent, lvl, (const BfsOpDev *)nullptr, 0u);
             }
             if (P > 1) {
                 exchange_begin();
@@ -458,6 +627,7 @@ void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, cons
         d2h(hst, st.ptr, 3);
         sync_stream();
         nf = hst[0]; mf = hst[1];
+        reached += nf;
         explored += mf; edges += mf;
         if (nf == 0) { lvl--; break; }
         u64 *t = frontier; frontier = newb; newb = t;

@@ -1817,9 +1817,11 @@ int LAGraph_cdlp(GrB_Vector *CDLP_handle, LAGraph_Graph G, int itermax, char *ms
 }
 // One BFS over rows [lo, lo + nrows(A)) of the n-vertex graph; level / parent of those rows go to `location` memory.  With AT
 // (the same rows of A') the direction-optimising engine runs, its out-degree table cached on A; without it (one GPU, lo = 0)
-// the top-down bfs_run.  Both give level and minimum-id parent.  dest >= 0 stops once that vertex is reached.
+// the top-down bfs_run.  Both give level and minimum-id parent.  dest >= 0 stops once that vertex is reached.  dirty (one GPU,
+// B200_bfs_delta): the engine walks those operands instead of A, with deg / total_edges from bfs_delta_degrees.
 static void bfs_staged(GrB_Matrix A, const DevCSR *AT, u64 n, u64 lo, BfsComm *comm, u64 src, i64 max_level, i64 dest,
-                       i64 *level, i64 *parent, int location, B200_BfsInfo *info_out) {
+                       i64 *level, i64 *parent, int location, B200_BfsInfo *info_out,
+                       const std::vector<BfsOperand> *dirty = nullptr, const u32 *deg = nullptr, u64 total_edges = 0) {
     const u64 nloc = A->nrows, hi = lo + nloc;
     DevBuf<i64> dl, dp;
     i64 *d_level = level, *d_parent = parent;
@@ -1829,7 +1831,9 @@ static void bfs_staged(GrB_Matrix A, const DevCSR *AT, u64 n, u64 lo, BfsComm *c
     }
     BfsInfo rec;
     memset(&rec, 0, sizeof(rec));
-    if (AT) {
+    if (dirty) {
+        bfs_do(A->dev, A->dev, n, lo, hi, deg, total_edges, comm, src, max_level, dest, d_level, d_parent, &rec, dirty);
+    } else if (AT) {
         if (!A->bfs_deg_valid) { bfs_build_degrees(A->dev, n, lo, hi, comm, A->bfs_deg, &A->bfs_edges); A->bfs_deg_valid = true; }
         bfs_do(A->dev, *AT, n, lo, hi, A->bfs_deg.ptr, A->bfs_edges, comm, src, max_level, dest, d_level, d_parent, &rec);
     } else {
@@ -2791,6 +2795,68 @@ GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, G
     GrB_Info info = guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; });   // no device: fail before any host work
     if (info) return info;
     return reach_impl(reached, sources, nsrc, m, dp, dm, nops, max_hops, include_sources, levels_out);
+}
+
+// ---- single-source BFS over relationship operands with pending writes (algo.BFS, algo_procedures.rs:1021-1166) ----
+// The reference builds A = U_t (m[t] \ dm[t]) u dp[t] afresh on every call (build_adjacency_matrix, graph.rs:3870-3893) and runs
+// LAGr_BreadthFirstSearch_Extended on it.  Here the direction-optimising engine walks the operands in place: each base's transpose
+// mirror and out-degree table are cached on its handle (ensure_devT, bfs_deg) and reused until the base changes; only the deltas'
+// transposes are built per call.  One operand without deltas is exactly B200_Matrix_prepare(A, 1) + B200_bfs_ex.
+GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index src, int64_t max_level,
+                        int64_t dest, int64_t *level, int64_t *parent, int location, B200_BfsInfo *info_out) {
+    CHECK_PTR(m); CHECK_PTR(level);
+    if (nops < 1) { tl_error = "bfs_delta: nops < 1"; return GrB_INVALID_VALUE; }
+    for (int t = 0; t < nops; t++) {
+        CHECK_MAT(m[t]);
+        if (dp && dp[t]) CHECK_MAT(dp[t]);
+        if (dm && dm[t]) CHECK_MAT(dm[t]);
+    }
+    const u64 n = m[0]->nrows;
+    for (int t = 0; t < nops; t++)
+        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
+            if (X && (X->nrows != n || X->ncols != n)) {
+                tl_error = "bfs_delta: operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+            }
+    if (is_huge(m[0])) { tl_error = "bfs_delta: host-resident operand"; return GrB_NOT_IMPLEMENTED; }
+    if (src >= n || (dest >= 0 && (u64)dest >= n)) { tl_error = "bfs_delta: src or dest out of range"; return GrB_INVALID_INDEX; }
+    GrB_Info info = device_ready();             // no device: fail before any host work
+    if (info) return info;
+    return guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (int t = 0; t < nops; t++) { all.push_back(m[t]); all.push_back(dp ? dp[t] : nullptr); all.push_back(dm ? dm[t] : nullptr); }
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        // the deltas that hold entries, on the device
+        std::vector<const DevCSR *> ddp(nops, nullptr), ddm(nops, nullptr);
+        bool clean = nops == 1;
+        for (int t = 0; t < nops; t++) {
+            GrB_Matrix P = dp ? dp[t] : nullptr, M = dm ? dm[t] : nullptr;
+            if (P && matrix_nvals(P)) { ensure_dev(P); ddp[t] = &P->dev; clean = false; }
+            if (M && matrix_nvals(M)) { ensure_dev(M); ddm[t] = &M->dev; clean = false; }
+        }
+        if (clean) {
+            ensure_devT(m[0]);
+            bfs_staged(m[0], &m[0]->devT, n, 0, nullptr, src, max_level, dest, level, parent, location, info_out);
+            return GrB_SUCCESS;
+        }
+        std::vector<DevCSR> dT(2 * nops);           // dp' and dm', built per call (the deltas change with every write)
+        std::vector<BfsOperand> ops(nops);
+        for (int t = 0; t < nops; t++) {
+            GrB_Matrix A = m[t];
+            ensure_devT(A);
+            if (!A->bfs_deg_valid) { bfs_build_degrees(A->dev, n, 0, n, nullptr, A->bfs_deg, &A->bfs_edges); A->bfs_deg_valid = true; }
+            if (ddp[t]) transpose_csr(*ddp[t], dT[2 * t], false);
+            if (ddm[t]) transpose_csr(*ddm[t], dT[2 * t + 1], false);
+            ops[t] = BfsOperand{&A->dev, &A->devT, ddp[t], ddp[t] ? &dT[2 * t] : nullptr, ddm[t], ddm[t] ? &dT[2 * t + 1] : nullptr,
+                                A->bfs_deg.ptr, A->bfs_edges};
+        }
+        DevBuf<u32> deg;
+        u64 total = 0;
+        bfs_delta_degrees(ops, n, deg, &total);
+        bfs_staged(m[0], nullptr, n, 0, nullptr, src, max_level, dest, level, parent, location, info_out, &ops, deg.ptr, total);
+        return GrB_SUCCESS;
+    });
 }
 
 // ---- relationship ids of a batch of rows (expand_row / bind_edge / ExpandInto's Tensor::get, cond_traverse.rs:663-702, 844-935,

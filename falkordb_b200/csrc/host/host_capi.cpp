@@ -3,6 +3,7 @@
 // at this boundary (graph/src/graph/graphblas/versioned_matrix.rs:1278-1523).  Links against libb200grb.so only.
 #include "cond_traverse.hpp"
 #include "cond_var_len_traverse.hpp"
+#include "algo_bfs.hpp"
 #include <functional>
 #include <map>
 #include <set>
@@ -1105,6 +1106,36 @@ int fdbh_expand_edges(void **tensors, uint64_t ntypes, const uint64_t *srcs, con
             memcpy(*dst, v.data(), sizeof(**dst) * v.size());
         };
         out(out_p, r.p); out(out_node, r.node); out(out_edge, r.edge); out(out_type, r.type); out(out_rev, r.rev);
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
+// algo.BFS (algo_bfs.hpp).  adj: the adjacency VersionedMatrix; all_types / named: Tensor pointers (nnamed = 0: no type named);
+// deleted: deleted node ids; max_depth < 0 unbounded.  route 0: algo_bfs (B200_bfs_delta + B200_expand_edges); 1:
+// algo_bfs_by_extract (the fresh matrix, LAGr_BreadthFirstSearch_Extended, a Tensor::get per pair).  Outputs are malloc'ed; free
+// with fdbh_free.
+int fdbh_algo_bfs(void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, const uint64_t *deleted, uint64_t ndel,
+                  uint64_t src, int64_t max_depth, int want_edges, int route, uint64_t **out_nodes, uint64_t *nnodes, uint64_t **out_edges,
+                  uint64_t *nedges) {
+    try {
+        BfsQuery q;
+        q.adj = (const VersionedMatrix *)adj;
+        for (uint64_t k = 0; k < nall; k++) q.all_types.push_back((const Tensor *)all_types[k]);
+        for (uint64_t k = 0; k < nnamed; k++) q.named.push_back((const Tensor *)named[k]);
+        if (ndel) q.deleted.assign(deleted, deleted + ndel);
+        q.src = src; q.max_depth = max_depth; q.want_edges = want_edges != 0;
+        if (!q.adj && q.named.empty()) throw std::invalid_argument("algo_bfs: no adjacency matrix and no type");
+        BfsResult r;
+        if (route == 0) r = algo_bfs(q);
+        else if (route == 1) r = algo_bfs_by_extract(q);
+        else throw std::invalid_argument("algo_bfs: unknown route");
+        auto out = [](uint64_t **dst, const std::vector<uint64_t> &v) {
+            *dst = (uint64_t *)malloc(sizeof(uint64_t) * (v.size() + 1));
+            if (!*dst) throw std::bad_alloc();
+            memcpy(*dst, v.data(), sizeof(uint64_t) * v.size());
+        };
+        out(out_nodes, r.nodes); out(out_edges, r.edges);
+        *nnodes = r.nodes.size(); *nedges = r.edges.size();
         return 0;
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
 }

@@ -100,8 +100,17 @@ int comm_rank(const BfsComm *c);
 int comm_world(const BfsComm *c);
 void comm_allgather(BfsComm *c, const void *send, void *recv, size_t bytes_per_rank);
 void bfs_build_degrees(const DevCSR &Aloc, u64 n, u64 lo, u64 hi, BfsComm *comm, DevBuf<u32> &deg_all, u64 *total_edges);
+// one operand of the BFS over A = U_t (m_t \ dm_t) u dp_t: the base, its transpose mirror and its cached out-degree table (edges =
+// nnz(m)); dp and dm and their per-call transposes (null: empty)
+struct BfsOperand {
+    const DevCSR *m, *mT, *dp, *dpT, *dm, *dmT;
+    const u32 *deg; u64 edges;
+};
+void bfs_delta_degrees(const std::vector<BfsOperand> &ops, u64 n, DevBuf<u32> &deg, u64 *total_edges);   // the switch's table
+// dirty (one GPU): the operands A is the union of; Aloc / ATloc are then not read, deg_all / total_edges from bfs_delta_degrees
 void bfs_do(const DevCSR &Aloc, const DevCSR &ATloc, u64 n, u64 lo, u64 hi, const u32 *deg_all, u64 total_edges, BfsComm *comm,
-            u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, BfsInfo *info);
+            u64 src, i64 max_level, i64 dest, i64 *d_level, i64 *d_parent, BfsInfo *info,
+            const std::vector<BfsOperand> *dirty = nullptr);
 void bfs_run(const DevCSR &A, u64 src, i64 max_level, i64 *d_level, i64 *d_parent, u64 *edges_traversed);
 
 // algo.cu : FP64 mxv (PLUS_TIMES / PLUS_SECOND) and PageRank

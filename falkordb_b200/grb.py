@@ -8,7 +8,7 @@ import enum
 
 import numpy as np
 
-from ._lib import lib, obj, check, GrbError, P, U64, I64
+from ._lib import lib, obj, check, GrbError, P, U64, I64, BfsInfo
 
 GxB_SPARSITY_STATUS, GxB_SPARSITY_CONTROL, GxB_HYPER_HASH, GxB_WILL_WAIT = 7034, 7036, 7048, 7076
 GrB_STORAGE_ORIENTATION_HINT = 100
@@ -384,14 +384,30 @@ def rmat(scale, edge_factor=16, seed=1):
     return Matrix(0, 0, bool, _handle=h)
 
 
-def bfs(A, src, max_level=-1, want_parent=True):
-    n = A.nrows()
+def bfs(A, src, max_level=-1, want_parent=True, deltas=None, dest=-1, info=None):
+    """B200_bfs: (level, parent, edges traversed).  `A` may also be a list of operands (the relationship types algo.BFS names),
+    and `deltas` one (dp, dm) pair per operand (either may be None): the BFS then walks the union of every (m \\ dm) u dp,
+    exactly, through B200_bfs_delta, with the `dest` early exit and, given a B200_BfsInfo as `info`, what the run did."""
+    if deltas is None and isinstance(A, Matrix) and dest < 0 and info is None:
+        n = A.nrows()
+        level = np.empty(n, np.int64)
+        parent = np.empty(n, np.int64) if want_parent else None
+        edges = U64()
+        check(lib().B200_bfs(A.h, src, max_level, level.ctypes.data, None if parent is None else parent.ctypes.data, 0,
+                             C.byref(edges)))
+        return level, parent, edges.value
+    ms = [A] if isinstance(A, Matrix) else list(A)
+    k = len(ms)
+    deltas = [(None, None)] * k if deltas is None else list(deltas)
+    assert len(deltas) == k, "one (dp, dm) pair per operand"
+    n = ms[0].nrows()
     level = np.empty(n, np.int64)
     parent = np.empty(n, np.int64) if want_parent else None
-    edges = U64()
-    check(lib().B200_bfs(A.h, src, max_level, level.ctypes.data, None if parent is None else parent.ctypes.data, 0,
-                         C.byref(edges)))
-    return level, parent, edges.value
+    rec = BfsInfo() if info is None else info
+    arr = lambda xs: (C.c_void_p * k)(*[None if x is None else x.h for x in xs])
+    check(lib().B200_bfs_delta(arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), k, src, max_level, dest,
+                               level.ctypes.data, None if parent is None else parent.ctypes.data, 0, C.byref(rec)))
+    return level, parent, rec.edges
 
 
 def get_stat(name):

@@ -1,6 +1,6 @@
 """ctypes binding of libfdbhost.so, the C++ host mirror of the reference's Tensor and CondTraverse (csrc/host): a relationship
 Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending, and the routes that read its
-relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get)."""
+relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), and the algo.BFS procedure over them."""
 import ctypes as C
 import os
 
@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _L = None
 
 ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
+BFS_DEVICE, BFS_BY_EXTRACT = 0, 1
 
 
 def host():
@@ -27,6 +28,12 @@ def host():
     L.fdbh_tensor_remove_all.argtypes = [P, P, P, P, U64]
     L.fdbh_tensor_layers.argtypes = [P, P]
     L.fdbh_expand_edges.argtypes = [P, U64, P, P, U64, C.c_int, C.c_int, C.c_int] + [P] * 5 + [C.POINTER(U64)]
+    L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
+    L.fdbh_vm_new.argtypes = [U64, U64]
+    L.fdbh_vm_new.restype = P
+    L.fdbh_vm_free.argtypes = [P]
+    L.fdbh_vm_set.argtypes = [P, U64, U64]
+    L.fdbh_vm_remove.argtypes = [P, U64, U64]
     L.fdbh_free.argtypes = [P]
     L.fdbh_last_message.restype = C.c_char_p
     _L = L
@@ -89,5 +96,48 @@ def expand_edges(tensors, sources, dir, mode, targets=None, route=ROUTE_BY_GET):
     for x, dt, k in zip(ptrs, (np.uint64, np.uint32, np.uint64, np.uint16, np.uint8), (len(src) + 1, m, m, m, m)):
         nbytes = k * np.dtype(dt).itemsize
         out.append(np.frombuffer((C.c_char * nbytes).from_address(x.value), dt).copy() if k else np.zeros(0, dt))
+        L.fdbh_free(x)
+    return tuple(out)
+
+
+class VersionedMatrix:
+    """csrc/host/versioned_matrix.hpp's VersionedMatrix<bool> (the graph's adjacency matrix): set / remove stay pending"""
+
+    def __init__(self, n):
+        self.L = host()
+        self.h = self.L.fdbh_vm_new(n, n)
+        if not self.h:
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            self.L.fdbh_vm_free(self.h)
+            self.h = None
+
+    def set(self, i, j):
+        if self.L.fdbh_vm_set(self.h, int(i), int(j)):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def remove(self, i, j):
+        if self.L.fdbh_vm_remove(self.h, int(i), int(j)):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+
+def algo_bfs(adj, all_types, named, src, max_depth=-1, want_edges=True, deleted=(), route=BFS_DEVICE):
+    """fdbh_algo_bfs: algo.BFS from `src` over `named` Tensors, or over the adjacency VersionedMatrix `adj` when none is named;
+    relationship ids from `named`, or from `all_types` when none is named.  Returns (nodes, edges) as uint64 arrays."""
+    L = host()
+    (dl,) = _u64(sorted(deleted))
+    at = (C.c_void_p * max(1, len(all_types)))(*[t.h for t in all_types])
+    nt = (C.c_void_p * max(1, len(named)))(*[t.h for t in named])
+    ptrs = [C.c_void_p(), C.c_void_p()]
+    nn, ne = U64(0), U64(0)
+    rc = L.fdbh_algo_bfs(None if adj is None else adj.h, at, len(all_types), nt, len(named), dl.ctypes.data, len(dl), int(src),
+                         int(max_depth), 1 if want_edges else 0, route, C.byref(ptrs[0]), C.byref(nn), C.byref(ptrs[1]), C.byref(ne))
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    out = []
+    for x, k in zip(ptrs, (nn.value, ne.value)):
+        out.append(np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64).copy() if k else np.zeros(0, np.uint64))
         L.fdbh_free(x)
     return tuple(out)

@@ -417,8 +417,9 @@ uint64_t B200_get_stat(const char *name);
 void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
- * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", and the accumulating
- * products of union hops, "bits_pull_acc" and "bits_push_acc".  0 on success. */
+ * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", the accumulating
+ * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", and B200_bfs_delta's kernels over
+ * dirty operands, "bfs_delta".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
@@ -436,6 +437,17 @@ typedef struct {
  * direction-optimising engine when the transpose mirror exists (B200_Matrix_prepare(A, 1)), else the top-down kernel. */
 GrB_Info B200_bfs_ex(GrB_Matrix A, GrB_Index src, int64_t max_level, int64_t dest, int64_t *level, int64_t *parent, int location,
                      B200_BfsInfo *info);
+/* B200_bfs_ex over relationship operands with pending writes (algo.BFS, algo_procedures.rs:1021-1166): the BFS walks
+ * A = U_t (m[t] \ dm[t]) u dp[t], pattern only, with B200_reach_batch_delta's operand rules (m / dp may be UINT64; within a type
+ * dp wins over dm; dm entries outside m have no effect; an entry one type holds survives another type's dm; dp / dm may be NULL
+ * arrays or hold NULL entries).  level / parent / max_level / dest / location / info as for B200_bfs_ex (minimum-id parent).  The
+ * direction-optimising engine runs on the operands in place: no union is built and no base is changed; each base's transpose
+ * mirror is built on first use and cached on its handle, the deltas' transposes are built per call.  One operand without deltas
+ * is exactly B200_Matrix_prepare(m[0], 1) + B200_bfs_ex.  Errors: nops < 1 GrB_INVALID_VALUE; operands not square of one size
+ * GrB_DIMENSION_MISMATCH; host-resident operands GrB_NOT_IMPLEMENTED; src or dest >= n GrB_INVALID_INDEX; with no device
+ * GxB_GPU_ERROR before any host work. */
+GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index src,
+                        int64_t max_level, int64_t dest, int64_t *level, int64_t *parent, int location, B200_BfsInfo *info);
 /* 1-D row-block partitioned BFS over NCCL (BASELINE config 5; SURVEY 8e).  Rank 0 obtains the 128-byte id, the caller ships it
  * to the other ranks, every rank calls B200_comm_init; world == 1 needs no id.  NCCL is resolved with dlopen at run time. */
 typedef struct B200_Comm_opaque *B200_Comm;

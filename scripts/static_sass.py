@@ -19,9 +19,12 @@ WANT = [
     ("materialise, count (carry-save)", r"k_bits_count_csa<8>"),
     ("materialise, fill", r"k_bits_fill<8>"),
     ("bitmap hand-off", r"k_bits_rowmajor"),
-    ("BFS top-down expand", r"k_do_expand"),
-    ("BFS bottom-up", r"k_do_pull"),
-    ("BFS parent assign", r"k_do_assign"),
+    ("BFS top-down expand", r"k_do_expand<false>"),
+    ("BFS bottom-up", r"k_do_pull<false>"),
+    ("BFS parent assign", r"k_do_assign<false>"),
+    ("BFS top-down expand, operands with deltas", r"k_do_expand<true>"),
+    ("BFS bottom-up, operands with deltas", r"k_do_pull<true>"),
+    ("BFS parent assign, operands with deltas", r"k_do_assign<true>"),
     ("masked SpGEMM pairs", r"k_masked_pairs"),
     ("set union", r"k_union"),
     ("mask filter", r"k_rowfilter_fill"),
