@@ -2296,39 +2296,64 @@ static void union_product(GrB_Matrix F, std::vector<UnionOperand> &ops, bool pt_
     }
 }
 
-// U = the union of every operand's effective pattern (m \ dm) u dp, built once with the flush kernels
-static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<UnionOperand> &ops, u64 n) {
-    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, n, n);
+// *U = a new BOOL matrix holding the union over the operands of their induced effective layers ((m \ dm) u dp restricted to the
+// kept vertices and renumbered by rank, adj.cu), and with symmetric its union with its transpose.  keep null: vertices below n_out,
+// U is n_out x n_out; else the strictly ascending keep[0 .. nkeep), U is nkeep x nkeep.  Arguments checked by the caller.
+static GrB_Info effective_adjacency(GrB_Matrix *U, const std::vector<UnionOperand> &ops, u64 n_out, const GrB_Index *keep, u64 nkeep,
+                                    bool symmetric) {
+    const u64 rows = keep ? nkeep : n_out;
+    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, rows, rows);
     if (info) return info;
     info = guarded([&]() {
         GpuLock g;
         uvec<GrB_Matrix> all;
-        for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
+        for (const UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
         all.push_back(*U);
         MultiLock lk(all.begin(), all.end());
         ensure_init();
+        DevBuf<u64> dkeep;
+        DevBuf<u32> rank;
+        if (keep) {
+            dkeep.alloc(nkeep ? nkeep : 1);
+            h2d(dkeep.ptr, (const u64 *)keep, nkeep);
+            adj_rank_table(dkeep.ptr, nkeep, ops[0].m->ncols, rank);
+        }
         DevCSR S;
         bool have = false;
-        for (UnionOperand &o : ops) {
+        for (const UnionOperand &o : ops) {
             ensure_dev(o.m);
+            const DevCSR *ddm = nullptr;
+            if (o.dm) { ensure_dev(o.dm); if (o.dm->dev.nnz) ddm = &o.dm->dev; }
             DevCSR E;
-            const DevCSR *e = &o.m->dev;
-            if (o.dm) {
-                ensure_dev(o.dm);
-                if (o.dm->dev.nnz) { filter_by_mask(*e, o.dm->dev, true, true, E); e = &E; }
-            }
+            adj_layer(o.m->dev, ddm, n_out, keep ? dkeep.ptr : nullptr, rank.ptr, nkeep, E);
             if (o.dp) {
                 ensure_dev(o.dp);
-                if (o.dp->dev.nnz) { DevCSR T; ewise_union(*e, o.dp->dev, false, T); E = std::move(T); e = &E; }
+                if (o.dp->dev.nnz) {                 // dp's layer is merged in whole: within a type dp wins over dm
+                    DevCSR D, T;
+                    adj_layer(o.dp->dev, nullptr, n_out, keep ? dkeep.ptr : nullptr, rank.ptr, nkeep, D);
+                    ewise_union(E, D, false, T);
+                    E = std::move(T);
+                }
             }
-            if (!have) { csr_copy(*e, S, false); have = true; }
-            else { DevCSR T; ewise_union(S, *e, false, T); S = std::move(T); }
+            if (!have) { S = std::move(E); have = true; }
+            else { DevCSR T; ewise_union(S, E, false, T); S = std::move(T); }
+        }
+        if (symmetric) {
+            DevCSR ST, T;
+            transpose_csr(S, ST, false);
+            ewise_union(S, ST, false, T);
+            S = std::move(T);
         }
         set_dev(*U, std::move(S));
         return GrB_SUCCESS;
     });
     if (info) GrB_Matrix_free(U);
     return info;
+}
+
+// U = the union of every operand's effective pattern (m \ dm) u dp over all n vertices
+static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<UnionOperand> &ops, u64 n) {
+    return effective_adjacency(U, ops, n, nullptr, 0, false);
 }
 
 // per call, for the frontier form: deltas' pending tuples finished, dp's device form, and dm's repair plan (dm' and the repaired
@@ -2681,7 +2706,7 @@ GrB_Info B200_traverse_batch_union(const GrB_Index *sources, GrB_Index nsrc, con
 // the reached set masked out, so a dp edge cannot re-add a vertex already reached.  With bits_mode -1 the dirty reach stays in frontier form whenever it is legal (a tiny
 // hop-1 frontier takes the CSR push there): the row-wise path would first need every dirty operand rewritten, O(nnz(m)) per call.
 // Where the frontier path does not apply (bits_mode 0, more than 1024 sources) every dirty operand is materialised once per call
-// with the flush kernels (filter_by_mask, ewise_union) and the level runs the calls above over their union.
+// by the adjacency builder (effective_adjacency, identity form) and the level runs the calls above over their union.
 
 // One level in frontier form: F <- (F * A) AND NOT R (R only when masked).  F has at most 1024 rows.  Runs under the submission
 // lock.  One operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does.
@@ -2857,6 +2882,31 @@ GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Mat
         bfs_staged(m[0], nullptr, n, 0, nullptr, src, max_level, dest, level, parent, location, info_out, &ops, deg.ptr, total);
         return GrB_SUCCESS;
     });
+}
+
+// ---- the adjacency of algo.pageRank / algo.WCC / algo.labelPropagation over operands with pending writes ----
+// The reference builds it afresh on every call: build_adjacency_matrix or build_symmetric_adjacency_matrix, then dup + resize to
+// node_count + deleted_nodes_count (algo_procedures.rs:718-724, 816-822, 1207-1213), or, with a label filter, a host walk over every
+// edge of every named tensor remapped through a hash map (build_compact_adj_*_from_tensors, :535-670).  Here both are one device
+// call over the operands as they stand (effective_adjacency); only the kept rows of each layer are read.
+GrB_Info B200_adjacency_delta(GrB_Matrix *A, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index n_out,
+                              const GrB_Index *keep, GrB_Index nkeep, int symmetric) {
+    CHECK_PTR(A);
+    GrB_Info info = union_check("adjacency_delta", m, dp, dm, nops);
+    if (info) return info;
+    const u64 n = m[0]->ncols;
+    if (keep) {
+        for (GrB_Index k = 0; k < nkeep; k++)
+            if (keep[k] >= n || (k && keep[k] <= keep[k - 1])) {
+                tl_error = "adjacency_delta: keep must be strictly ascending vertex ids below ncols(m)"; return GrB_INVALID_INDEX;
+            }
+    } else if (n_out >= ((u64)1 << 32)) {
+        tl_error = "adjacency_delta: n_out must be below 2^32"; return GrB_INVALID_VALUE;
+    }
+    info = device_ready();                       // no device: fail before any host work
+    if (info) return info;
+    std::vector<UnionOperand> ops = union_operands(m, dp, dm, nops);
+    return effective_adjacency(A, ops, n_out, keep, keep ? nkeep : 0, symmetric != 0);
 }
 
 // ---- relationship ids of a batch of rows (expand_row / bind_edge / ExpandInto's Tensor::get, cond_traverse.rs:663-702, 844-935,

@@ -4,6 +4,7 @@
 #include "cond_traverse.hpp"
 #include "cond_var_len_traverse.hpp"
 #include "algo_bfs.hpp"
+#include "algo_procs.hpp"
 #include <functional>
 #include <map>
 #include <set>
@@ -1140,4 +1141,61 @@ int fdbh_algo_bfs(void *adj, void **all_types, uint64_t nall, void **named, uint
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
 }
 
+// algo.pageRank / algo.WCC / algo.labelPropagation (algo_procs.hpp).  adj: the adjacency VersionedMatrix; all_types / named:
+// Tensor pointers (nnamed = 0: no type named; a null entry: a type the graph does not have); labels: label VersionedMatrix pointers
+// (nlabels = 0: no filter; null: a missing label); node_count: live nodes; deleted: deleted node ids.  route 0: algo_proc
+// (B200_adjacency_delta); 1: algo_proc_by_extract (the reference's fresh matrix).  out_nodes and out_vals (double scores or int64
+// ids) are malloc'ed; free with fdbh_free.
+static int algo_entry(AlgoProc proc, void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, void **labels,
+                      uint64_t nlabels, uint64_t node_count, const uint64_t *deleted, uint64_t ndel, int max_iterations, int route,
+                      uint64_t **out_nodes, void **out_vals, uint64_t *nout) {
+    try {
+        AlgoQuery q;
+        q.proc = proc;
+        q.adj = (const VersionedMatrix *)adj;
+        for (uint64_t k = 0; k < nall; k++) q.all_types.push_back((const Tensor *)all_types[k]);
+        for (uint64_t k = 0; k < nnamed; k++) q.named.push_back((const Tensor *)named[k]);
+        for (uint64_t k = 0; k < nlabels; k++) q.labels.push_back((const VersionedMatrix *)labels[k]);
+        if (ndel) q.deleted.assign(deleted, deleted + ndel);
+        q.node_count = node_count;
+        q.max_iterations = max_iterations;
+        AlgoResult r;
+        if (route == 0) r = algo_proc(q);
+        else if (route == 1) r = algo_proc_by_extract(q);
+        else throw std::invalid_argument("algo: unknown route");
+        auto out = [](void **dst, const void *src, size_t bytes) {
+            *dst = malloc(bytes + 8);
+            if (!*dst) throw std::bad_alloc();
+            if (bytes) memcpy(*dst, src, bytes);
+        };
+        out((void **)out_nodes, r.nodes.data(), 8 * r.nodes.size());
+        if (proc == AlgoProc::PageRank) out(out_vals, r.score.data(), 8 * r.score.size());
+        else out(out_vals, r.id.data(), 8 * r.id.size());
+        *nout = r.nodes.size();
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
+int fdbh_algo_pagerank(void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, void **labels, uint64_t nlabels,
+                       uint64_t node_count, const uint64_t *deleted, uint64_t ndel, int route, uint64_t **out_nodes, double **out_score,
+                       uint64_t *nout) {
+    return algo_entry(AlgoProc::PageRank, adj, all_types, nall, named, nnamed, labels, nlabels, node_count, deleted, ndel, 0, route,
+                      out_nodes, (void **)out_score, nout);
+}
+
+int fdbh_algo_wcc(void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, void **labels, uint64_t nlabels,
+                  uint64_t node_count, const uint64_t *deleted, uint64_t ndel, int route, uint64_t **out_nodes, int64_t **out_id,
+                  uint64_t *nout) {
+    return algo_entry(AlgoProc::WCC, adj, all_types, nall, named, nnamed, labels, nlabels, node_count, deleted, ndel, 0, route,
+                      out_nodes, (void **)out_id, nout);
+}
+
+int fdbh_algo_cdlp(void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, void **labels, uint64_t nlabels,
+                   uint64_t node_count, const uint64_t *deleted, uint64_t ndel, int max_iterations, int route, uint64_t **out_nodes,
+                   int64_t **out_id, uint64_t *nout) {
+    return algo_entry(AlgoProc::CDLP, adj, all_types, nall, named, nnamed, labels, nlabels, node_count, deleted, ndel, max_iterations,
+                      route, out_nodes, (void **)out_id, nout);
+}
+
 } // extern "C"
+

@@ -139,6 +139,12 @@ struct EdgeTypeDev {  // one relationship type: forward m / dp (u64 values) / dm
 u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<EdgeTypeDev> &types, int dir, int mode, u64 *out_p,
                 u32 *out_node, u64 *out_edge, uint16_t *out_type, uint8_t *out_rev, u64 capacity);
 
+// adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
+// replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
+// and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.
+void adj_rank_table(const u64 *d_keep, u64 nkeep, u64 n, DevBuf<u32> &tab);   // tab[v] = v's position in keep, or ~0u
+void adj_layer(const DevCSR &L, const DevCSR *dm, u64 n_out, const u64 *d_keep, const u32 *rank_tab, u64 nkeep, DevCSR &out);
+
 // hypersparse host form <-> dense device rowptr (ewise.cu)
 void rowptr_from_hyper(const u64 *d_hrow, const u64 *d_hptr, u64 nvec, u64 nrows, u64 *d_p);
 u64 hyper_from_rowptr(const u64 *d_p, u64 nrows, u64 nnz, DevBuf<u64> &d_hrow, DevBuf<u64> &d_hptr);

@@ -508,6 +508,24 @@ def reach_batch(sources, A, max_hops=None, include_sources=False, deltas=None):
     return Matrix(0, 0, bool, _handle=h), lv.value
 
 
+def adjacency(ms, deltas=None, n=None, keep=None, symmetric=False):
+    """B200_adjacency_delta: the adjacency algo.pageRank / algo.WCC / algo.labelPropagation run on, as a new BOOL Matrix.  `ms`: one
+    operand or a list, `deltas` one (dp, dm) pair per operand (either may be None); the result is the union of every (m \\ dm) u dp
+    restricted to the vertices below `n` (default ncols) or, given `keep` (strictly ascending ids), to those, renumbered 0 ..
+    len(keep) - 1.  `symmetric`: that union with its transpose."""
+    ms = [ms] if isinstance(ms, Matrix) else list(ms)
+    k = len(ms)
+    deltas = [(None, None)] * k if deltas is None else list(deltas)
+    assert len(deltas) == k, "one (dp, dm) pair per operand"
+    arr = lambda xs: (C.c_void_p * max(1, k))(*[None if x is None else x.h for x in xs])
+    kp = None if keep is None else _u64arr(keep)
+    h = P()
+    check(lib().B200_adjacency_delta(C.byref(h), arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), k,
+                                     (ms[0].ncols() if k else 0) if n is None else int(n),
+                                     None if kp is None else kp.ctypes.data, 0 if kp is None else len(kp), 1 if symmetric else 0))
+    return Matrix(0, 0, bool, _handle=h)
+
+
 def multi_source_reach(sources, A, max_hops=None, include_sources=False):
     """Reachability from up to 1024 sources at once by level-synchronous mxm -- the multiplicity-insensitive core of a
     variable-length traversal `-[*1..k]->` with `emit_path = false` (cond_var_len_traverse.rs:196; SURVEY 8f-1) and of the

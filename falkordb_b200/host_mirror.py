@@ -1,6 +1,7 @@
 """ctypes binding of libfdbhost.so, the C++ host mirror of the reference's Tensor and CondTraverse (csrc/host): a relationship
 Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending, and the routes that read its
-relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), and the algo.BFS procedure over them."""
+relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), and the algo.BFS, algo.pageRank, algo.WCC
+and algo.labelPropagation procedures over them."""
 import ctypes as C
 import os
 
@@ -13,6 +14,7 @@ _L = None
 
 ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
 BFS_DEVICE, BFS_BY_EXTRACT = 0, 1
+ALGO_DEVICE, ALGO_BY_EXTRACT = 0, 1
 
 
 def host():
@@ -29,6 +31,10 @@ def host():
     L.fdbh_tensor_layers.argtypes = [P, P]
     L.fdbh_expand_edges.argtypes = [P, U64, P, P, U64, C.c_int, C.c_int, C.c_int] + [P] * 5 + [C.POINTER(U64)]
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
+    algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
+    L.fdbh_algo_pagerank.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
+    L.fdbh_algo_wcc.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
+    L.fdbh_algo_cdlp.argtypes = algo + [C.c_int, C.c_int, P, P, C.POINTER(U64)]
     L.fdbh_vm_new.argtypes = [U64, U64]
     L.fdbh_vm_new.restype = P
     L.fdbh_vm_free.argtypes = [P]
@@ -141,3 +147,40 @@ def algo_bfs(adj, all_types, named, src, max_depth=-1, want_edges=True, deleted=
         out.append(np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64).copy() if k else np.zeros(0, np.uint64))
         L.fdbh_free(x)
     return tuple(out)
+
+
+def _algo(fn, dt, adj, all_types, named, labels, node_count, deleted, route, *extra):
+    L = host()
+    (dl,) = _u64(sorted(deleted))
+    arr = lambda xs: (C.c_void_p * max(1, len(xs)))(*[None if x is None else x.h for x in xs])
+    named, labels = list(named or ()), list(labels or ())
+    ptrs = [C.c_void_p(), C.c_void_p()]
+    nv = U64(0)
+    rc = getattr(L, fn)(None if adj is None else adj.h, arr(all_types), len(all_types), arr(named), len(named), arr(labels), len(labels),
+                        int(node_count), dl.ctypes.data, len(dl), *extra, route, C.byref(ptrs[0]), C.byref(ptrs[1]), C.byref(nv))
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    out = []
+    for x, t in zip(ptrs, (np.uint64, dt)):
+        k = nv.value
+        out.append(np.frombuffer((C.c_char * (8 * k)).from_address(x.value), t).copy() if k else np.zeros(0, t))
+        L.fdbh_free(x)
+    return tuple(out)
+
+
+def algo_pagerank(adj, all_types, named=(), labels=(), node_count=0, deleted=(), route=ALGO_DEVICE):
+    """fdbh_algo_pagerank: algo.pageRank over the adjacency VersionedMatrix `adj`, or over the `named` Tensors (None: a type the
+    graph does not have); `labels`: () or one label VersionedMatrix (None: a missing label); `node_count` live nodes, `deleted` the
+    deleted ids.  Returns (nodes uint64, scores float64)."""
+    return _algo("fdbh_algo_pagerank", np.float64, adj, all_types, named, labels, node_count, deleted, route)
+
+
+def algo_wcc(adj, all_types, named=(), labels=(), node_count=0, deleted=(), route=ALGO_DEVICE):
+    """fdbh_algo_wcc: algo.WCC, arguments as algo_pagerank with any number of labels (nodeLabels).  Returns (nodes uint64,
+    component ids int64): the component ids are compact indices, as the procedure returns them."""
+    return _algo("fdbh_algo_wcc", np.int64, adj, all_types, named, labels, node_count, deleted, route)
+
+
+def algo_cdlp(adj, all_types, named=(), labels=(), node_count=0, deleted=(), max_iterations=10, route=ALGO_DEVICE):
+    """fdbh_algo_cdlp: algo.labelPropagation, arguments as algo_wcc.  Returns (nodes uint64, community ids int64)."""
+    return _algo("fdbh_algo_cdlp", np.int64, adj, all_types, named, labels, node_count, deleted, route, int(max_iterations))

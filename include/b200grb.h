@@ -418,8 +418,8 @@ void B200_reset_stats(void);
 /* with option "timing"=1 the library brackets its main kernels with CUDA events on its stream; this returns the
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
  * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", the accumulating
- * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", and B200_bfs_delta's kernels over
- * dirty operands, "bfs_delta".  0 on success. */
+ * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", B200_bfs_delta's kernels over
+ * dirty operands, "bfs_delta", and B200_adjacency_delta's induced-layer kernels, "adj_build".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
@@ -448,6 +448,22 @@ GrB_Info B200_bfs_ex(GrB_Matrix A, GrB_Index src, int64_t max_level, int64_t des
  * GxB_GPU_ERROR before any host work. */
 GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index src,
                         int64_t max_level, int64_t dest, int64_t *level, int64_t *parent, int location, B200_BfsInfo *info);
+/* The adjacency the algorithm procedures run on (algo.pageRank / algo.WCC / algo.labelPropagation, algo_procedures.rs:718-732,
+ * 816-832, 1207-1223), built on the device in one call over relationship operands with pending writes.  *A is a new BOOL, iso
+ * matrix: the union over t of the induced effective layer (m[t] \ dm[t]) u dp[t], restricted to the kept vertices (rows and
+ * columns) with both indices replaced by their rank among them.
+ *   keep == NULL: the vertices below n_out, A is n_out x n_out (the reference's dup + resize to node_count + deleted_nodes_count:
+ *                 entries at or beyond n_out are dropped, rows beyond ncols(m) are empty).  n_out must be below 2^32.
+ *   keep != NULL: keep[0 .. nkeep) strictly ascending ids below ncols(m[0]), A is nkeep x nkeep and vertex keep[k] is index k
+ *                 (the compact matrix of a label filter).  nkeep == 0 gives a 0 x 0 matrix.
+ *   symmetric:    A u A' (build_symmetric_adjacency_matrix, the input of WCC and CDLP).
+ * Only the kept rows of each m, dp and dm are read.  Operand rules as B200_reach_batch_delta (m / dp may be UINT64, values are
+ * ignored; within a type dp wins over dm; dm entries outside m have no effect; an entry one type holds survives another type's dm;
+ * dp / dm may be NULL arrays or hold NULL entries).  No operand is changed.  Errors: nops < 1 or n_out >= 2^32 GrB_INVALID_VALUE;
+ * operands not square of one size GrB_DIMENSION_MISMATCH; keep not strictly ascending or holding an id >= ncols(m[0])
+ * GrB_INVALID_INDEX; host-resident operands GrB_NOT_IMPLEMENTED; with no device GxB_GPU_ERROR before any host work. */
+GrB_Info B200_adjacency_delta(GrB_Matrix *A, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops,
+                              GrB_Index n_out, const GrB_Index *keep, GrB_Index nkeep, int symmetric);
 /* 1-D row-block partitioned BFS over NCCL (BASELINE config 5; SURVEY 8e).  Rank 0 obtains the 128-byte id, the caller ships it
  * to the other ranks, every rank calls B200_comm_init; world == 1 needs no id.  NCCL is resolved with dlopen at run time. */
 typedef struct B200_Comm_opaque *B200_Comm;

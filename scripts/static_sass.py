@@ -28,6 +28,10 @@ WANT = [
     ("masked SpGEMM pairs", r"k_masked_pairs"),
     ("set union", r"k_union"),
     ("mask filter", r"k_rowfilter_fill"),
+    ("adjacency layer, count (identity form)", r"k_adj_layer<b200::RankIdentity, false>"),
+    ("adjacency layer, fill (identity form)", r"k_adj_layer<b200::RankIdentity, true>"),
+    ("adjacency layer, count (kept list)", r"k_adj_layer<b200::RankTable, false>"),
+    ("adjacency layer, fill (kept list)", r"k_adj_layer<b200::RankTable, true>"),
     ("FP64 mxv (PLUS_SECOND)", r"k_mxv_fp64<false>"),
     ("WCC hook", r"k_cc_hook"),
     ("CDLP pick", r"k_cdlp_pick"),
