@@ -2981,6 +2981,73 @@ GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, G
     });
 }
 
+// ---- the read phase of a Tensor's relationship inserts and deletes (set_all_from_slices / remove_all, tensor.rs:333-629) for a
+// whole batch in one call: writes.cu.  Only reads the layers; their pending tuples are finished like any device read's.
+static_assert(B200_PLAN_COMMITTED == WP_COMMITTED && B200_PLAN_CANCEL == WP_CANCEL && B200_PLAN_MT_BASE == WP_MT_BASE &&
+              B200_PLAN_EMPTIED == WP_EMPTIED && B200_PLAN_DEMOTED == WP_DEMOTED && B200_PLAN_M_HAS == WP_M_HAS &&
+              B200_PLAN_M_EQ == WP_M_EQ, "plan flags");
+
+static GrB_Info write_plan(const char *what, bool insert, const B200_TensorLayers *t, const GrB_Index *a, const GrB_Index *b,
+                           const GrB_Index *c, GrB_Index n, uint64_t *rec_src, uint64_t *rec_dst, uint64_t *rec_val,
+                           uint8_t *rec_flags, uint64_t *nrec, uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
+    CHECK_PTR(t); CHECK_PTR(nrec); CHECK_PTR(nme);
+    if (n) {
+        CHECK_PTR(a); CHECK_PTR(b); CHECK_PTR(c);
+        CHECK_PTR(rec_src); CHECK_PTR(rec_dst); CHECK_PTR(rec_val); CHECK_PTR(rec_flags);
+        CHECK_PTR(me_key); CHECK_PTR(me_id); CHECK_PTR(me_base);
+    }
+    CHECK_MAT(t->m);
+    CHECK_MAT(t->mt);
+    for (GrB_Matrix X : {t->dp, t->dm, t->mt_dp, t->mt_dm, t->me, t->me_dp, t->me_dm}) if (X) CHECK_MAT(X);
+    if (t->m->type != T_UINT64 || (t->dp && t->dp->type != T_UINT64)) {
+        tl_error = std::string(what) + ": the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
+    }
+    const u64 nv = t->m->nrows;
+    for (GrB_Matrix X : {t->m, t->dp, t->dm, t->mt, t->mt_dp, t->mt_dm})
+        if (X && (X->nrows != nv || X->ncols != nv)) {
+            tl_error = std::string(what) + ": forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+        }
+    if (is_huge(t->m)) { tl_error = std::string(what) + ": host-resident forward layers"; return GrB_NOT_IMPLEMENTED; }
+    // insert: (a, b, c) = (srcs, dsts, ids); remove: (ids, srcs, dsts)
+    const GrB_Index *src = insert ? a : b, *dst = insert ? b : c, *ids = insert ? c : a;
+    for (u64 k = 0; k < n; k++)
+        if (src[k] >= nv || dst[k] >= nv || ids[k] >= ((u64)1 << 60)) {
+            tl_error = std::string(what) + ": a vertex id >= n or an edge id >= 2^60"; return GrB_INVALID_INDEX;
+        }
+    *nrec = 0; *nme = 0;
+    if (n == 0) return GrB_SUCCESS;
+    GrB_Info info = device_ready();             // no device: fail before any host work
+    if (info) return info;
+    return guarded([&]() {
+        GpuLock g;
+        MultiLock lk{t->m, t->dp, t->dm, t->mt, t->mt_dp, t->mt_dm, t->me, t->me_dp, t->me_dm};
+        ensure_init();
+        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
+        const EdgeTypeDev td{dev(t->m), dev(t->dp), dev(t->dm), dev(t->mt), nullptr, nullptr, id_store(t->me),
+                             insert ? nullptr : id_store(t->me_dp), insert ? nullptr : id_store(t->me_dm)};
+        DevBuf<u64> ds(n), dd(n), di(n);
+        h2d(ds.ptr, (const u64 *)src, n);
+        h2d(dd.ptr, (const u64 *)dst, n);
+        h2d(di.ptr, (const u64 *)ids, n);
+        WritePlan P{rec_src, rec_dst, rec_val, rec_flags, 0, me_key, me_id, me_base, 0};
+        if (insert) tensor_insert_plan(td, ds.ptr, dd.ptr, di.ptr, n, nv, P);
+        else tensor_remove_plan(td, di.ptr, ds.ptr, dd.ptr, n, nv, P);
+        *nrec = P.nrec; *nme = P.nme;
+        return GrB_SUCCESS;
+    });
+}
+
+GrB_Info B200_Tensor_insert_plan(const B200_TensorLayers *t, const GrB_Index *srcs, const GrB_Index *dsts, const GrB_Index *ids,
+                                 GrB_Index n, uint64_t *in_src, uint64_t *in_dst, uint64_t *in_val, uint8_t *in_flags, uint64_t *nin,
+                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
+    return write_plan("insert_plan", true, t, srcs, dsts, ids, n, in_src, in_dst, in_val, in_flags, nin, me_key, me_id, me_base, nme);
+}
+GrB_Info B200_Tensor_remove_plan(const B200_TensorLayers *t, const GrB_Index *ids, const GrB_Index *srcs, const GrB_Index *dsts,
+                                 GrB_Index n, uint64_t *pr_src, uint64_t *pr_dst, uint64_t *pr_val, uint8_t *pr_flags, uint64_t *npr,
+                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
+    return write_plan("remove_plan", false, t, ids, srcs, dsts, n, pr_src, pr_dst, pr_val, pr_flags, npr, me_key, me_id, me_base, nme);
+}
+
 // returns every cached device block to the driver (the caching allocator otherwise keeps freed blocks for reuse)
 GrB_Info B200_pool_trim(void) {
     return guarded([&]() {

@@ -197,6 +197,16 @@ static void t_motogp_two_hop() {
 }
 
 // ---- tensor.rs:1340-1669 : the per-relationship-type edge store ----
+// The writes of these tests go through one of the two routes: the reference's (Tensor::set_all_from_slices / remove_all) or the
+// device plans' (set_all_from_slices_dev / remove_all_dev); the *_dev test names run the second.
+static bool g_write_dev = false;
+static void tensor_add(Tensor &t, const std::vector<uint64_t> &s, const std::vector<uint64_t> &d, const std::vector<uint64_t> &i) {
+    if (g_write_dev) t.set_all_from_slices_dev(s, d, i);
+    else t.set_all_from_slices(s, d, i);
+}
+static std::vector<std::pair<uint64_t, uint64_t>> tensor_remove(Tensor &t, const std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> &r) {
+    return g_write_dev ? t.remove_all_dev(r) : t.remove_all(r);
+}
 static uint64_t count_sentinels(const Tensor &t, uint64_t pairs) {
     uint64_t s = 0, v;
     for (uint64_t i = 0; i < pairs; i++) if (t.eff_get(i, i + 1, &v) && v == MULTI_EDGE) s++;
@@ -208,7 +218,7 @@ static void t_multi_pairs_after_within_batch_duplicates() {      // tensor.rs:13
         Tensor t(n, n);
         std::vector<uint64_t> srcs, dsts, ids;
         for (uint64_t i = 0; i < pairs; i++) for (uint64_t d = 0; d < dup; d++) { srcs.push_back(i); dsts.push_back(i + 1); ids.push_back(next_id++); }
-        t.set_all_from_slices(srcs, dsts, ids);
+        tensor_add(t, srcs, dsts, ids);
         t.wait_fwd();
         uint64_t sentinels = count_sentinels(t, pairs), derived = t.multi_pairs(), edges = 0;
         for (uint64_t i = 0; i < pairs; i++) edges += t.get(i, i + 1).size();
@@ -226,7 +236,7 @@ static void t_multi_pairs_matches_the_sentinel_count() {         // tensor.rs:13
         for (uint64_t round = 0; round < dup; round++) {
             std::vector<uint64_t> ids;
             for (uint64_t i = 0; i < pairs; i++) ids.push_back(round * pairs + i);
-            t.set_all_from_slices(srcs, dsts, ids);
+            tensor_add(t, srcs, dsts, ids);
         }
         t.wait_fwd();
         uint64_t sentinels = count_sentinels(t, pairs), derived = t.multi_pairs(), edges = 0;
@@ -240,14 +250,14 @@ static void t_bulk_remove_and_extract_edge_id_zero() {           // tensor.rs:14
     Tensor t0(N + 1, N + 1);
     std::vector<uint64_t> srcs, dsts, ids;
     for (uint64_t i = 0; i < N; i++) { srcs.push_back(i); dsts.push_back(i + 1); ids.push_back(i); }
-    t0.set_all_from_slices(srcs, dsts, ids);
+    tensor_add(t0, srcs, dsts, ids);
     Tensor t = t0.dup();
     t.flush();
     t.fwd_m().wait();
     REQUIRE(t.fwd_m().contains(0, 1), "edge id 0 not folded into base");
     uint64_t v = 77;
     REQUIRE(t.fwd_m().get(0, 1, &v) && v == 0, "edge id 0 changed value in the fold");
-    t.remove_all({std::make_tuple(0ULL, 0ULL, 1ULL), std::make_tuple(5ULL, 5ULL, 6ULL)});
+    tensor_remove(t, {std::make_tuple(0ULL, 0ULL, 1ULL), std::make_tuple(5ULL, 5ULL, 6ULL)});
     REQUIRE(t.get(0, 1).empty(), "edge id 0 still readable");
     REQUIRE(t.get(5, 6).empty(), "edge id 5 still readable");
     Matrix<bool> ex = t.extract();
@@ -261,7 +271,7 @@ static void t_deleting_everything_folds_the_tombstones_away() {  // tensor.rs:15
     Tensor t0(N + 1, N + 1);
     std::vector<uint64_t> srcs, dsts, ids;
     for (uint64_t i = 0; i < N; i++) { srcs.push_back(i); dsts.push_back(i + 1); ids.push_back(i); }
-    t0.set_all_from_slices(srcs, dsts, ids);
+    tensor_add(t0, srcs, dsts, ids);
     Tensor t1 = t0.dup();
     t1.flush();
     t1.wait_fwd();
@@ -269,7 +279,7 @@ static void t_deleting_everything_folds_the_tombstones_away() {  // tensor.rs:15
     Tensor t = t1.dup();
     std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rels;
     for (uint64_t i = 0; i < N; i++) rels.push_back(std::make_tuple(i, i, i + 1));
-    t.remove_all(rels);
+    tensor_remove(t, rels);
     t.fold_oversized();
     t.wait_fwd();
     REQUIRE(t.fwd_m().nvals() == 0, "base kept its deleted entries");
@@ -280,7 +290,7 @@ static Tensor committed_pairs(uint64_t n) {                      // tensor.rs:15
     Tensor t(n + 1, n + 1);
     std::vector<uint64_t> srcs, dsts, ids;
     for (uint64_t i = 0; i < n; i++) for (int k = 0; k < 2; k++) { srcs.push_back(i); dsts.push_back(i + 1); ids.push_back(2 * i + k); }
-    t.set_all_from_slices(srcs, dsts, ids);
+    tensor_add(t, srcs, dsts, ids);
     t.fold_oversized();
     t.wait();
     REQUIRE(t.fwd_m().nvals() == n, "sentinels not folded into the base");
@@ -291,7 +301,7 @@ static void t_batch_demote_leaves_every_survivor_inline() {      // tensor.rs:15
     Tensor t = committed_pairs(N);
     std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rels;
     for (uint64_t i = 0; i < N; i++) rels.push_back(std::make_tuple(2 * i + 1, i, i + 1));
-    auto emptied = t.remove_all(rels);
+    auto emptied = tensor_remove(t, rels);
     REQUIRE(emptied.empty(), "demoted pairs reported as emptied");
     REQUIRE(t.edge_count() == N, "edge count after demoting every pair: " << t.edge_count());
     REQUIRE(t.multi_pairs() == 0, "a demoted pair still counts as multi");
@@ -309,7 +319,7 @@ static void t_batch_can_demote_and_then_empty_the_same_pair() {  // tensor.rs:15
         rels.push_back(std::make_tuple(2 * i, i, i + 1));
         rels.push_back(std::make_tuple(2 * i, i, i + 1));
     }
-    auto emptied = t.remove_all(rels);
+    auto emptied = tensor_remove(t, rels);
     std::sort(emptied.begin(), emptied.end());
     REQUIRE(emptied.size() == N, "every pair should be reported emptied exactly once: " << emptied.size());
     for (uint64_t i = 0; i < N; i++) REQUIRE(emptied[i] == std::make_pair(i, i + 1), "emptied list wrong at " << i);
@@ -318,6 +328,28 @@ static void t_batch_can_demote_and_then_empty_the_same_pair() {  // tensor.rs:15
     t.matrix_t().wait();
     REQUIRE(t.matrix_t().extract().nvals() == 0, "backward adjacency kept the pairs");
     for (uint64_t i = 0; i < N; i++) REQUIRE(t.get(i, i + 1).empty(), "pair " << i << " still readable");
+}
+static void t_demoting_to_the_committed_value_cancels_to_clean() {  // tensor.rs:1634-1668
+    const uint64_t N = 512;
+    Tensor t0(N + 1, N + 1);
+    std::vector<uint64_t> srcs, dsts, ids;
+    for (uint64_t i = 0; i < N; i++) { srcs.push_back(i); dsts.push_back(i + 1); ids.push_back(i + 1); }
+    tensor_add(t0, srcs, dsts, ids);
+    t0.fold_oversized();
+    t0.wait();
+    uint64_t v = 0;
+    REQUIRE(t0.fwd_m().get(0, 1, &v) && v == 1, "single edge not committed");
+    Tensor t = t0.dup();                          // promote in this version (m = 1, dp = M, me = {1, 9}), then remove the new edge
+    tensor_add(t, {0}, {1}, {9});
+    auto emptied = tensor_remove(t, {std::make_tuple(9ULL, 0ULL, 1ULL)});
+    REQUIRE(emptied.empty(), "surviving pair reported as emptied");
+    t.wait();
+    REQUIRE(t.fwd_dp().nvals() == 0, "dp still shadows m with m's own value");
+    REQUIRE(t.fwd_dm().nvals() == 0, "demotion left a tombstone");
+    REQUIRE(t.edge_versioned().nvals() == 0, "`me` not emptied by the demotion");
+    REQUIRE(t.edge_count() == N, "edge count after promote + demote: " << t.edge_count());
+    auto g = t.get(0, 1);
+    REQUIRE(g.size() == 1 && g[0] == 1, "committed edge lost");
 }
 // CondTraverse over a relationship tensor (TraversalMatrix::U64, cond_traverse.rs:83): the u64 edge ids -- including
 // id 0 and the MULTI_EDGE sentinel -- are never read by ANY_PAIR; only the pattern matters.
@@ -941,6 +973,7 @@ static TestEntry TESTS[] = {
     {"deleting_everything_folds_the_tombstones_away", t_deleting_everything_folds_the_tombstones_away},
     {"batch_demote_leaves_every_survivor_inline", t_batch_demote_leaves_every_survivor_inline},
     {"batch_can_demote_and_then_empty_the_same_pair", t_batch_can_demote_and_then_empty_the_same_pair},
+    {"demoting_to_the_committed_value_cancels_to_clean", t_demoting_to_the_committed_value_cancels_to_clean},
     {"traverse_over_tensor_operand", t_traverse_over_tensor_operand},
     {"coalesced_traverse_over_tensor_operand", t_coalesced_traverse_over_tensor_operand},
     {"var_len_reach_matches_trails", t_var_len_reach_matches_trails},
@@ -970,6 +1003,20 @@ int fdbh_run_test(const char *name) {
         }
     g_msg = "unknown test";
     return 2;
+}
+// the tensor.rs tests whose writes can take either route; write_dev 1: through the device plans
+static const char *WRITE_TESTS[] = {"multi_pairs_after_within_batch_duplicates", "multi_pairs_matches_the_sentinel_count",
+                                    "bulk_remove_and_extract_edge_id_zero", "deleting_everything_folds_the_tombstones_away",
+                                    "batch_demote_leaves_every_survivor_inline", "batch_can_demote_and_then_empty_the_same_pair",
+                                    "demoting_to_the_committed_value_cancels_to_clean"};
+int fdbh_run_write_test(const char *name, int write_dev) {
+    bool known = false;
+    for (const char *w : WRITE_TESTS) known = known || !strcmp(w, name);
+    if (!known) { g_msg = "not a write-route test"; return 2; }
+    g_write_dev = write_dev != 0;
+    int rc = fdbh_run_test(name);
+    g_write_dev = false;
+    return rc;
 }
 
 void *fdbh_vm_from_csr(uint64_t nrows, uint64_t ncols, const uint64_t *Ap, const uint32_t *Aj) {
@@ -1067,6 +1114,74 @@ int fdbh_tensor_remove_all(void *t, const uint64_t *ids, const uint64_t *srcs, c
         std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rels;
         for (uint64_t q = 0; q < k; q++) rels.push_back(std::make_tuple(ids[q], srcs[q], dsts[q]));
         ((Tensor *)t)->remove_all(rels);
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+// Tensor::set_all_from_slices_dev / remove_all_dev (the device plans), and remove_all with its emptied pairs.  Emptied pairs are
+// malloc'ed (free with fdbh_free): the device route lists them ascending, the reference in discovery order.
+int fdbh_tensor_set_all_dev(void *t, const uint64_t *srcs, const uint64_t *dsts, const uint64_t *ids, uint64_t k) {
+    try {
+        ((Tensor *)t)->set_all_from_slices_dev(std::vector<uint64_t>(srcs, srcs + k), std::vector<uint64_t>(dsts, dsts + k),
+                                               std::vector<uint64_t>(ids, ids + k));
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+static int remove_emptied(void *t, const uint64_t *ids, const uint64_t *srcs, const uint64_t *dsts, uint64_t k, bool dev,
+                          uint64_t **out_src, uint64_t **out_dst, uint64_t *nout) {
+    try {
+        std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rels;
+        for (uint64_t q = 0; q < k; q++) rels.push_back(std::make_tuple(ids[q], srcs[q], dsts[q]));
+        auto em = dev ? ((Tensor *)t)->remove_all_dev(rels) : ((Tensor *)t)->remove_all(rels);
+        *nout = em.size();
+        *out_src = (uint64_t *)malloc(sizeof(uint64_t) * (em.size() + 1));
+        *out_dst = (uint64_t *)malloc(sizeof(uint64_t) * (em.size() + 1));
+        if (!*out_src || !*out_dst) { free(*out_src); free(*out_dst); throw std::bad_alloc(); }
+        for (size_t q = 0; q < em.size(); q++) { (*out_src)[q] = em[q].first; (*out_dst)[q] = em[q].second; }
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+int fdbh_tensor_remove_all_dev(void *t, const uint64_t *ids, const uint64_t *srcs, const uint64_t *dsts, uint64_t k,
+                               uint64_t **out_src, uint64_t **out_dst, uint64_t *nout) {
+    return remove_emptied(t, ids, srcs, dsts, k, true, out_src, out_dst, nout);
+}
+int fdbh_tensor_remove_all_emptied(void *t, const uint64_t *ids, const uint64_t *srcs, const uint64_t *dsts, uint64_t k,
+                                   uint64_t **out_src, uint64_t **out_dst, uint64_t *nout) {
+    return remove_emptied(t, ids, srcs, dsts, k, false, out_src, out_dst, nout);
+}
+// the six Delta counters (dp, dm; mt's dp, dm; me's dp, dm)
+int fdbh_tensor_counts(void *t, uint64_t *out6) {
+    try { ((const Tensor *)t)->counts(out6); return 0; } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+void *fdbh_tensor_dup(void *t) {
+    try { return new Tensor(((const Tensor *)t)->dup()); } catch (const std::exception &e) { g_msg = e.what(); return nullptr; }
+}
+int fdbh_tensor_fold_oversized(void *t) {
+    try { ((Tensor *)t)->fold_oversized(); return 0; } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+int fdbh_tensor_flush(void *t) {
+    try { ((Tensor *)t)->flush(); return 0; } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+int64_t fdbh_tensor_edge_count(void *t) {
+    try { return (int64_t)((const Tensor *)t)->edge_count(); } catch (const std::exception &e) { g_msg = e.what(); return -1; }
+}
+// VersionedMatrix::set_all<NEW> (route 0) or set_all_dev<NEW> (route 1) over the pairs (rows[k], cols[k])
+int fdbh_vm_set_all(void *vm, const uint64_t *rows, const uint64_t *cols, uint64_t k, int is_new, int route) {
+    try {
+        std::vector<std::pair<uint64_t, uint64_t>> e;
+        for (uint64_t q = 0; q < k; q++) e.push_back({rows[q], cols[q]});
+        VersionedMatrix *v = (VersionedMatrix *)vm;
+        if (route == 0) { if (is_new) v->set_all<true>(e); else v->set_all<false>(e); }
+        else { if (is_new) v->set_all_dev<true>(e); else v->set_all_dev<false>(e); }
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+// the two Delta counters and the three layer handles (m, dp, dm) of a VersionedMatrix, borrowed
+int fdbh_vm_state(void *vm, uint64_t *out2, void **out3) {
+    try {
+        const VersionedMatrix *v = (const VersionedMatrix *)vm;
+        v->wait_all();
+        v->counts(out2);
+        out3[0] = v->m().inner(); out3[1] = v->dp().inner(); out3[2] = v->dm().inner();
         return 0;
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
 }

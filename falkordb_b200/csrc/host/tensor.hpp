@@ -6,6 +6,7 @@
 // read the u64 values -- which is why edge id 0 must survive every structural round trip (tensor.rs:1427-1476).
 #pragma once
 #include "versioned_matrix.hpp"
+#include <algorithm>
 #include <map>
 #include <unordered_map>
 
@@ -136,20 +137,7 @@ class Tensor {
         std::vector<std::pair<uint64_t, uint64_t>> emptied;
         if (rels.empty()) return emptied;
         flush();
-        if (!has_multi_edge()) {                 // fast path: a few bulk GraphBLAS ops (same math as remove_mask)
-            wait_fwd();
-            uint64_t nr = fwd_m().nrows(), nc = fwd_m().ncols();
-            std::vector<uint64_t> mr, mc, tr, tc;
-            for (auto &r : rels) { mr.push_back(std::get<1>(r)); mc.push_back(std::get<2>(r)); tr.push_back(std::get<2>(r)); tc.push_back(std::get<1>(r)); }
-            Matrix<bool> m_mask(nr, nc), mt_mask(nc, nr);
-            m_mask.build(mr, mc);
-            mt_mask.build(tr, tc);
-            dm_.tombstone_masked(m_mask, fwd_m());   // PAIR never reads m's u64 values: edge id 0 is safe
-            dp_.remove_all(m_mask);
-            mt_.remove_mask(mt_mask);
-            for (auto &r : rels) emptied.push_back({std::get<1>(r), std::get<2>(r)});
-            return emptied;
-        }
+        if (!has_multi_edge()) return remove_bulk(rels);
         wait_fwd();
         enum Kind { Multi, Single, Emptied, Absent };
         struct Plan { Kind kind; std::vector<uint64_t> ids; uint64_t id = 0; bool demoted = false; };
@@ -200,6 +188,118 @@ class Tensor {
                 uint64_t committed;
                 if (fwd_m().get(src, dst, &committed) && committed == p.id) dp_.erase(src, dst);
                 else dp_set.push_back(std::make_tuple(src, dst, p.id));
+            }
+        }
+        for (auto &t : dp_set) dp_.insert(std::get<0>(t), std::get<1>(t), std::get<2>(t));
+        return emptied;
+    }
+
+    // remove_all's fast path when no pair has several edges: a few bulk GraphBLAS ops (same math as remove_mask).  Every named
+    // pair is removed and reported, whatever id names it.
+    std::vector<std::pair<uint64_t, uint64_t>> remove_bulk(const std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> &rels) {
+        std::vector<std::pair<uint64_t, uint64_t>> emptied;
+        wait_fwd();
+        uint64_t nr = fwd_m().nrows(), nc = fwd_m().ncols();
+        std::vector<uint64_t> mr, mc, tr, tc;
+        for (auto &r : rels) { mr.push_back(std::get<1>(r)); mc.push_back(std::get<2>(r)); tr.push_back(std::get<2>(r)); tc.push_back(std::get<1>(r)); }
+        Matrix<bool> m_mask(nr, nc), mt_mask(nc, nr);
+        m_mask.build(mr, mc);
+        mt_mask.build(tr, tc);
+        dm_.tombstone_masked(m_mask, fwd_m());   // PAIR never reads m's u64 values: edge id 0 is safe
+        dp_.remove_all(m_mask);
+        mt_.remove_mask(mt_mask);
+        for (auto &r : rels) emptied.push_back({std::get<1>(r), std::get<2>(r)});
+        return emptied;
+    }
+
+    // the nine layer handles (B200_TensorLayers order), borrowed
+    B200_TensorLayers layers() const {
+        return B200_TensorLayers{fwd_m().inner(), fwd_dp().inner(), fwd_dm().inner(), mt_.m().inner(), mt_.dp().inner(), mt_.dm().inner(),
+                                 me_.m().inner(), me_.dp().inner(), me_.dm().inner()};
+    }
+    // the six Delta counters: dp, dm, mt's dp, dm, me's dp, dm
+    void counts(uint64_t *out6) const {
+        out6[0] = dp_.get_count(); out6[1] = dm_.get_count();
+        mt_.counts(out6 + 2);
+        me_.counts(out6 + 4);
+    }
+
+    // set_all_from_slices with its read phase as one device call (B200_Tensor_insert_plan): the plan replaces every dp.get /
+    // dm.contains / m.get / mt.m / me.m probe, so a base with no host form is never downloaded.  The write phase makes the
+    // reference's Delta calls, in number and, where the order can change a counter, in order.
+    void set_all_from_slices_dev(const std::vector<uint64_t> &srcs, const std::vector<uint64_t> &dsts, const std::vector<uint64_t> &ids) {
+        if (srcs.empty()) return;
+        if (srcs.size() != dsts.size() || srcs.size() != ids.size()) throw std::logic_error("set_all_from_slices_dev: slices differ in length");
+        flush();
+        fwd_dp().wait();
+        fwd_dm().wait();
+        const size_t n = srcs.size();
+        std::vector<uint64_t> in_src(n), in_dst(n), in_val(n), me_key(2 * n), me_id(2 * n);
+        std::vector<uint8_t> in_flags(n), me_base(2 * n);
+        uint64_t nin = 0, nme = 0;
+        B200_TensorLayers L = layers();
+        grb_ok(B200_Tensor_insert_plan(&L, srcs.data(), dsts.data(), ids.data(), n, in_src.data(), in_dst.data(), in_val.data(),
+                                       in_flags.data(), &nin, me_key.data(), me_id.data(), me_base.data(), &nme),
+               "B200_Tensor_insert_plan");
+        for (uint64_t k = 0; k < nme; k++) me_.set_known(me_key[k], me_id[k], me_base[k] != 0);
+        // dp takes inserts and (CANCEL) erases of absent entries.  Its counter saturates at 0, so when the erases could reach 0 the
+        // records go in the reference's order, the batch order of each pair's first edge; every other layer takes one kind of call
+        // and any order gives the same counter.
+        std::vector<uint64_t> order(nin);
+        for (uint64_t k = 0; k < nin; k++) order[k] = k;
+        uint64_t cancels = 0;
+        for (uint64_t k = 0; k < nin; k++) cancels += (in_flags[k] & B200_PLAN_CANCEL) != 0;
+        if (cancels > dp_.get_count()) {
+            std::unordered_map<uint64_t, uint64_t> first;
+            for (size_t t = n; t-- > 0;) first[compound_key(srcs[t], dsts[t])] = t;
+            std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) {
+                return first[compound_key(in_src[a], in_dst[a])] < first[compound_key(in_src[b], in_dst[b])];
+            });
+        }
+        for (uint64_t k : order) {
+            const uint64_t s = in_src[k], d = in_dst[k], id = in_val[k];
+            const uint8_t f = in_flags[k];
+            mt_.set_known(d, s, (f & B200_PLAN_MT_BASE) != 0);
+            if (f & B200_PLAN_COMMITTED) {
+                dm_.erase(s, d);
+                if (f & B200_PLAN_CANCEL) { dp_.erase(s, d); continue; }
+            }
+            dp_.insert(s, d, id);
+        }
+    }
+
+    // remove_all with its read phase as one device call (B200_Tensor_remove_plan).  Without multi-edges it keeps remove_all's bulk
+    // path, which removes a named pair whatever id names it.  Emptied pairs come back ascending (the reference: discovery order).
+    std::vector<std::pair<uint64_t, uint64_t>> remove_all_dev(const std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> &rels) {
+        std::vector<std::pair<uint64_t, uint64_t>> emptied;
+        if (rels.empty()) return emptied;
+        flush();
+        if (!has_multi_edge()) return remove_bulk(rels);
+        wait_fwd();
+        const size_t n = rels.size();
+        std::vector<uint64_t> rid(n), rs(n), rd(n);
+        for (size_t k = 0; k < n; k++) { rid[k] = std::get<0>(rels[k]); rs[k] = std::get<1>(rels[k]); rd[k] = std::get<2>(rels[k]); }
+        std::vector<uint64_t> pr_src(n), pr_dst(n), pr_val(n), me_key(2 * n), me_id(2 * n);
+        std::vector<uint8_t> pr_flags(n), me_base(2 * n);
+        uint64_t npr = 0, nme = 0;
+        B200_TensorLayers L = layers();
+        grb_ok(B200_Tensor_remove_plan(&L, rid.data(), rs.data(), rd.data(), n, pr_src.data(), pr_dst.data(), pr_val.data(),
+                                       pr_flags.data(), &npr, me_key.data(), me_id.data(), me_base.data(), &nme),
+               "B200_Tensor_remove_plan");
+        for (uint64_t k = 0; k < nme; k++) me_.remove_known(me_key[k], me_id[k], me_base[k] != 0);
+        std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> dp_set;
+        for (uint64_t k = 0; k < npr; k++) {                     // pairs ascending, as remove_all's std::map walk
+            const uint64_t src = pr_src[k], dst = pr_dst[k];
+            const uint8_t f = pr_flags[k];
+            if (f & B200_PLAN_EMPTIED) {
+                dp_.erase(src, dst);
+                if (f & B200_PLAN_M_HAS) dm_.insert(src, dst);
+                mt_.remove_known(dst, src, (f & B200_PLAN_MT_BASE) != 0);
+                emptied.push_back({src, dst});
+            } else if (f & B200_PLAN_M_EQ) {
+                dp_.erase(src, dst);
+            } else {
+                dp_set.push_back(std::make_tuple(src, dst, pr_val[k]));
             }
         }
         for (auto &t : dp_set) dp_.insert(std::get<0>(t), std::get<1>(t), std::get<2>(t));

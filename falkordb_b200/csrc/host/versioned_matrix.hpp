@@ -214,6 +214,18 @@ class VersionedMatrix {
         if (m().get(i, j)) dm_.insert(i, j);
         else dp_.erase(i, j);
     }
+    // set / remove with the base probe m().get(i, j) supplied by the caller (a write plan read it on the device): the same Delta
+    // calls, no read of m
+    void set_known(uint64_t i, uint64_t j, bool in_base) {
+        flush();
+        if (in_base) dm_.erase(i, j);
+        else dp_.insert(i, j);
+    }
+    void remove_known(uint64_t i, uint64_t j, bool in_base) {
+        flush();
+        if (in_base) dm_.insert(i, j);
+        else dp_.erase(i, j);
+    }
     void remove_mask(const Matrix<bool> &mask) {                // :799-816
         flush();
         m().wait();
@@ -233,6 +245,31 @@ class VersionedMatrix {
             for (auto &e : entries) set(e.first, e.second);
         }
     }
+
+    // set_all with its per-entry m.get as one B200_Matrix_extract_pairs call (made only when a probe is read): the same Delta calls
+    template <bool NEW>
+    void set_all_dev(const std::vector<std::pair<uint64_t, uint64_t>> &entries) {
+        flush();
+        dm().wait();
+        const bool dm_empty = dm().nvals() == 0;
+        std::vector<uint8_t> in_base(entries.size(), 0);
+        if (!entries.empty() && (!NEW || !dm_empty)) {
+            std::vector<uint64_t> I(entries.size()), J(entries.size());
+            for (size_t k = 0; k < entries.size(); k++) { I[k] = entries[k].first; J[k] = entries[k].second; }
+            grb_ok(B200_Matrix_extract_pairs(m().inner(), I.data(), J.data(), I.size(), in_base.data(), nullptr),
+                   "B200_Matrix_extract_pairs");
+        }
+        if (dm_empty) {
+            for (size_t k = 0; k < entries.size(); k++) {
+                if (!NEW && in_base[k]) continue;
+                dp_.insert(entries[k].first, entries[k].second);
+            }
+        } else {
+            for (size_t k = 0; k < entries.size(); k++) set_known(entries[k].first, entries[k].second, in_base[k] != 0);
+        }
+    }
+    // the two Delta counters (dp, dm)
+    void counts(uint64_t *out2) const { out2[0] = dp_.get_count(); out2[1] = dm_.get_count(); }
 
     void flush() {                                              // :892-938
         if (!needs_flush.load(std::memory_order_relaxed)) return;

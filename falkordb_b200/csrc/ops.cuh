@@ -139,6 +139,18 @@ struct EdgeTypeDev {  // one relationship type: forward m / dp (u64 values) / dm
 u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<EdgeTypeDev> &types, int dir, int mode, u64 *out_p,
                 u32 *out_node, u64 *out_edge, uint16_t *out_type, uint8_t *out_rev, u64 capacity);
 
+// writes.cu : the read phase of a Tensor's batched relationship inserts and deletes (B200_Tensor_insert_plan / _remove_plan),
+// over one type's live layers (m, dp, dm, mt and the me stores of EdgeTypeDev; mt_dp / mt_dm are not read).  The flags are
+// include/b200grb.h's B200_PLAN_*.  The plan goes to the caller's host arrays: rec_* (capacity n) and me_* (capacity 2n).
+enum : uint8_t { WP_COMMITTED = 1, WP_CANCEL = 2, WP_MT_BASE = 4, WP_EMPTIED = 8, WP_DEMOTED = 16, WP_M_HAS = 32, WP_M_EQ = 64 };
+struct WritePlan {
+    u64 *rec_src, *rec_dst, *rec_val; uint8_t *rec_flags; u64 nrec;
+    u64 *me_key, *me_id; uint8_t *me_base; u64 nme;
+};
+// n >= 1; src / dst < nv, ids < 2^60 (checked by the caller)
+void tensor_insert_plan(const EdgeTypeDev &t, const u64 *d_src, const u64 *d_dst, const u64 *d_id, u64 n, u64 nv, WritePlan &P);
+void tensor_remove_plan(const EdgeTypeDev &t, const u64 *d_id, const u64 *d_src, const u64 *d_dst, u64 n, u64 nv, WritePlan &P);
+
 // adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
 // replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
 // and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.

@@ -152,7 +152,8 @@ static u64 g_n[TK_COUNT_], g_bytes[TK_COUNT_];
 const char *timed_name(int id) {
     static const char *names[] = {"bits_pull", "bits_push", "heavy_accumulate", "small_rows", "bits_fill",
                                   "bits_count", "bitmap_expand", "bfs_expand", "union", "filter", "mxv_fp64", "spgemm_masked", "transpose",
-                                  "bits_delta", "bits_repair", "bits_pull_acc", "bits_push_acc", "edge_expand", "bfs_delta", "adj_build"};
+                                  "bits_delta", "bits_repair", "bits_pull_acc", "bits_push_acc", "edge_expand", "bfs_delta", "adj_build",
+                                  "tensor_write"};
     return (id >= 0 && id < TK_COUNT_) ? names[id] : "?";
 }
 static cudaEvent_t get_event() {

@@ -601,3 +601,41 @@ def expand_edges(sources, types, dir=DIR_OUT, mode=EDGES_ALL, targets=None, capa
         break
     m = nv.value
     return p, node[:m], edge[:m], typ[:m], rev[:m]
+
+
+PLAN_COMMITTED, PLAN_CANCEL, PLAN_MT_BASE, PLAN_EMPTIED, PLAN_DEMOTED, PLAN_M_HAS, PLAN_M_EQ = 1, 2, 4, 8, 16, 32, 64
+
+
+def _layers1(t):
+    ls = TensorLayers()
+    vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
+    for name, x in zip(TENSOR_LAYERS, vals):
+        setattr(ls, name, _handle(x))
+    return ls
+
+
+def _plan(fn, t, a, b, c):
+    a, b, c = _u64arr(a), _u64arr(b), _u64arr(c)
+    n = len(a)
+    assert len(b) == n and len(c) == n, "one entry per edge in each slice"
+    rs, rd, rv, rf = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint8)
+    mk, mi, mb = np.zeros(max(2 * n, 1), np.uint64), np.zeros(max(2 * n, 1), np.uint64), np.zeros(max(2 * n, 1), np.uint8)
+    nr, nm = U64(0), U64(0)
+    check(fn(C.byref(_layers1(t)), a.ctypes.data if n else None, b.ctypes.data if n else None, c.ctypes.data if n else None, n,
+             rs.ctypes.data, rd.ctypes.data, rv.ctypes.data, rf.ctypes.data, C.byref(nr), mk.ctypes.data, mi.ctypes.data, mb.ctypes.data,
+             C.byref(nm)))
+    r, m = nr.value, nm.value
+    return {"src": rs[:r], "dst": rd[:r], "val": rv[:r], "flags": rf[:r], "me_key": mk[:m], "me_id": mi[:m], "me_base": mb[:m].astype(bool)}
+
+
+def insert_plan(t, srcs, dsts, ids):
+    """B200_Tensor_insert_plan: the read phase of Tensor::set_all_from_slices over one type's layers `t` (a sequence or dict in
+    TENSOR_LAYERS order, as expand_edges takes them).  Returns a dict of numpy arrays: the inline records (src, dst, val, flags) and
+    the me entries (me_key, me_id, me_base)."""
+    return _plan(lib().B200_Tensor_insert_plan, t, srcs, dsts, ids)
+
+
+def remove_plan(t, ids, srcs, dsts):
+    """B200_Tensor_remove_plan: the read phase of Tensor::remove_all's multi-edge path; the pair records (src, dst, val, flags) and
+    the me entries, as insert_plan returns them."""
+    return _plan(lib().B200_Tensor_remove_plan, t, ids, srcs, dsts)

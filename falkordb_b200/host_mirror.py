@@ -1,5 +1,6 @@
 """ctypes binding of libfdbhost.so, the C++ host mirror of the reference's Tensor and CondTraverse (csrc/host): a relationship
-Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending, and the routes that read its
+Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending (through the reference's read phase
+or the device plans, B200_Tensor_insert_plan / B200_Tensor_remove_plan), and the routes that read its
 relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), and the algo.BFS, algo.pageRank, algo.WCC
 and algo.labelPropagation procedures over them."""
 import ctypes as C
@@ -15,6 +16,7 @@ _L = None
 ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
 BFS_DEVICE, BFS_BY_EXTRACT = 0, 1
 ALGO_DEVICE, ALGO_BY_EXTRACT = 0, 1
+WRITE_REFERENCE, WRITE_DEVICE = 0, 1
 
 
 def host():
@@ -29,6 +31,19 @@ def host():
     L.fdbh_tensor_set_all.argtypes = [P, P, P, P, U64]
     L.fdbh_tensor_remove_all.argtypes = [P, P, P, P, U64]
     L.fdbh_tensor_layers.argtypes = [P, P]
+    L.fdbh_tensor_set_all_dev.argtypes = [P, P, P, P, U64]
+    L.fdbh_tensor_remove_all_dev.argtypes = [P, P, P, P, U64, C.POINTER(P), C.POINTER(P), C.POINTER(U64)]
+    L.fdbh_tensor_remove_all_emptied.argtypes = [P, P, P, P, U64, C.POINTER(P), C.POINTER(P), C.POINTER(U64)]
+    L.fdbh_tensor_counts.argtypes = [P, P]
+    L.fdbh_tensor_dup.argtypes = [P]
+    L.fdbh_tensor_dup.restype = P
+    L.fdbh_tensor_fold_oversized.argtypes = [P]
+    L.fdbh_tensor_flush.argtypes = [P]
+    L.fdbh_tensor_edge_count.argtypes = [P]
+    L.fdbh_tensor_edge_count.restype = C.c_int64
+    L.fdbh_vm_set_all.argtypes = [P, P, P, U64, C.c_int, C.c_int]
+    L.fdbh_vm_state.argtypes = [P, P, P]
+    L.fdbh_run_write_test.argtypes = [C.c_char_p, C.c_int]
     L.fdbh_expand_edges.argtypes = [P, U64, P, P, U64, C.c_int, C.c_int, C.c_int] + [P] * 5 + [C.POINTER(U64)]
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
     algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
@@ -65,17 +80,65 @@ class Tensor:
             self.L.fdbh_tensor_free(self.h)
             self.h = None
 
-    def add(self, src, dst, ids):
-        """Tensor::set_all_from_slices"""
-        a = _u64(src, dst, ids)
-        if self.L.fdbh_tensor_set_all(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0])):
+    @classmethod
+    def _adopt(cls, h):
+        t = cls.__new__(cls)
+        t.L = host()
+        if not h:
+            raise RuntimeError(t.L.fdbh_last_message().decode())
+        t.h = h
+        return t
+
+    def _check(self, rc):
+        if rc:
             raise RuntimeError(self.L.fdbh_last_message().decode())
 
-    def remove(self, ids, src, dst):
-        """Tensor::remove_all"""
+    def add(self, src, dst, ids, route=WRITE_REFERENCE):
+        """Tensor::set_all_from_slices, or with route=WRITE_DEVICE set_all_from_slices_dev (its read phase as one device plan)"""
+        a = _u64(src, dst, ids)
+        fn = self.L.fdbh_tensor_set_all_dev if route == WRITE_DEVICE else self.L.fdbh_tensor_set_all
+        self._check(fn(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0])))
+
+    def remove(self, ids, src, dst, route=WRITE_REFERENCE):
+        """Tensor::remove_all, or with route=WRITE_DEVICE remove_all_dev.  Returns the emptied pairs as a (k, 2) uint64 array: the
+        reference lists them in discovery order, the device route ascending."""
         a = _u64(ids, src, dst)
-        if self.L.fdbh_tensor_remove_all(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0])):
+        fn = self.L.fdbh_tensor_remove_all_dev if route == WRITE_DEVICE else self.L.fdbh_tensor_remove_all_emptied
+        ps, pd, nv = C.c_void_p(), C.c_void_p(), U64(0)
+        self._check(fn(self.h, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data, len(a[0]), C.byref(ps), C.byref(pd), C.byref(nv)))
+        k = nv.value
+        out = np.zeros((k, 2), np.uint64)
+        for col, x in enumerate((ps, pd)):
+            if k:
+                out[:, col] = np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64)
+            self.L.fdbh_free(x)
+        return out
+
+    def dup(self):
+        """Tensor::dup: a new version sharing the layers copy-on-write"""
+        return Tensor._adopt(self.L.fdbh_tensor_dup(self.h))
+
+    def fold_oversized(self):
+        self._check(self.L.fdbh_tensor_fold_oversized(self.h))
+
+    def flush(self):
+        self._check(self.L.fdbh_tensor_flush(self.h))
+
+    def edge_count(self):
+        n = self.L.fdbh_tensor_edge_count(self.h)
+        if n < 0:
             raise RuntimeError(self.L.fdbh_last_message().decode())
+        return n
+
+    def counts(self):
+        """the six Delta counters: dp, dm, mt's dp, dm, me's dp, dm"""
+        out = np.zeros(6, np.uint64)
+        self._check(self.L.fdbh_tensor_counts(self.h, out.ctypes.data))
+        return out
+
+    def tuples(self):
+        """the nine layers' stored entries (TENSOR_LAYERS order) as (rows, cols, values or None) numpy arrays, after Tensor::wait()"""
+        return [_tuples(h, k < 2) for k, h in enumerate(self.layers())]
 
     def layers(self):
         """the nine layer handles in B200_TensorLayers order, after Tensor::wait(); valid until the tensor changes"""
@@ -127,6 +190,40 @@ class VersionedMatrix:
     def remove(self, i, j):
         if self.L.fdbh_vm_remove(self.h, int(i), int(j)):
             raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def set_all(self, rows, cols, new=False, route=WRITE_REFERENCE):
+        """VersionedMatrix::set_all<NEW>, or with route=WRITE_DEVICE set_all_dev<NEW> (one batched base probe)"""
+        r, c = _u64(rows, cols)
+        if self.L.fdbh_vm_set_all(self.h, r.ctypes.data, c.ctypes.data, len(r), 1 if new else 0, route):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+
+    def state(self):
+        """(the two Delta counters, the (rows, cols) of m, dp and dm)"""
+        cnt, hs = np.zeros(2, np.uint64), (C.c_void_p * 3)()
+        if self.L.fdbh_vm_state(self.h, cnt.ctypes.data, hs):
+            raise RuntimeError(self.L.fdbh_last_message().decode())
+        return cnt, [_tuples(hs[k], False)[:2] for k in range(3)]
+
+
+def _tuples(h, valued):
+    from ._lib import lib, check
+    L = lib()
+    n = U64(0)
+    check(L.GrB_Matrix_nvals(C.byref(n), h))
+    k = n.value
+    rows, cols = np.zeros(max(k, 1), np.uint64), np.zeros(max(k, 1), np.uint64)
+    vals = np.zeros(max(k, 1), np.uint64) if valued else None
+    nv = U64(max(k, 1))
+    fn = L.GrB_Matrix_extractTuples_UINT64 if valued else L.GrB_Matrix_extractTuples_BOOL
+    check(fn(rows.ctypes.data, cols.ctypes.data, None if vals is None else vals.ctypes.data, C.byref(nv), h))
+    return rows[:k], cols[:k], None if vals is None else vals[:k]
+
+
+def run_write_test(name, route):
+    """one transcribed tensor.rs test with its writes through `route` (WRITE_REFERENCE / WRITE_DEVICE); '' on success"""
+    L = host()
+    rc = L.fdbh_run_write_test(name.encode(), route)
+    return "" if rc == 0 else L.fdbh_last_message().decode()
 
 
 def algo_bfs(adj, all_types, named, src, max_depth=-1, want_edges=True, deleted=(), route=BFS_DEVICE):

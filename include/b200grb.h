@@ -409,6 +409,41 @@ typedef struct {
 GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, GrB_Index n, const B200_TensorLayers *types,
                            int ntypes, int dir, int mode, uint64_t *out_p, uint32_t *out_node, uint64_t *out_edge,
                            uint16_t *out_type, uint8_t *out_rev, uint64_t out_capacity, uint64_t *nout);
+/* Flags of the write plans below. */
+#define B200_PLAN_COMMITTED 0x01 /* insert: m holds the pair, its value is to be reconciled (dm.erase) */
+#define B200_PLAN_CANCEL 0x02    /* insert: COMMITTED and m's value equals the new inline value (dp.erase instead of dp.insert) */
+#define B200_PLAN_MT_BASE 0x04   /* insert / remove: mt's base m holds (dst, src) */
+#define B200_PLAN_EMPTIED 0x08   /* remove: the pair lost its last edge */
+#define B200_PLAN_DEMOTED 0x10   /* remove: the pair is down to one edge, pr_val */
+#define B200_PLAN_M_HAS 0x20     /* remove: m holds the pair */
+#define B200_PLAN_M_EQ 0x40      /* remove: DEMOTED and m's value equals the survivor */
+/* The read phase of Tensor::set_all_from_slices (tensor.rs:333-447) and of Tensor::remove_all's multi-edge path (:454-629) for a
+ * whole batch, on the device, over one relationship type's layers as they stand before the batch (m, dp, dm, mt, me, and for
+ * removes me_dp / me_dm; mt_dp / mt_dm are checked but not read).  The caller then makes the reference's write calls from the plan
+ * and reads no layer.  No layer changes, apart from finishing pending tuples.
+ * Insert: each distinct pair P with batch ids i1..ig in batch order; cur = dp's value if present, else none if dm holds P, else m's.
+ *  - cur MULTI_EDGE: me entries i1..ig, no inline record;
+ *  - cur a single id c: me entries c, i1..ig, inline MULTI_EDGE; COMMITTED when dp held P and m holds P;
+ *  - none, g = 1: inline i1;  none, g >= 2: me entries i1..ig, inline MULTI_EDGE; COMMITTED when dm held P and m holds P.
+ *  Inline records (in_src, in_dst, in_val, in_flags: COMMITTED, CANCEL, MT_BASE) at most n; me entries (me_key = src << 32 | dst,
+ *  me_id, me_base = me's base m holds (key, id)) at most 2n.
+ * Remove: each distinct pair with its distinct batch ids R, by Tensor::eff_get:
+ *  - a single id x: an EMPTIED record when x is in R;
+ *  - MULTI_EDGE with the merged id list L = (me \ me_dm) u me_dp, H = R n L nonempty, rem = L \ H: |rem| >= 2: me entries H; |rem|
+ *    = 1: me entries L and a DEMOTED record, pr_val = the survivor; |rem| = 0: me entries L and an EMPTIED record.  A list of
+ *    fewer than two ids (only reached by adding an id the pair already holds) takes the |rem| >= 2 row, as the host's walk does.
+ *  Pair records (pr_*: EMPTIED / DEMOTED, M_HAS, MT_BASE, M_EQ; pr_val the survivor, else the pair's value before the batch) at most
+ *  n; me entries at most 2n.  The reference lists emptied pairs in discovery order; its callers use them as a set.
+ * Pairs ascending; a pair's me entries in the order above (insert) or ascending (remove).
+ * Errors: m or mt NULL GrB_NULL_POINTER; m / dp not UINT64 GrB_DOMAIN_MISMATCH; layers not square of one size n
+ * GrB_DIMENSION_MISMATCH; src / dst >= n or an id >= 2^60 GrB_INVALID_INDEX; host-resident m GrB_NOT_IMPLEMENTED; n == 0 success
+ * with no device work; with no device GxB_GPU_ERROR before any host work. */
+GrB_Info B200_Tensor_insert_plan(const B200_TensorLayers *t, const GrB_Index *srcs, const GrB_Index *dsts, const GrB_Index *ids,
+                                 GrB_Index n, uint64_t *in_src, uint64_t *in_dst, uint64_t *in_val, uint8_t *in_flags, uint64_t *nin,
+                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme);
+GrB_Info B200_Tensor_remove_plan(const B200_TensorLayers *t, const GrB_Index *ids, const GrB_Index *srcs, const GrB_Index *dsts,
+                                 GrB_Index n, uint64_t *pr_src, uint64_t *pr_dst, uint64_t *pr_val, uint8_t *pr_flags, uint64_t *npr,
+                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme);
 GrB_Info B200_sync(void);
 GrB_Info B200_pool_trim(void); /* hand the caching allocator's free device blocks back to the driver */
 void *B200_stream(void); /* the cudaStream_t every kernel of this library is launched on */

@@ -36,6 +36,13 @@ WANT = [
     ("WCC hook", r"k_cc_hook"),
     ("CDLP pick", r"k_cdlp_pick"),
     ("bulk tensor build, run marking", r"k_bulk_mark"),
+    ("relationship ids, count", r"k_ee_count"),
+    ("relationship ids, fill", r"k_ee_fill"),
+    ("insert plan, count", r"k_ins_count"),
+    ("insert plan, fill", r"k_ins_fill"),
+    ("remove plan, count", r"k_rm_count"),
+    ("remove plan, fill", r"k_rm_fill"),
+    ("write plans, run heads", r"k_wp_heads"),
 ]
 OPS = [("LDG.*\\.256", r"\bLDG\.[A-Z0-9_.]*256"), ("LDG.*\\.128", r"\bLDG\.[A-Z0-9_.]*128"), ("LDG.*\\.64", r"\bLDG\.[A-Z0-9_.]*\.64\b"),
        ("LDG other", r"\bLDG\."), ("STG.*\\.256", r"\bSTG\.[A-Z0-9_.]*256"), ("STG.*\\.128", r"\bSTG\.[A-Z0-9_.]*128"), ("STG other", r"\bSTG\."),
