@@ -43,7 +43,8 @@ k_mxv_fp64(const u64 *__restrict__ p, const u32 *__restrict__ j, const u64 *__re
 void mxv_fp64(const DevCSR &A, bool use_values, const double *x, const unsigned char *present, double *y, unsigned char *ypresent,
               double init, bool accum) {
     if (!A.nrows) return;
-    if (use_values && !A.has_values()) throw GrbError(-5, "PLUS_TIMES needs a valued matrix");
+    // a valued matrix without entries has no value array on the device: its product is empty, not a domain error
+    if (use_values && A.nnz && !A.has_values()) throw GrbError(-5, "PLUS_TIMES needs a valued matrix");
     // algorithmic bytes: col_idx + (values) + row pointers + one 8-byte gather per entry + y
     TimedScope ts(TK_MXV, (use_values ? 12 : 4) * A.nnz + 8 * (A.nrows + 1) + 8 * A.nnz + 8 * A.nrows);
     const u32 grid = grid_for(A.nrows * 8, 256, (u64)ctx().num_sms * 32);

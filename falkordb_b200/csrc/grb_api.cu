@@ -1534,7 +1534,8 @@ static double vec_value_f64(GrB_Vector v, u64 k) {       // k-th stored entry as
         if (v->type == T_FP64) return ((const double *)v->fx)[k];
         return v->type == T_INT64 ? (double)(i64)vec_at(v, k) : (double)vec_at(v, k);
     }
-    return v->type == T_FP64 ? bits_f64(v->val[k]) : (double)v->val[k];
+    if (v->type == T_FP64) return bits_f64(v->val[k]);
+    return v->type == T_UINT64 ? (double)(u64)v->val[k] : (double)v->val[k];     // `val` is i64: UINT64 >= 2^63 must not turn negative
 }
 GrB_Info GrB_Vector_setElement_FP64(GrB_Vector v, double x, GrB_Index i) {
     CHECK_PTR(v);
