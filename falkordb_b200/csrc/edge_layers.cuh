@@ -30,6 +30,12 @@ __device__ __forceinline__ u64 ub32(const u32 *__restrict__ j, u64 lo, u64 hi, u
     while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] <= c) lo = mid + 1; else hi = mid; }
     return lo;
 }
+// largest g with lstart[g] <= e (lstart ascending, lstart[0] = 0): the segment of flat position e behind a scan of lengths
+__device__ __forceinline__ u64 list_at(const u64 *__restrict__ lstart, u64 G, u64 e) {
+    u64 lo = 0, hi = G - 1;
+    while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (lstart[mid] <= e) lo = mid; else hi = mid - 1; }
+    return lo;
+}
 // position of (r, c) in A, or ~0
 __device__ __forceinline__ u64 find_rc(const ECsr &A, u64 r, u32 c) {
     if (!A.p) return ~0ULL;
@@ -78,5 +84,12 @@ __device__ u64 merged_ids(const EType &t, u64 key, F f) {
     }
     return k;
 }
+
+// edges.cu: the adjacency of n >= 1 distinct nodes d_src (device) over T types dt (device), in Graph::get_node_relationships_by_type's
+// order (graph.rs:1797-1835): per node, types in order; per type the outgoing half (neighbour ascending, ids ascending), then the
+// incoming half (source ascending); under dir 2 a self-loop once, in the outgoing half.  Device outputs: node i covers
+// p[i] .. p[i+1] of node (the neighbour) and edge (the id).  Returns the entries; adds the passes' compulsory bytes to *bytes.
+u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
+                   u64 *bytes);
 
 } // namespace b200

@@ -14,6 +14,8 @@
 // counts of the entries ahead of it -- smaller neighbours, and the same neighbour in a lower-index type -- read from the scan of
 // the counts with one binary search per list (2T per entry; ewise.cu's rank sums).  No sort and no merge loop.
 // Fill.  node, id, type and direction of every output entry; a MULTI_EDGE entry writes its merged id list.
+// edge_adjacency (the trail enumerator's per-level fetch, trails.cu) runs the same lists, counts and scan over device-resident
+// rows, and places the entries in Graph::get_node_relationships_by_type's order instead (k_ee_ref_fill): type, block, neighbour.
 // The me layers are host-resident (2^60 x 2^60); their sorted (key, ids) stores are uploaded once and cached on the handle.
 #include "edge_layers.cuh"
 
@@ -39,12 +41,6 @@ __device__ __forceinline__ ListId list_of(const EArgs &A, u64 g) {
     return r;
 }
 __device__ __forceinline__ const ECsr &layer_of(const EType &t, bool rev, u32 l) { return rev ? (l ? t.mtdp : t.mt) : (l ? t.dp : t.m); }
-// largest g with lstart[g] <= e (lstart ascending, lstart[0] = 0)
-__device__ __forceinline__ u64 list_at(const u64 *__restrict__ lstart, u64 G, u64 e) {
-    u64 lo = 0, hi = G - 1;
-    while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (lstart[mid] <= e) lo = mid; else hi = mid - 1; }
-    return lo;
-}
 
 // per list: its first position in the layer's col_idx and its length.  stat[0] += forward entries, stat[1] += reverse entries,
 // stat[2] += entries of the delta-minus rows the count pass searches (the byte formula)
@@ -174,6 +170,95 @@ __global__ void k_ee_fill(EArgs A, const u64 *__restrict__ lstart, const u64 *__
     }
 }
 
+// The reference's order (edge_adjacency): per row, type, then block (outgoing, then incoming), then neighbour and id.  An entry's
+// position is the row offset, plus the counts of every list of an earlier (type, block), plus the entries ahead of it in its own
+// list and in the other layer of its (type, block) -- one binary search.  A base entry and a delta-plus entry never both count.
+__global__ void k_ee_ref_fill(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo, const u64 *__restrict__ len,
+                              const u64 *__restrict__ val, const u32 *__restrict__ cnt, const u64 *__restrict__ pos,
+                              u32 *__restrict__ node, u64 *__restrict__ edge) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < A.E; e += (u64)gridDim.x * blockDim.x) {
+        const u32 c = cnt[e];
+        if (!c) continue;
+        const u64 g = list_at(lstart, A.G, e);
+        const ListId L = list_of(A, g);
+        const EType &t = A.types[L.t];
+        const u32 x = layer_of(t, L.rev, L.l).j[lo[g] + (e - lstart[g])];
+        const u64 row = g - (g % (2 * (u64)A.T * A.nb));
+        u64 o = pos[lstart[row]];
+        for (u32 t2 = 0; t2 <= L.t; t2++)
+            for (u32 b2 = 0; b2 < A.nb && (t2 < L.t || b2 < L.b); b2++) {
+                const u64 g2 = row + 2 * ((u64)b2 * A.T + t2);
+                o += pos[lstart[g2 + 2]] - pos[lstart[g2]];
+            }
+        const u64 g0 = g & ~1ULL;
+        for (u32 l2 = 0; l2 < 2; l2++) {
+            const u64 g2 = g0 + l2;
+            const u64 e2 = g2 == g ? e : rank_in(A, lstart, lo, len, g2, L.rev, x, false);
+            o += pos[e2] - pos[lstart[g2]];
+        }
+        const u64 v = val[e];
+        auto put = [&](u64 k, u64 id) {
+            node[o + k] = x;
+            edge[o + k] = id;
+            return k + 1 < c;
+        };
+        if (v != EE_MULTI) put(0, v);
+        else {
+            const u64 s = A.src[L.i];
+            merged_ids(t, L.rev ? ((u64)x << 32 | s) : (s << 32 | x), put);
+        }
+    }
+}
+
+// The passes before the fill, shared by both orders: the lists, their entries' values and counts, and the scan of the counts.
+struct EeBatch {
+    EArgs A;
+    DevBuf<u64> lo, llen, lstart, stat, val, pos;
+    DevBuf<u32> cnt, first;
+    u32 *fin = nullptr;
+    u64 h[4] = {0, 0, 0, 0};         // forward entries, reverse entries, delta-minus entries searched, list entries
+    explicit EeBatch(const EArgs &a) : A(a), lo(a.G), llen(a.G + 1), lstart(a.G + 1), stat(3) { stat.zero(); }
+    void prepare(int mode, u32 grid) {
+        CUDA_TRY(cudaMemsetAsync(llen.ptr + A.G, 0, sizeof(u64), stream()));
+        LAUNCH(k_ee_lists, grid_for(A.G, 256, grid), 256, 0, A, lo.ptr, llen.ptr, stat.ptr);
+        exclusive_scan_u64(llen.ptr, lstart.ptr, A.G + 1);
+        d2h(h, stat.ptr, 3);
+        d2h(h + 3, lstart.ptr + A.G, 1);
+        sync_stream();
+        A.E = h[3];
+        val.alloc(A.E); pos.alloc(A.E + 1); cnt.alloc(A.E + 1);
+        fin = cnt.ptr;
+        CUDA_TRY(cudaMemsetAsync(cnt.ptr + A.E, 0, sizeof(u32), stream()));
+        if (A.E) LAUNCH(k_ee_count, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, val.ptr, cnt.ptr);
+        if (mode == 1 && A.E) {
+            first.alloc(A.E + 1);
+            CUDA_TRY(cudaMemsetAsync(first.ptr + A.E, 0, sizeof(u32), stream()));
+            LAUNCH(k_ee_first, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, llen.ptr, cnt.ptr, first.ptr);
+            fin = first.ptr;
+        }
+        exclusive_scan_u32_to_u64(fin, pos.ptr, A.E + 1);
+    }
+    u64 bytes() const { return 16 * A.G + 12 * h[0] + 28 * h[1] + 4 * h[2]; }
+};
+
+u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
+                   u64 *bytes) {
+    const u32 nb = dir == 2 ? 2 : 1, grid = (u32)ctx().num_sms * 8;
+    EeBatch B(EArgs{d_src, nullptr, dt, n, n * nb * T * 2, 0, T, nb, dir});
+    B.prepare(0, grid);
+    p.alloc(n + 1);
+    LAUNCH(k_ee_rowptr, grid_for(n + 1, 256, grid), 256, 0, B.A, B.lstart.ptr, B.pos.ptr, p.ptr);
+    u64 total = 0;
+    d2h(&total, p.ptr + n, 1);
+    sync_stream();
+    node.alloc(total); edge.alloc(total);
+    if (total)
+        LAUNCH(k_ee_ref_fill, grid_for(B.A.E, 256, grid), 256, 0, B.A, B.lstart.ptr, B.lo.ptr, B.llen.ptr, B.val.ptr, B.fin, B.pos.ptr,
+               node.ptr, edge.ptr);
+    *bytes += B.bytes() + 12 * total;
+    return total;
+}
+
 void DevIdStore::upload(const u64 *hkey, const u64 *hptr, const u64 *hid, u64 nk) {
     clear();
     nkey = nk;
@@ -205,37 +290,18 @@ u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<Edg
         sync_stream();
         return 0;
     }
-    DevBuf<u64> lo(A.G), llen(A.G + 1), lstart(A.G + 1), stat(3);
-    stat.zero();
+    EeBatch B(A);
     // Compulsory bytes ("edge_expand"): 16 per list (its row pointers), 12 per forward entry (column + value), 28 per reverse
     // entry (column 4, plus its forward point lookup: row pointers 16, value 8), 4 per entry of the delta-minus rows searched,
     // and 14 per output entry (node 4, id 8, type 2), 15 with the direction.
     TimedScope ts(TK_EDGE_EXPAND, 0);
-    CUDA_TRY(cudaMemsetAsync(llen.ptr + A.G, 0, sizeof(u64), stream()));
-    LAUNCH(k_ee_lists, grid_for(A.G, 256, grid), 256, 0, A, lo.ptr, llen.ptr, stat.ptr);
-    exclusive_scan_u64(llen.ptr, lstart.ptr, A.G + 1);
-    u64 h[4];
-    d2h(h, stat.ptr, 3);
-    d2h(h + 3, lstart.ptr + A.G, 1);
-    sync_stream();
-    A.E = h[3];
-    DevBuf<u64> val(A.E), pos(A.E + 1);
-    DevBuf<u32> cnt(A.E + 1), first;
-    u32 *fin = cnt.ptr;
-    CUDA_TRY(cudaMemsetAsync(cnt.ptr + A.E, 0, sizeof(u32), stream()));
-    if (A.E) LAUNCH(k_ee_count, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, val.ptr, cnt.ptr);
-    if (mode == 1 && A.E) {
-        first.alloc(A.E + 1);
-        CUDA_TRY(cudaMemsetAsync(first.ptr + A.E, 0, sizeof(u32), stream()));
-        LAUNCH(k_ee_first, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, llen.ptr, cnt.ptr, first.ptr);
-        fin = first.ptr;
-    }
-    exclusive_scan_u32_to_u64(fin, pos.ptr, A.E + 1);
-    LAUNCH(k_ee_rowptr, grid_for(n + 1, 256, grid), 256, 0, A, lstart.ptr, pos.ptr, out.ptr);
+    B.prepare(mode, grid);
+    A = B.A;
+    LAUNCH(k_ee_rowptr, grid_for(n + 1, 256, grid), 256, 0, A, B.lstart.ptr, B.pos.ptr, out.ptr);
     d2h(out_p, out.ptr, n + 1);
     sync_stream();
     const u64 total = out_p[n];
-    ts.bytes = 16 * A.G + 12 * h[0] + 28 * h[1] + 4 * h[2] + (out_rev ? 15 : 14) * total;
+    ts.bytes = B.bytes() + (out_rev ? 15 : 14) * total;
     if (total > capacity || total == 0) return total;
     DevBuf<u32> dnode(total);
     DevBuf<u64> dedge(total);
@@ -243,8 +309,8 @@ u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<Edg
     DevBuf<uint8_t> drev;
     if (out_type) dtype.alloc(total);
     if (out_rev) drev.alloc(total);
-    LAUNCH(k_ee_fill, grid_for(A.E, 256, grid), 256, 0, A, lstart.ptr, lo.ptr, llen.ptr, val.ptr, fin, pos.ptr, dnode.ptr, dedge.ptr,
-           dtype.ptr, drev.ptr);
+    LAUNCH(k_ee_fill, grid_for(A.E, 256, grid), 256, 0, A, B.lstart.ptr, B.lo.ptr, B.llen.ptr, B.val.ptr, B.fin, B.pos.ptr, dnode.ptr,
+           dedge.ptr, dtype.ptr, drev.ptr);
     d2h(out_node, dnode.ptr, total);
     d2h(out_edge, dedge.ptr, total);
     if (out_type) d2h(out_type, dtype.ptr, total);

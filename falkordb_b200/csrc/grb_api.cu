@@ -2982,6 +2982,102 @@ GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, G
     });
 }
 
+// ---- CondVarLenTraverse's trails (cond_var_len_traverse.rs:152-386) for a batch of starts in one call: trails.cu.  The type
+// layers are read as B200_expand_edges reads them; the destination labels' (m, dp, dm) become one bitmap on the device.
+GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_Index nstarts, const B200_TensorLayers *types,
+                             int ntypes, int dir, uint64_t min_hops, uint64_t max_hops, const GrB_Matrix *lab_m,
+                             const GrB_Matrix *lab_dp, const GrB_Matrix *lab_dm, int nlabels, uint64_t tree_capacity,
+                             uint64_t *out_p, uint32_t *out_end, uint32_t *out_hops, uint64_t out_capacity,
+                             uint64_t *path_edge, uint32_t *path_node, uint64_t path_capacity, uint64_t *nout, uint64_t *npath) {
+    CHECK_PTR(types); CHECK_PTR(out_p); CHECK_PTR(nout); CHECK_PTR(npath);
+    if (nstarts) CHECK_PTR(starts);
+    if (out_end) CHECK_PTR(out_hops);
+    if (path_edge) CHECK_PTR(path_node);
+    if (ntypes < 1 || ntypes > 65536 || dir < B200_DIR_OUT || dir > B200_DIR_BOTH || nlabels < 0) {
+        tl_error = "var_len_trails: ntypes outside 1 .. 65536, dir out of range, or nlabels < 0"; return GrB_INVALID_VALUE;
+    }
+    if (nlabels) CHECK_PTR(lab_m);
+    for (int t = 0; t < ntypes; t++) {
+        const B200_TensorLayers &L = types[t];
+        CHECK_MAT(L.m);
+        for (GrB_Matrix X : {L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) if (X) CHECK_MAT(X);
+        if (dir != B200_DIR_OUT && !L.mt) { tl_error = "var_len_trails: incoming edges need the transpose mt"; return GrB_NULL_POINTER; }
+        if (L.m->type != T_UINT64 || (L.dp && L.dp->type != T_UINT64)) {
+            tl_error = "var_len_trails: the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
+        }
+    }
+    const u64 nv = types[0].m->nrows;
+    bool missing = false;
+    std::vector<GrB_Matrix> labs;                // (m, dp, dm) per present label
+    for (int k = 0; k < nlabels; k++) {
+        GrB_Matrix m = lab_m[k], dp = lab_dp ? lab_dp[k] : nullptr, dm = lab_dm ? lab_dm[k] : nullptr;
+        for (GrB_Matrix X : {m, dp, dm}) if (X) CHECK_MAT(X);
+        if (!m) { missing = true; continue; }
+        labs.insert(labs.end(), {m, dp, dm});
+    }
+    for (int t = 0; t < ntypes; t++) {
+        const B200_TensorLayers &L = types[t];
+        for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm})
+            if (X && (X->nrows != nv || X->ncols != nv)) {
+                tl_error = "var_len_trails: forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
+            }
+    }
+    for (GrB_Matrix X : labs)
+        if (X && (X->nrows != nv || X->ncols != nv)) {
+            tl_error = "var_len_trails: label layers must be n x n"; return GrB_DIMENSION_MISMATCH;
+        }
+    if (is_huge(types[0].m)) { tl_error = "var_len_trails: host-resident forward or transpose layers"; return GrB_NOT_IMPLEMENTED; }
+    for (GrB_Matrix X : labs)
+        if (is_huge(X)) { tl_error = "var_len_trails: host-resident label layers"; return GrB_NOT_IMPLEMENTED; }
+    for (u64 i = 0; i < nstarts; i++)
+        if (starts[i] >= nv || (dests && dests[i] >= 0 && (u64)dests[i] >= nv)) {
+            tl_error = "var_len_trails: start or destination out of range"; return GrB_INVALID_INDEX;
+        }
+    if (nstarts == 0 || min_hops > max_hops) {
+        for (u64 i = 0; i <= nstarts; i++) out_p[i] = 0;
+        *nout = 0; *npath = 0;
+        return GrB_SUCCESS;
+    }
+    GrB_Info info = device_ready();             // no device: fail before any host work
+    if (info) return info;
+    return guarded([&]() {
+        GpuLock g;
+        uvec<GrB_Matrix> all;
+        for (int t = 0; t < ntypes; t++) {
+            const B200_TensorLayers &L = types[t];
+            for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) all.push_back(X);
+        }
+        for (GrB_Matrix X : labs) all.push_back(X);
+        MultiLock lk(all.begin(), all.end());
+        ensure_init();
+        if (missing) {                           // a label the graph lacks: every trail is walked, none emits (:162, :316)
+            for (u64 i = 0; i <= nstarts; i++) out_p[i] = 0;
+            *nout = 0; *npath = 0;
+            return GrB_SUCCESS;
+        }
+        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
+        std::vector<EdgeTypeDev> td(ntypes);
+        for (int t = 0; t < ntypes; t++) {
+            const B200_TensorLayers &L = types[t];
+            const bool rev = dir != B200_DIR_OUT;
+            td[t] = EdgeTypeDev{dev(L.m), dev(L.dp), dev(L.dm), rev ? dev(L.mt) : nullptr, rev ? dev(L.mt_dp) : nullptr,
+                                rev ? dev(L.mt_dm) : nullptr, id_store(L.me), id_store(L.me_dp), id_store(L.me_dm)};
+        }
+        std::vector<LabelDev> ld;
+        for (size_t k = 0; k < labs.size(); k += 3) ld.push_back(LabelDev{dev(labs[k]), dev(labs[k + 1]), dev(labs[k + 2])});
+        TrailsOut o{out_p, out_end, out_hops, path_edge, path_node, out_capacity, path_capacity};
+        const int r = var_len_trails((const u64 *)starts, (const i64 *)dests, nstarts, td, dir, min_hops, max_hops, ld, nv, tree_capacity, o);
+        if (r == 2) {
+            *nout = *npath = UINT64_MAX;
+            tl_error = "var_len_trails: the stored trail tree would exceed tree_capacity entries";
+            return GrB_INSUFFICIENT_SPACE;
+        }
+        *nout = o.nout; *npath = o.npath;
+        if (r == 1) { tl_error = "var_len_trails: output capacity too small (*nout / *npath = what is needed)"; return GrB_INSUFFICIENT_SPACE; }
+        return GrB_SUCCESS;
+    });
+}
+
 // ---- the read phase of a Tensor's relationship inserts and deletes (set_all_from_slices / remove_all, tensor.rs:333-629) for a
 // whole batch in one call: writes.cu.  Only reads the layers; their pending tuples are finished like any device read's.
 static_assert(B200_PLAN_COMMITTED == WP_COMMITTED && B200_PLAN_CANCEL == WP_CANCEL && B200_PLAN_MT_BASE == WP_MT_BASE &&

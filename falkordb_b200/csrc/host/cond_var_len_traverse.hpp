@@ -13,6 +13,7 @@
 // min_hops <= 1) is the reach loop of grb.py: multi_source_reach / the frontier kernels, not this DFS.
 #pragma once
 #include "tensor.hpp"
+#include <functional>
 #include <unordered_map>
 
 namespace fdb {
@@ -41,7 +42,8 @@ inline std::vector<Edge> node_relationships(const Tensor &t, uint64_t node, Edge
     return out;
 }
 
-struct VarLenResult { uint64_t from, to; std::vector<uint64_t> edges; };   // edges: the trail, filled when emit_path is set
+// edges / nodes: the trail in walk order from the start (nodes includes the start), filled when emit_path is set; hops: its length
+struct VarLenResult { uint64_t from, to; std::vector<uint64_t> edges, nodes; uint64_t hops = 0; };
 
 // Adj: callable (node, EdgeDirection) -> std::vector<Edge>, the adjacency fetch (the only part that touches GraphBLAS)
 template <class Adj>
@@ -51,11 +53,23 @@ class VarLenIterT {
                 int64_t dest_id = -1, bool emit_path = false)
         : fetch_(adj), min_(min_hops), max_(max_hops), reversed_(reversed), bidir_(bidirectional), dest_(dest_id), emit_path_(emit_path) {}
 
+    // the destination labels (:555-563): a trail emits only at a node holding every label; a null entry is a label the graph
+    // lacks, and then nothing emits
+    void set_dest_labels(std::vector<const VersionedMatrix *> labels) {
+        set_dest_label_check([labels](uint64_t v) {
+            for (const VersionedMatrix *l : labels) if (!l || !l->get(v, v)) return false;   // node_has_label_id
+            return true;
+        });
+    }
+    void set_dest_label_check(std::function<bool(uint64_t)> f) { label_ok_ = std::move(f); }   // (the same over plain sets)
+    void set_dest(int64_t dest_id) { dest_ = dest_id; }
+
     void begin_start_node(uint64_t start) {                       // :152-183
         start_ = start;
         stack_.clear(); buf_.clear();
-        if (min_ == 0 && (dest_ < 0 || (uint64_t)dest_ == start)) buf_.push_back({start, start, {}});
-        stack_.push_back({start, {}, 0});
+        if (min_ == 0 && (dest_ < 0 || (uint64_t)dest_ == start) && has_labels(start))
+            buf_.push_back({start, start, {}, emit_path_ ? std::vector<uint64_t>{start} : std::vector<uint64_t>(), 0});
+        stack_.push_back({start, {}, emit_path_ ? std::vector<uint64_t>{start} : std::vector<uint64_t>(), 0});
     }
     bool next(VarLenResult &out) {                                // Iterator::next :388-
         while (true) {
@@ -66,7 +80,8 @@ class VarLenIterT {
     }
 
   private:
-    struct Frame { uint64_t node; std::vector<uint64_t> used; uint64_t depth; };
+    struct Frame { uint64_t node; std::vector<uint64_t> used, nodes; uint64_t depth; };
+    bool has_labels(uint64_t node) const { return !label_ok_ || label_ok_(node); }
     void advance() {                                              // :196-386
         const EdgeDirection dir = bidir_ ? EdgeDirection::Both : reversed_ ? EdgeDirection::Incoming : EdgeDirection::Outgoing;
         while (!stack_.empty()) {
@@ -88,14 +103,15 @@ class VarLenIterT {
             }
             for (auto &pr : scratch) {
                 const uint64_t dest = pr.second;
-                const bool will_emit = hop >= min_ && (dest_ < 0 || (uint64_t)dest_ == dest);
+                const bool will_emit = hop >= min_ && (dest_ < 0 || (uint64_t)dest_ == dest) && has_labels(dest);
                 const bool will_continue = hop < max_;
                 if (!will_emit && !will_continue) continue;
-                std::vector<uint64_t> used = f.used;
+                std::vector<uint64_t> used = f.used, nodes = f.nodes;
                 used.push_back(pr.first);
+                if (emit_path_) nodes.push_back(dest);
                 const uint64_t from = reversed_ ? dest : start_, to = reversed_ ? start_ : dest;
-                if (will_emit) buf_.push_back({from, to, emit_path_ ? used : std::vector<uint64_t>()});
-                if (will_continue) stack_.push_back({dest, std::move(used), hop});
+                if (will_emit) buf_.push_back({from, to, emit_path_ ? used : std::vector<uint64_t>(), nodes, hop});
+                if (will_continue) stack_.push_back({dest, std::move(used), std::move(nodes), hop});
             }
             if (!buf_.empty()) { std::reverse(buf_.begin(), buf_.end()); return; }   // pop() then yields adjacency order (:374-377)
         }
@@ -109,12 +125,25 @@ class VarLenIterT {
     std::vector<Frame> stack_;
     std::vector<VarLenResult> buf_;
     std::unordered_map<uint64_t, std::vector<Edge>> adj_;
+    std::function<bool(uint64_t)> label_ok_;
 };
 
 struct TensorAdjacency {
     const Tensor *t;
     std::vector<Edge> operator()(uint64_t node, EdgeDirection dir) const { return node_relationships(*t, node, dir); }
 };
+// Graph::get_node_relationships_by_type over several relationship types (graph.rs:1797-1835): each type's adjacency (One: a
+// callable as Adj above), types in the order given
+template <class One>
+struct TypesAdjacencyT {
+    std::vector<One> ts;
+    std::vector<Edge> operator()(uint64_t node, EdgeDirection dir) const {
+        std::vector<Edge> out;
+        for (const One &t : ts) { std::vector<Edge> e = t(node, dir); out.insert(out.end(), e.begin(), e.end()); }
+        return out;
+    }
+};
+typedef TypesAdjacencyT<TensorAdjacency> TypesAdjacency;
 struct VarLenIter : VarLenIterT<TensorAdjacency> {
     VarLenIter(const Tensor &t, uint64_t min_hops, uint64_t max_hops, bool reversed = false, bool bidirectional = false,
                int64_t dest_id = -1, bool emit_path = false)
@@ -151,6 +180,85 @@ inline Matrix<bool> var_len_reach(const std::vector<const Tensor *> &types, Edge
                                   max_hops > (uint64_t)INT64_MAX ? -1 : (int64_t)max_hops, min_hops == 0 ? 1 : 0, &levels),
            "B200_reach_batch_delta");
     return Matrix<bool>::adopt(raw, false);
+}
+
+// The trails of a batch of starts: start i's results are r[p[i] .. p[i+1]).
+struct VarLenBatch { std::vector<uint64_t> p{0}; std::vector<VarLenResult> r; };
+
+// The reference's route: one VarLenIterT over TypesAdjacency per start (dests empty or dests[i] < 0: no fixed destination; a
+// null label is one the graph lacks).
+inline VarLenBatch var_len_trails_dfs(const std::vector<const Tensor *> &types, EdgeDirection dir, const std::vector<uint64_t> &starts,
+                                      const std::vector<int64_t> &dests, uint64_t min_hops, uint64_t max_hops,
+                                      const std::vector<const VersionedMatrix *> &labels, bool emit_path) {
+    for (const Tensor *t : types) t->wait();
+    TypesAdjacency adj;
+    for (const Tensor *t : types) adj.ts.push_back(TensorAdjacency{t});
+    VarLenIterT<TypesAdjacency> it(adj, min_hops, max_hops, dir == EdgeDirection::Incoming, dir == EdgeDirection::Both,
+                                   -1, emit_path);
+    it.set_dest_labels(labels);
+    VarLenBatch b;
+    for (size_t i = 0; i < starts.size(); i++) {
+        it.set_dest(dests.empty() ? -1 : dests[i]);
+        it.begin_start_node(starts[i]);
+        VarLenResult r;
+        while (it.next(r)) b.r.push_back(std::move(r));
+        b.p.push_back(b.r.size());
+    }
+    return b;
+}
+
+// The device route: one B200_var_len_trails call over every type's live layers (as B200_expand_edges takes them) and the labels'
+// (m, dp, dm).  Counts first, then the entries into their exact size; (from, to) from the walk's end as :346-350 maps them.
+inline VarLenBatch var_len_trails(const std::vector<const Tensor *> &types, EdgeDirection dir, const std::vector<uint64_t> &starts,
+                                  const std::vector<int64_t> &dests, uint64_t min_hops, uint64_t max_hops,
+                                  const std::vector<const VersionedMatrix *> &labels, bool emit_path,
+                                  uint64_t tree_capacity = UINT64_MAX) {
+    std::vector<B200_TensorLayers> ls;
+    for (const Tensor *t : types) {
+        t->wait();
+        t->fwd_m().wait(); t->fwd_dp().wait(); t->fwd_dm().wait();
+        const VersionedMatrix &mt = t->matrix_t(), &me = t->edge_versioned();
+        mt.wait_all(); me.wait_all();
+        ls.push_back(B200_TensorLayers{t->fwd_m().inner(), t->fwd_dp().inner(), t->fwd_dm().inner(), mt.m().inner(), mt.dp().inner(),
+                                       mt.dm().inner(), me.m().inner(), me.dp().inner(), me.dm().inner()});
+    }
+    std::vector<GrB_Matrix> lm, ldp, ldm;
+    for (const VersionedMatrix *l : labels) {
+        if (l) { l->wait(); l->wait_all(); }
+        lm.push_back(l ? l->m().inner() : nullptr); ldp.push_back(l ? l->dp().inner() : nullptr); ldm.push_back(l ? l->dm().inner() : nullptr);
+    }
+    const int d = dir == EdgeDirection::Outgoing ? B200_DIR_OUT : dir == EdgeDirection::Incoming ? B200_DIR_IN : B200_DIR_BOTH;
+    const size_t n = starts.size();
+    VarLenBatch b;
+    b.p.assign(n + 1, 0);
+    uint64_t nout = 0, npath = 0;
+    auto call = [&](uint32_t *end, uint32_t *hops, uint64_t cap, uint64_t *pe, uint32_t *pn, uint64_t pcap) {
+        return B200_var_len_trails(starts.data(), dests.empty() ? nullptr : dests.data(), n, ls.data(), (int)ls.size(), d, min_hops,
+                                   max_hops, lm.data(), ldp.data(), ldm.data(), (int)lm.size(), tree_capacity, b.p.data(), end, hops,
+                                   cap, pe, pn, pcap, &nout, &npath);
+    };
+    grb_ok(call(nullptr, nullptr, 0, nullptr, nullptr, 0), "B200_var_len_trails");
+    std::vector<uint32_t> end(nout + 1), hops(nout + 1), pn(emit_path ? npath + nout + 1 : 0);
+    std::vector<uint64_t> pe(emit_path ? npath + 1 : 0);
+    grb_ok(call(end.data(), hops.data(), nout, emit_path ? pe.data() : nullptr, emit_path ? pn.data() : nullptr, npath),
+           "B200_var_len_trails");
+    uint64_t eb = 0;
+    size_t i = 0;
+    for (uint64_t k = 0; k < nout; k++) {
+        while (b.p[i + 1] <= k) i++;
+        VarLenResult r;
+        const bool rev = dir == EdgeDirection::Incoming;
+        r.from = rev ? end[k] : starts[i];
+        r.to = rev ? starts[i] : end[k];
+        r.hops = hops[k];
+        if (emit_path) {
+            r.edges.assign(pe.begin() + eb, pe.begin() + eb + hops[k]);
+            r.nodes.assign(pn.begin() + eb + k, pn.begin() + eb + k + hops[k] + 1);
+        }
+        eb += hops[k];
+        b.r.push_back(std::move(r));
+    }
+    return b;
 }
 
 } // namespace fdb

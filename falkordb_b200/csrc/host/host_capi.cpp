@@ -474,6 +474,82 @@ static void t_var_len_trails() {            // the same over a Tensor: adjacency
     vl_check([&](uint64_t lo, uint64_t hi, bool rev, bool bi, int64_t dest) { return VarLenIter(t, lo, hi, rev, bi, dest, true); });
 }
 
+// The same enumerator over several relationship types (TypesAdjacencyT, get_node_relationships_by_type's order) with destination
+// labels, against a brute-force enumeration of every trail over the union of the types' edges: parallel edges on one pair in two
+// types and inside one type, self-loops, a cycle, Out / In / Both, fixed destinations, and labels present, absent or missing.
+// Host only: the per-type adjacency is a plain edge list in tensor storage order.
+struct IdListAdjacency {        // one type: out by (dst, id), in by (src, id); under Both a self-loop only in the out half
+    std::vector<uint64_t> S, D, I;
+    std::vector<Edge> operator()(uint64_t node, EdgeDirection dir) const {
+        std::vector<Edge> out, in;
+        for (size_t e = 0; e < S.size(); e++) {
+            if (S[e] == node) out.push_back({S[e], D[e], I[e]});
+            if (D[e] == node && !(dir == EdgeDirection::Both && S[e] == node)) in.push_back({S[e], D[e], I[e]});
+        }
+        std::sort(out.begin(), out.end(), [](const Edge &a, const Edge &b) { return a.dst != b.dst ? a.dst < b.dst : a.id < b.id; });
+        std::sort(in.begin(), in.end(), [](const Edge &a, const Edge &b) { return a.src != b.src ? a.src < b.src : a.id < b.id; });
+        std::vector<Edge> r;
+        if (dir != EdgeDirection::Incoming) r = out;
+        if (dir != EdgeDirection::Outgoing) r.insert(r.end(), in.begin(), in.end());
+        return r;
+    }
+};
+static void t_var_len_types_labels_logic() {
+    const std::vector<IdListAdjacency> types = {
+        {{0, 0, 1, 2, 2, 3}, {1, 1, 2, 0, 3, 3}, {10, 11, 12, 13, 14, 15}},   // a multi-edge pair (0,1), a cycle, a self-loop at 3
+        {{0, 1, 3}, {1, 2, 0}, {20, 21, 22}},                                 // (0,1) and (1,2) again in a second type
+        {{1, 2}, {1, 4}, {30, 31}}};                                          // a self-loop at 1, a dead end at 4
+    std::vector<Edge> all;
+    for (const IdListAdjacency &t : types)
+        for (size_t e = 0; e < t.S.size(); e++) all.push_back({t.S[e], t.D[e], t.I[e]});
+    const std::set<uint64_t> L1{0, 1, 2, 3}, L2{1, 2, 3};
+    typedef std::tuple<uint64_t, uint64_t, std::vector<uint64_t>, std::vector<uint64_t>> Row;
+    for (int mode = 0; mode < 3; mode++)
+        for (int labs = 0; labs < 4; labs++)             // none, {L1}, {L1, L2}, {L1, missing}
+            for (uint64_t start : {0ull, 1ull, 2ull, 3ull, 4ull})
+                for (auto win : std::vector<std::pair<uint64_t, uint64_t>>{{0, 0}, {1, 1}, {0, 2}, {2, 4}, {1, 9}})
+                    for (int64_t dest : {(int64_t)-1, (int64_t)1, (int64_t)3}) {
+                        auto ok = [&](uint64_t v) { return labs == 0 || (L1.count(v) && (labs == 1 || (labs == 2 && L2.count(v)))); };
+                        std::multiset<Row> want, got;
+                        std::function<void(uint64_t, std::vector<uint64_t> &, std::vector<uint64_t> &)> go =
+                            [&](uint64_t cur, std::vector<uint64_t> &used, std::vector<uint64_t> &nodes) {
+                                const uint64_t depth = used.size();
+                                if (depth >= win.first && (dest < 0 || (uint64_t)dest == cur) && ok(cur))
+                                    want.insert(Row{mode == 1 ? cur : start, mode == 1 ? start : cur, used, nodes});
+                                if (depth == win.second) return;
+                                for (const Edge &e : all) {
+                                    if (std::find(used.begin(), used.end(), e.id) != used.end()) continue;
+                                    std::vector<uint64_t> nbs;
+                                    if (mode != 1 && e.src == cur) nbs.push_back(e.dst);
+                                    if (mode != 0 && e.dst == cur && !(mode == 2 && e.src == cur)) nbs.push_back(e.src);
+                                    for (uint64_t nb : nbs) {
+                                        used.push_back(e.id); nodes.push_back(nb);
+                                        go(nb, used, nodes);
+                                        used.pop_back(); nodes.pop_back();
+                                    }
+                                }
+                            };
+                        std::vector<uint64_t> used, nodes{start};
+                        go(start, used, nodes);
+                        VarLenIterT<TypesAdjacencyT<IdListAdjacency>> it(TypesAdjacencyT<IdListAdjacency>{types}, win.first, win.second,
+                                                                         mode == 1, mode == 2, dest, true);
+                        it.set_dest_label_check(ok);
+                        it.begin_start_node(start);
+                        VarLenResult r;
+                        while (it.next(r)) got.insert(Row{r.from, r.to, r.edges, r.nodes});
+                        REQUIRE(got == want, "trails over types differ: mode " << mode << " labels " << labs << " start " << start
+                                << " hops " << win.first << ".." << win.second << " dest " << dest << " (" << got.size() << " vs "
+                                << want.size() << ")");
+                    }
+    // the first frame of start 0, Out, *1..1: type order first (10, 11 in type 0, then 20 in type 1)
+    VarLenIterT<TypesAdjacencyT<IdListAdjacency>> it(TypesAdjacencyT<IdListAdjacency>{types}, 1, 1, false, false, -1, true);
+    it.begin_start_node(0);
+    std::vector<uint64_t> order;
+    VarLenResult r;
+    while (it.next(r)) order.push_back(r.edges[0]);
+    REQUIRE((order == std::vector<uint64_t>{10, 11, 20}), "emissions follow types in order, then neighbour and id");
+}
+
 // The reference's query-level goldens for variable-length traversals (tests/flow/test_variable_length_traversals.py), transcribed
 // at the level this mirror covers: which (from, to) pairs and path lengths the trail enumerator yields.  Host only.
 struct ListAdjacency {          // node_relationships over explicit edge lists (ids = positions): out by (dst, id), in by (src, id)
@@ -982,6 +1058,7 @@ static TestEntry TESTS[] = {
     {"repack_logic", t_repack_logic},
     {"var_len_trails", t_var_len_trails},
     {"var_len_trails_logic", t_var_len_trails_logic},
+    {"var_len_types_labels_logic", t_var_len_types_labels_logic},
     {"var_len_flow_goldens", t_var_len_flow_goldens},
     {"multiple_edges_flow", t_multiple_edges_flow},
     {"tensor_decodes_the_c_written_form", t_tensor_decodes_the_c_written_form},
@@ -1224,6 +1301,62 @@ int fdbh_expand_edges(void **tensors, uint64_t ntypes, const uint64_t *srcs, con
         out(out_p, r.p); out(out_node, r.node); out(out_edge, r.edge); out(out_type, r.type); out(out_rev, r.rev);
         return 0;
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
+// CondVarLenTraverse's trails over Tensor pointers (dir 0 out / 1 in / 2 both; dests NULL or < 0: none; labels: VersionedMatrix
+// pointers, NULL = a label the graph lacks).  fdbh_var_len_trails: B200_var_len_trails (var_len_trails); fdbh_var_len_trails_dfs:
+// the reference's DFS (var_len_trails_dfs).  Outputs (malloc'ed; free with fdbh_free): p[nstarts + 1]; per trail its end (the walk's
+// last node) and hop count; with emit_path the edges (npath) and nodes (npath + nout) in walk order, as B200_var_len_trails lays them.
+static int var_len_out(const VarLenBatch &b, EdgeDirection dir, uint64_t **out_p, uint64_t **out_end, uint64_t **out_hops,
+                       uint64_t **path_edge, uint64_t **path_node, uint64_t *nout, uint64_t *npath) {
+    std::vector<uint64_t> end, hops, pe, pn;
+    for (const VarLenResult &r : b.r) {
+        end.push_back(dir == EdgeDirection::Incoming ? r.from : r.to);
+        hops.push_back(r.hops);
+        pe.insert(pe.end(), r.edges.begin(), r.edges.end());
+        pn.insert(pn.end(), r.nodes.begin(), r.nodes.end());
+    }
+    *nout = end.size(); *npath = pe.size();
+    auto out = [](uint64_t **dst, const std::vector<uint64_t> &v) {
+        *dst = (uint64_t *)malloc(sizeof(uint64_t) * (v.size() + 1));
+        if (!*dst) throw std::bad_alloc();
+        memcpy(*dst, v.data(), sizeof(uint64_t) * v.size());
+    };
+    out(out_p, b.p); out(out_end, end); out(out_hops, hops); out(path_edge, pe); out(path_node, pn);
+    return 0;
+}
+static int var_len_c(bool dev, void **tensors, uint64_t ntypes, int dir, const uint64_t *starts, const int64_t *dests, uint64_t nstarts,
+                     uint64_t min_hops, uint64_t max_hops, void **labels, uint64_t nlabels, int emit_path, uint64_t tree_capacity,
+                     uint64_t **out_p, uint64_t **out_end, uint64_t **out_hops, uint64_t **path_edge, uint64_t **path_node,
+                     uint64_t *nout, uint64_t *npath) {
+    try {
+        std::vector<const Tensor *> types;
+        for (uint64_t k = 0; k < ntypes; k++) types.push_back((const Tensor *)tensors[k]);
+        std::vector<const VersionedMatrix *> labs;
+        for (uint64_t k = 0; k < nlabels; k++) labs.push_back((const VersionedMatrix *)labels[k]);
+        if (dir < 0 || dir > 2) throw std::invalid_argument("var_len_trails: dir must be 0, 1 or 2");
+        const EdgeDirection d = dir == 0 ? EdgeDirection::Outgoing : dir == 1 ? EdgeDirection::Incoming : EdgeDirection::Both;
+        std::vector<uint64_t> s(starts, starts + nstarts);
+        std::vector<int64_t> ds;
+        if (dests) ds.assign(dests, dests + nstarts);
+        VarLenBatch b = dev ? var_len_trails(types, d, s, ds, min_hops, max_hops, labs, emit_path != 0, tree_capacity)
+                            : var_len_trails_dfs(types, d, s, ds, min_hops, max_hops, labs, emit_path != 0);
+        return var_len_out(b, d, out_p, out_end, out_hops, path_edge, path_node, nout, npath);
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+int fdbh_var_len_trails(void **tensors, uint64_t ntypes, int dir, const uint64_t *starts, const int64_t *dests, uint64_t nstarts,
+                        uint64_t min_hops, uint64_t max_hops, void **labels, uint64_t nlabels, int emit_path, uint64_t tree_capacity,
+                        uint64_t **out_p, uint64_t **out_end, uint64_t **out_hops, uint64_t **path_edge, uint64_t **path_node,
+                        uint64_t *nout, uint64_t *npath) {
+    return var_len_c(true, tensors, ntypes, dir, starts, dests, nstarts, min_hops, max_hops, labels, nlabels, emit_path, tree_capacity,
+                     out_p, out_end, out_hops, path_edge, path_node, nout, npath);
+}
+int fdbh_var_len_trails_dfs(void **tensors, uint64_t ntypes, int dir, const uint64_t *starts, const int64_t *dests, uint64_t nstarts,
+                            uint64_t min_hops, uint64_t max_hops, void **labels, uint64_t nlabels, int emit_path, uint64_t **out_p,
+                            uint64_t **out_end, uint64_t **out_hops, uint64_t **path_edge, uint64_t **path_node, uint64_t *nout,
+                            uint64_t *npath) {
+    return var_len_c(false, tensors, ntypes, dir, starts, dests, nstarts, min_hops, max_hops, labels, nlabels, emit_path, UINT64_MAX,
+                     out_p, out_end, out_hops, path_edge, path_node, nout, npath);
 }
 
 // algo.BFS (algo_bfs.hpp).  adj: the adjacency VersionedMatrix; all_types / named: Tensor pointers (nnamed = 0: no type named);

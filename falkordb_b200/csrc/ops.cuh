@@ -151,6 +151,21 @@ struct WritePlan {
 void tensor_insert_plan(const EdgeTypeDev &t, const u64 *d_src, const u64 *d_dst, const u64 *d_id, u64 n, u64 nv, WritePlan &P);
 void tensor_remove_plan(const EdgeTypeDev &t, const u64 *d_id, const u64 *d_src, const u64 *d_dst, u64 n, u64 nv, WritePlan &P);
 
+// trails.cu : CondVarLenTraverse's trails for a batch of starts (B200_var_len_trails) over relationship tensors' live layers
+struct LabelDev { const DevCSR *m, *dp, *dm; };   // one destination label's layers (null or empty: absent)
+struct TrailsOut {
+    u64 *out_p;                                    // host, nstarts + 1
+    u32 *out_end, *out_hops;                       // host; out_end null: count only
+    u64 *path_edge; u32 *path_node;                // host; path_edge null: no paths
+    u64 out_capacity, path_capacity;
+    u64 nout = 0, npath = 0;
+};
+// nstarts >= 1, starts < nv and min_hops <= max_hops (checked by the caller); dir 0 out / 1 in / 2 both; h_dests null or < 0: no
+// fixed destination.  Returns 0 (done), 1 (the outputs do not fit: only out_p, nout and npath written) or 2 (the stored trail tree
+// would exceed tree_capacity entries: nothing written).
+int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const std::vector<EdgeTypeDev> &types, int dir, u64 min_hops,
+                   u64 max_hops, const std::vector<LabelDev> &labels, u64 nv, u64 tree_capacity, TrailsOut &o);
+
 // adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
 // replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
 // and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.

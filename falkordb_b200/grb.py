@@ -639,3 +639,50 @@ def remove_plan(t, ids, srcs, dsts):
     """B200_Tensor_remove_plan: the read phase of Tensor::remove_all's multi-edge path; the pair records (src, dst, val, flags) and
     the me entries, as insert_plan returns them."""
     return _plan(lib().B200_Tensor_remove_plan, t, ids, srcs, dsts)
+
+
+def var_len_trails(starts, types, dir=DIR_OUT, min_hops=1, max_hops=None, dests=None, labels=(), mode="paths", tree_capacity=None,
+                   capacity=None):
+    """B200_var_len_trails: CondVarLenTraverse's trails from each start over relationship types (`types` as expand_edges takes
+    them), in the reference's emission order.  max_hops None: unbounded.  dests: None or one int64 per start (< 0: none).  labels:
+    destination labels, each a (m, dp, dm) triple of layers (Matrix, raw handle or None) or None for a label the graph lacks.
+    mode "count": p only; "ends": p, end, hops; "paths": also the edges and nodes of every trail in walk order (trail k's edges are
+    edges[E_k : E_k + hops[k]], E_k = sum(hops[:k]), its nodes nodes[E_k + k : E_k + k + hops[k] + 1]).  Returns a dict of numpy
+    arrays.  Sized by a count call first unless `capacity` = (trails, path edges) is given."""
+    starts = _u64arr(starts)
+    n = len(starts)
+    ds = None if dests is None else np.ascontiguousarray(dests, dtype=np.int64)
+    assert ds is None or len(ds) == n, "one destination per start"
+    ls = (TensorLayers * max(1, len(types)))()
+    for k, t in enumerate(types):
+        vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
+        for name, x in zip(TENSOR_LAYERS, vals):
+            setattr(ls[k], name, _handle(x))
+    nl = len(labels)
+    lm, ldp, ldm = (P * max(1, nl))(), (P * max(1, nl))(), (P * max(1, nl))()
+    for k, lab in enumerate(labels):
+        if lab is not None:
+            lm[k], ldp[k], ldm[k] = (_handle(x) for x in (list(lab) + [None, None])[:3])
+    mx = (1 << 64) - 1 if max_hops is None else int(max_hops)
+    tc = (1 << 64) - 1 if tree_capacity is None else int(tree_capacity)
+    p, nv, npth = np.zeros(n + 1, np.uint64), U64(0), U64(0)
+
+    def call(end, hops, cap, pe, pn, pcap):
+        return lib().B200_var_len_trails(starts.ctypes.data if n else None, None if ds is None else ds.ctypes.data, n, ls, len(types),
+                                         dir, int(min_hops), mx, lm, ldp, ldm, nl, tc, p.ctypes.data, end, hops, cap, pe, pn, pcap,
+                                         C.byref(nv), C.byref(npth))
+    if mode == "count" or capacity is None:
+        check(call(None, None, 0, None, None, 0))
+        if mode == "count":
+            return {"p": p, "nout": nv.value, "npath": npth.value}
+        capacity = (nv.value, npth.value)
+    cap, pcap = int(capacity[0]), int(capacity[1])
+    end, hops = np.zeros(max(cap, 1), np.uint32), np.zeros(max(cap, 1), np.uint32)
+    paths = mode == "paths"
+    pe, pn = np.zeros(max(pcap, 1), np.uint64), np.zeros(max(pcap + cap, 1), np.uint32)
+    check(call(end.ctypes.data, hops.ctypes.data, cap, pe.ctypes.data if paths else None, pn.ctypes.data if paths else None, pcap))
+    m, q = nv.value, npth.value
+    out = {"p": p, "end": end[:m], "hops": hops[:m], "nout": m, "npath": q}
+    if paths:
+        out["edges"], out["nodes"] = pe[:q], pn[:q + m]
+    return out

@@ -1,7 +1,8 @@
 """ctypes binding of libfdbhost.so, the C++ host mirror of the reference's Tensor and CondTraverse (csrc/host): a relationship
 Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending (through the reference's read phase
 or the device plans, B200_Tensor_insert_plan / B200_Tensor_remove_plan), and the routes that read its
-relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), and the algo.BFS, algo.pageRank, algo.WCC
+relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), CondVarLenTraverse's trails
+(B200_var_len_trails, or the reference's DFS), and the algo.BFS, algo.pageRank, algo.WCC
 and algo.labelPropagation procedures over them."""
 import ctypes as C
 import os
@@ -45,6 +46,9 @@ def host():
     L.fdbh_vm_state.argtypes = [P, P, P]
     L.fdbh_run_write_test.argtypes = [C.c_char_p, C.c_int]
     L.fdbh_expand_edges.argtypes = [P, U64, P, P, U64, C.c_int, C.c_int, C.c_int] + [P] * 5 + [C.POINTER(U64)]
+    vl = [P, U64, C.c_int, P, P, U64, U64, U64, P, U64, C.c_int]
+    L.fdbh_var_len_trails.argtypes = vl + [U64] + [P] * 5 + [C.POINTER(U64)] * 2
+    L.fdbh_var_len_trails_dfs.argtypes = vl + [P] * 5 + [C.POINTER(U64)] * 2
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
     algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
     L.fdbh_algo_pagerank.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
@@ -167,6 +171,36 @@ def expand_edges(tensors, sources, dir, mode, targets=None, route=ROUTE_BY_GET):
         out.append(np.frombuffer((C.c_char * nbytes).from_address(x.value), dt).copy() if k else np.zeros(0, dt))
         L.fdbh_free(x)
     return tuple(out)
+
+
+def var_len_trails(tensors, starts, dir, min_hops=1, max_hops=None, dests=None, labels=(), emit_path=True, route=ROUTE_DEVICE,
+                   tree_capacity=None):
+    """CondVarLenTraverse's trails over Tensor objects: route ROUTE_DEVICE (fdbh_var_len_trails, one B200_var_len_trails call) or
+    ROUTE_BY_GET (fdbh_var_len_trails_dfs, the reference's DFS over TypesAdjacency).  labels: VersionedMatrix objects, None for a
+    label the graph lacks.  Returns a dict of numpy uint64 arrays: p, end, hops, and with emit_path edges and nodes in walk order."""
+    L = host()
+    (src,) = _u64(starts)
+    ds = None if dests is None else np.ascontiguousarray(dests, dtype=np.int64)
+    ts = (C.c_void_p * max(1, len(tensors)))(*[t.h for t in tensors])
+    lb = (C.c_void_p * max(1, len(labels)))(*[None if x is None else x.h for x in labels])
+    mx = (1 << 64) - 1 if max_hops is None else int(max_hops)
+    ptrs = [C.c_void_p() for _ in range(5)]
+    nv, npth = U64(0), U64(0)
+    args = [ts, len(tensors), dir, src.ctypes.data, None if ds is None else ds.ctypes.data, len(src), int(min_hops), mx, lb, len(labels),
+            1 if emit_path else 0]
+    if route == ROUTE_DEVICE:
+        rc = L.fdbh_var_len_trails(*args, (1 << 64) - 1 if tree_capacity is None else int(tree_capacity), *[C.byref(x) for x in ptrs],
+                                   C.byref(nv), C.byref(npth))
+    else:
+        rc = L.fdbh_var_len_trails_dfs(*args, *[C.byref(x) for x in ptrs], C.byref(nv), C.byref(npth))
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    m, q = nv.value, npth.value
+    out = {}
+    for name, x, k in zip(("p", "end", "hops", "edges", "nodes"), ptrs, (len(src) + 1, m, m, q, q + m if emit_path else 0)):
+        out[name] = np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64).copy() if k else np.zeros(0, np.uint64)
+        L.fdbh_free(x)
+    return out
 
 
 class VersionedMatrix:

@@ -409,6 +409,33 @@ typedef struct {
 GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, GrB_Index n, const B200_TensorLayers *types,
                            int ntypes, int dir, int mode, uint64_t *out_p, uint32_t *out_node, uint64_t *out_edge,
                            uint16_t *out_type, uint8_t *out_rev, uint64_t out_capacity, uint64_t *nout);
+/* CondVarLenTraverse's trails (cond_var_len_traverse.rs:152-386) from each starts[i], over ntypes tensors' live layers: every
+ * relationship-unique path of min_hops .. max_hops edges, in the reference's emission order.  Adjacency per node is
+ * Graph::get_node_relationships_by_type's (graph.rs:1797-1835): types in order; per type the outgoing half (neighbour ascending,
+ * ids ascending), then the incoming half (source ascending); under Both a self-loop once, in the outgoing half.  Per start: the
+ * 0-hop emission (min_hops == 0), then per frame its emitting edges in adjacency order, then the frames of its continuing edges in
+ * reverse adjacency order (a DFS stack).  Starts come out in input order.
+ * dir: B200_DIR_OUT (forward), B200_DIR_IN (reversed), B200_DIR_BOTH (bidirectional; the reference never combines it with
+ * reversed, :534).  max_hops = UINT64_MAX: unbounded.  dests NULL or dests[i] < 0: no fixed destination.  Destination labels:
+ * nlabels triples (lab_m, lab_dp, lab_dm), the label's diagonal being (m \ dm) u dp; a NULL lab_m is a label the graph lacks:
+ * nothing emits.  lab_dp / lab_dm may be NULL arrays or hold NULL entries.
+ * out_p[nstarts + 1] is always written (but see tree_capacity): trails of start i are out_p[i] .. out_p[i+1], in the reference's
+ * emission order.  out_end (the node the walk ends at) and out_hops; out_end NULL: count only.  With path_edge / path_node the
+ * trail itself in walk order from the start: trail k's edges are path_edge[E_k .. E_k + h_k), E_k = sum_{j<k} h_j, and its nodes
+ * are path_node[E_k + k .. E_k + k + h_k] (path_node holds *npath + *nout entries).
+ * Entries are written only when they fit: out_capacity trails and path_capacity edges.  Otherwise GrB_INSUFFICIENT_SPACE, with
+ * *nout / *npath = what is needed.
+ * If the stored trail tree (every trail shorter than max_hops) would exceed tree_capacity entries: GrB_INSUFFICIENT_SPACE with
+ * *nout = *npath = UINT64_MAX, nothing written.
+ * Errors follow B200_expand_edges (types' layers, ntypes, dir); nlabels < 0 GrB_INVALID_VALUE; a start or destination >= n
+ * GrB_INVALID_INDEX; label layers not n x n GrB_DIMENSION_MISMATCH, host-resident GrB_NOT_IMPLEMENTED; out_end without out_hops, or
+ * path_edge without path_node, GrB_NULL_POINTER.  nstarts == 0 or min_hops > max_hops: success with no device work.  No layer
+ * changes, apart from finishing pending tuples; no base is downloaded. */
+GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_Index nstarts, const B200_TensorLayers *types,
+                             int ntypes, int dir, uint64_t min_hops, uint64_t max_hops, const GrB_Matrix *lab_m,
+                             const GrB_Matrix *lab_dp, const GrB_Matrix *lab_dm, int nlabels, uint64_t tree_capacity,
+                             uint64_t *out_p, uint32_t *out_end, uint32_t *out_hops, uint64_t out_capacity,
+                             uint64_t *path_edge, uint32_t *path_node, uint64_t path_capacity, uint64_t *nout, uint64_t *npath);
 /* Flags of the write plans below. */
 #define B200_PLAN_COMMITTED 0x01 /* insert: m holds the pair, its value is to be reconciled (dm.erase) */
 #define B200_PLAN_CANCEL 0x02    /* insert: COMMITTED and m's value equals the new inline value (dp.erase instead of dp.insert) */
@@ -454,7 +481,8 @@ void B200_reset_stats(void);
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
  * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", the accumulating
  * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", B200_bfs_delta's kernels over
- * dirty operands, "bfs_delta", and B200_adjacency_delta's induced-layer kernels, "adj_build".  0 on success. */
+ * dirty operands, "bfs_delta", B200_adjacency_delta's induced-layer kernels, "adj_build", and B200_var_len_trails' kernels,
+ * "var_len_trails".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */

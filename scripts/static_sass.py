@@ -43,6 +43,11 @@ WANT = [
     ("remove plan, count", r"k_rm_count"),
     ("remove plan, fill", r"k_rm_fill"),
     ("write plans, run heads", r"k_wp_heads"),
+    ("relationship ids, reference order fill", r"k_ee_ref_fill"),
+    ("trails, candidates", r"k_tr_cand"),
+    ("trails, stored level fill", r"k_tr_fill"),
+    ("trails, last-level emissions", r"k_tr_out_last"),
+    ("trails, stored-level emissions", r"k_tr_out("),
 ]
 OPS = [("LDG.*\\.256", r"\bLDG\.[A-Z0-9_.]*256"), ("LDG.*\\.128", r"\bLDG\.[A-Z0-9_.]*128"), ("LDG.*\\.64", r"\bLDG\.[A-Z0-9_.]*\.64\b"),
        ("LDG other", r"\bLDG\."), ("STG.*\\.256", r"\bSTG\.[A-Z0-9_.]*256"), ("STG.*\\.128", r"\bSTG\.[A-Z0-9_.]*128"), ("STG other", r"\bSTG\."),
