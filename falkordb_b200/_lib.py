@@ -84,7 +84,7 @@ def lib():
         "B200_Matrix_export_bitmap": [P, P, U64, C.POINTER(U64), C.c_int],
         "B200_Matrix_export_bitmap_async": [P, P, U64, C.POINTER(P)], "B200_Ticket_wait": [C.POINTER(P)],
         "B200_Matrix_device_view": [P, C.POINTER(P), C.POINTER(P), C.POINTER(P)],
-        "B200_Matrix_digest": [P, P], "B200_Matrix_prepare": [P, C.c_int], "B200_Matrix_rmat": [C.POINTER(P), C.c_int, U64, U64], "B200_sync": [], "B200_pool_trim": [],
+        "B200_Matrix_digest": [P, P], "B200_Matrix_prepare": [P, C.c_int], "B200_Matrix_push_operand": [P, P, P, P], "B200_Matrix_rmat": [C.POINTER(P), C.c_int, U64, U64], "B200_sync": [], "B200_pool_trim": [],
         "B200_traverse_batch": [P, U64, P, C.c_int, C.c_int, P, U64, P, P, U64, C.POINTER(U64), C.POINTER(U64), C.POINTER(C.c_int)],
         "B200_traverse_batch_delta": [P, U64, P, P, P, C.c_int, C.c_int, P, U64, P, P, U64, C.POINTER(U64), C.POINTER(U64),
                                       C.POINTER(C.c_int)],

@@ -579,14 +579,15 @@ __global__ void k_csr_entry_info(const u64 *__restrict__ Fp, const u32 *__restri
     for (int o = 16; o > 0; o >>= 1) ed += __shfl_xor_sync(0xffffffffu, ed, o);
     if (lane == 0 && ed) atomicAdd((unsigned long long *)edges, ed);
 }
-// ANDNOT (the dirty hop's deleted-edge term, bits_apply_deltas) clears bit i instead of setting it
-template <int W, bool ANDNOT>
+// ANDNOT (the dirty hop's deleted-edge term, bits_apply_deltas) clears bit i instead of setting it.  SLICED (csr_push_sliced): the
+// entries are sub-entries, Ap[e] is where sub-entry e starts in Aj, Fj is not read, and a CTA takes CHUNK flops.
+template <int W, bool ANDNOT, bool SLICED = false, u64 CHUNK = PUSH_CHUNK>
 __global__ void __launch_bounds__(256)
 k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *__restrict__ cum, u64 nent, u64 total,
            const u64 *__restrict__ Ap, const u32 *__restrict__ Aj, u64 *__restrict__ Y, const u32 *__restrict__ perm) {
     __shared__ u64 s_e0, s_e1;
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    u64 lo = (u64)blockIdx.x * PUSH_CHUNK, hi = lo + PUSH_CHUNK;
+    u64 lo = (u64)blockIdx.x * CHUNK, hi = lo + CHUNK;
     if (hi > total) hi = total;
     if (tid == 0) {
         s_e0 = find_le64(cum, 0, nent - 1, lo);
@@ -600,7 +601,7 @@ k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *
         if (t < hi) {
             while (e < e1 && cum[e + 1] <= t) e++;
             const u32 i = erow[e];
-            u32 col = Aj[Ap[Fj[e]] + (t - cum[e])];
+            u32 col = Aj[(SLICED ? Ap[e] : Ap[Fj[e]]) + (t - cum[e])];
             // hot-set order through the table (the deltas, which have no relabelled copy); a prepared operand passes its
             // relabelled col_idx (PullTables::ap) as Aj instead, with perm null
             if (perm) col = __ldg(perm + col);
@@ -618,6 +619,72 @@ static void csr_push_impl(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBi
     TimedScope ts(acc ? TK_BITS_PUSH_ACC : TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops);
     LAUNCH((k_csr_push<W, false>), (u32)nchunks, 256, 0, erow, F.j.ptr, cum, F.nnz, flops, A.p.ptr, Aj, Y.w.ptr, perm);
 }
+// The same REDs in destination order.  Y is n * W words, many times the L2 on a large graph, and a RED to a record that is not
+// resident reads its sector from HBM and writes it back on eviction.  With every row of Aj ascending by position
+// (PullTables::ap_sorted), positions [0, n) are cut into P slices of S, and entry (i, k) of F into one sub-entry per slice: the
+// part of row k whose positions fall in it, found with one lower bound per (entry, slice boundary).  The non-empty sub-entries
+// are listed slice-major -- all of slice 0, then slice 1, ... -- as (row i, first position in Aj, length), and k_csr_push chunks
+// the prefix sums of their lengths as it chunks the entries': the flops and the load balance are unchanged, only their order.
+// The chunk is SLICE_CHUNK flops, so that the CTAs resident at one time span few slices.
+static const u64 SLICE_CHUNK = 512, SLICE_MAX_SUB = (u64)1 << 24, SLICE_MIN_CAP = (u64)1 << 22;
+__global__ void k_slice_bounds(const u32 *__restrict__ Fj, u64 nent, const u64 *__restrict__ Ap, const u32 *__restrict__ Aj, u32 P,
+                               u64 S, u32 *__restrict__ bnd) {
+    const u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nent * (P + 1)) return;
+    const u64 e = q / (P + 1), p = q - e * (P + 1);
+    const u32 k = Fj[e];
+    const u32 *row = Aj + Ap[k];
+    u32 lo = 0, hi = (u32)(Ap[k + 1] - Ap[k]);       // the first entry of row k at position >= p * S
+    if (p == 0) hi = 0;
+    else if (p == P) lo = hi;
+    while (lo < hi) {
+        const u32 mid = lo + ((hi - lo) >> 1);
+        if ((u64)row[mid] < p * S) lo = mid + 1; else hi = mid;
+    }
+    bnd[q] = lo;
+}
+// flag[p * nent + e] = sub-entry (e, p) is not empty: slice-major, the order the scan numbers them in
+__global__ void k_slice_flags(const u32 *__restrict__ bnd, u64 nent, u32 P, u32 *__restrict__ flag) {
+    const u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nent * P) return;
+    const u64 p = q / nent, e = q - p * nent;
+    flag[q] = bnd[e * (P + 1) + p + 1] > bnd[e * (P + 1) + p];
+}
+__global__ void k_slice_emit(const u32 *__restrict__ bnd, const u32 *__restrict__ flag, const u64 *__restrict__ pos, u64 nent, u32 P,
+                             const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *__restrict__ Ap,
+                             u32 *__restrict__ srow, u64 *__restrict__ sstart, u64 *__restrict__ slen) {
+    const u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nent * P || !flag[q]) return;
+    const u64 p = q / nent, e = q - p * nent, o = pos[q];
+    const u32 b0 = bnd[e * (P + 1) + p];
+    srow[o] = erow[e];
+    sstart[o] = Ap[Fj[e]] + b0;
+    slen[o] = bnd[e * (P + 1) + p + 1] - b0;
+}
+template <int W>
+static void csr_push_sliced(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBits &Y, u64 flops, const u32 *erow, u32 P, u64 S) {
+    const u64 nent = F.nnz, nsub = nent * P;
+    // the sub-entry table costs 12 bytes per (entry, boundary) and 20 per non-empty sub-entry, counted at their upper bound
+    TimedScope ts(TK_BITS_PUSH, 4 * flops + 16 * F.nnz + 8 * flops + 32 * nsub);
+    // One workspace for the six arrays, its capacity a power of two of at least SLICE_MIN_CAP sub-entries: nnz(F) drifts from
+    // batch to batch, and a request of a new size class is a cudaMalloc, which costs as much as the push saves, inside the hop.
+    u64 cap = SLICE_MIN_CAP;
+    while (cap < nsub + nent + 1) cap <<= 1;
+    DevBuf<u64> ws(cap * 3 + (cap * 3 + 1) / 2);
+    u64 *pos = ws.ptr, *sstart = pos + cap, *scum = sstart + cap;
+    u32 *bnd = (u32 *)(scum + cap), *flag = bnd + cap, *srow = flag + cap;
+    LAUNCH(k_slice_bounds, grid_for(nent * (P + 1), 256), 256, 0, F.j.ptr, nent, A.p.ptr, Aj, P, S, bnd);
+    LAUNCH(k_slice_flags, grid_for(nsub, 256), 256, 0, bnd, nent, P, flag);
+    CUDA_TRY(cudaMemsetAsync(flag + nsub, 0, sizeof(u32), stream()));
+    exclusive_scan_u32_to_u64(flag, pos, nsub + 1);
+    // the slots past the last non-empty sub-entry stay empty: their cum is flops
+    CUDA_TRY(cudaMemsetAsync(scum, 0, (nsub + 1) * sizeof(u64), stream()));
+    LAUNCH(k_slice_emit, grid_for(nsub, 256), 256, 0, bnd, flag, pos, nent, P, erow, F.j.ptr, A.p.ptr, srow, sstart, scum);
+    exclusive_scan_u64(scum, scum, nsub + 1);
+    const u64 nchunks = (flops + SLICE_CHUNK - 1) / SLICE_CHUNK;
+    LAUNCH((k_csr_push<W, false, true, SLICE_CHUNK>), (u32)nchunks, 256, 0, srow, (const u32 *)nullptr, scum, nsub, flops, sstart, Aj,
+           Y.w.ptr, (const u32 *)nullptr);
+}
 // Whether the push straight from F's CSR entries beats the bit-matrix hop.  edges = the out-degrees summed over the DISTINCT
 // columns of F (what the bit-matrix hop walks), flops = over all its entries (one RED each for the CSR push).
 //  * edges * 4 > nnz(A): no -- the bit-matrix hop pulls these frontiers.
@@ -631,6 +698,8 @@ static void csr_push_impl(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBi
 //  * flops * 4 <= nnz(A) is always taken (it implies the edges bound), as before the bound existed: at W >= 8 that region lies
 //    inside the bound; at W = 1 (64 rows: crossover 1.7 to 1.9 * n * W at 15 and 30 M edges, below 2.5 at 60 M) it keeps some
 //    frontiers that the bit-matrix hop would take up to 0.4 ms faster.
+//  * the sliced push (csr_push_sliced) moved the W = 8 crossover to about 1.0 * n * W where it applies (H100 80GB HBM3, 700 W
+//    limit; DESIGN.md 4.8); W = 16 was not re-measured, so the bound stays where no frontier is slower than before it.
 static bool csr_push_wins(u64 flops, u64 edges, u64 n, u32 W, u64 nnzA) {
     if (flops * 4 <= nnzA) return true;
     return edges * 4 <= nnzA && (flops - edges) * 2 <= n * W;
@@ -667,14 +736,33 @@ bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops
     // a square operand with pull tables: write the result in its hot-set order, the form the next pull gathers from directly --
     // through the operand's relabelled col_idx when the tables have it, else through pperm per flop
     const u32 *perm = nullptr, *Aj = A.j.ptr;
+    u32 P = 0;                                   // destination slices of the sliced push (0: entry order)
+    u64 S = 0;
     if (!acc && pt && ctx().opt_perm_push && pt->perm_tag && pt->pperm && A.nrows == A.ncols && pt->pperm->n == A.ncols) {
         if (pt->ap.ptr && pt->ap.n == A.nnz) Aj = pt->ap.ptr;
         else perm = pt->pperm->ptr;
+        // slices of a quarter of the L2, so that the slices the resident CTAs span stay in it together
+        const i64 ps = ctx().opt_push_slices;
+        if (!perm && pt->ap_sorted && ps != 0 && A.ncols) {
+            S = ps > 0 ? (A.ncols + (u64)ps - 1) / (u64)ps : std::max<u64>(1, ctx().l2_bytes / 4 / (8ULL * W));
+            const u64 np = (A.ncols + S - 1) / S;
+            if ((ps > 0 || np > 1) && np * F.nnz <= SLICE_MAX_SUB) P = (u32)np;
+        }
         Y.pvert = pt->pvert;
         Y.pperm = pt->pperm;
         Y.perm_tag = pt->perm_tag;
     }
     if (flops == 0) return true;
+    if (P) {
+        switch (W) {
+        case 1: csr_push_sliced<1>(F, A, Aj, Y, flops, erow.ptr, P, S); break;
+        case 2: csr_push_sliced<2>(F, A, Aj, Y, flops, erow.ptr, P, S); break;
+        case 4: csr_push_sliced<4>(F, A, Aj, Y, flops, erow.ptr, P, S); break;
+        case 8: csr_push_sliced<8>(F, A, Aj, Y, flops, erow.ptr, P, S); break;
+        default: csr_push_sliced<16>(F, A, Aj, Y, flops, erow.ptr, P, S); break;
+        }
+        return true;
+    }
     switch (W) {
     case 1: csr_push_impl<1>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
     case 2: csr_push_impl<2>(F, A, Aj, Y, flops, erow.ptr, cum.ptr, perm, acc); break;
@@ -1130,7 +1218,7 @@ k_ordered_flops(const u32 *__restrict__ hdeg, u64 n1, const u64 *__restrict__ Xp
 
 static void build_hot_pack(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     u64 n = A.nrows;
-    pt.vert.release(); pt.jp.release(); pt.ap.release(); pt.slot.release(); pt.hdeg.release(); pt.n1 = 0; pt.packed = false;
+    pt.vert.release(); pt.jp.release(); pt.ap.release(); pt.ap_sorted = false; pt.slot.release(); pt.hdeg.release(); pt.n1 = 0; pt.packed = false;
     if (n == 0 || AT.nnz == 0 || n >= 0xFFFFFFFFULL) return;
     DevBuf<u64> keys(n), cnt(1);
     cnt.zero();
@@ -1166,6 +1254,12 @@ static void build_pull_tables(const DevCSR &A, const DevCSR &AT, PullTables &pt)
     if (pt.packed && !pt.ap.ptr && ctx().opt_perm_push && A.nnz && A.nrows == A.ncols) {
         pt.ap.alloc(A.nnz);
         LAUNCH(k_relabel_cols, grid_for(A.nnz, 256, (u64)ctx().num_sms * 32), 256, 0, A.j.ptr, A.nnz, pt.pperm->ptr, pt.ap.ptr);
+    }
+    // its rows ascending by position, for the sliced push (csr_push_sliced): OR commutes and only the CSR push reads ap, so the
+    // order inside a row changes no result.  Like ap itself, added at the next build when push_slices was off at the first
+    if (pt.ap.ptr && !pt.ap_sorted && ctx().opt_push_slices != 0 && A.nnz <= 0x7fffffffULL) {
+        sort_rows_u32(A.p.ptr, A.nrows, pt.ap.ptr, A.nnz);
+        pt.ap_sorted = true;
     }
     if (!pt.built) {
         build_seg_list(AT, pt);

@@ -39,6 +39,7 @@ struct Context {
     bool ready = false;
     int device = 0;
     int num_sms = 132;                // read from the device at bring-up (prims.cu)
+    u64 l2_bytes = 50ULL << 20;       // likewise: the L2 cache the sliced CSR push sizes its destination slices by
     cudaStream_t stream = nullptr;
     std::atomic<u64> launches{0};     // kernels of THIS library launched (bench.py gpu_launches)
     std::atomic<u64> lib_launches{0}; // CUB primitives launched on our behalf (sort / scan)
@@ -62,6 +63,7 @@ struct Context {
     i64 opt_hot_pack = 1;          // gather through the degree-sorted, sink-free relabelling of the frontier
     i64 opt_fused_prep = 1;        // pull hops: pack the frontier, count flops / edges and OR it in one pass
     i64 opt_csr_push = 1;          // small CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes); 2 = whatever their size (measurement)
+    i64 opt_push_slices = -1;      // the CSR push through a prepared operand issues its REDs in L2-sized destination slices: -1 = slices sized from the L2, 0 = off (entry order), k > 0 = k slices (measurement and tests)
     i64 opt_diag_filter = 1;       // frontier-form mxm by a diagonal (label) matrix runs as an elementwise column filter
     i64 opt_pull_grid = 0;         // CTAs per SM of the segment pull kernel (0 = occupancy: one resident wave)
     i64 opt_union_accum = 1;       // union hops: clean extra operands OR into one product (0 = a product per operand plus an OR pass; measurement)
@@ -243,5 +245,6 @@ void exclusive_scan_u32_to_u64(const u32 *in, u64 *out, size_t n);
 void sort_keys_u64(u64 *keys_in_out, size_t n, int end_bit);            // ascending, in place (uses temp)
 void sort_pairs_u64(u64 *keys_in_out, u64 *vals_in_out, size_t n, int end_bit); // stable
 u64 reduce_sum_u64(const u64 *in, size_t n);
+void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz);  // every CSR row's entries ascending, in place (uses temp)
 
 } // namespace b200

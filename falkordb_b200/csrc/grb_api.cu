@@ -2139,6 +2139,21 @@ GrB_Info B200_Matrix_prepare(GrB_Matrix A, int want_transpose) {
     });
 }
 
+GrB_Info B200_Matrix_push_operand(GrB_Matrix A, uint32_t *ap_out, uint32_t *pperm_out, int *sorted) {
+    CHECK_MAT(A);
+    CHECK_PTR(sorted);
+    return guarded([&]() {
+        GpuLock g;
+        MultiLock lk{A};
+        if (!A->devT_valid || !A->pt.ap.ptr || !A->pt.pperm) throw GrbError(GrB_INVALID_VALUE, "push_operand: the matrix has no relabelled col_idx (not prepared, or not square)");
+        if (ap_out) d2h(ap_out, A->pt.ap.ptr, A->pt.ap.n);
+        if (pperm_out) d2h(pperm_out, A->pt.pperm->ptr, A->pt.pperm->n);
+        sync_stream();
+        *sorted = A->pt.ap_sorted ? 1 : 0;
+        return GrB_SUCCESS;
+    });
+}
+
 GrB_Info B200_Matrix_rmat(GrB_Matrix *A, int scale, uint64_t edge_factor, uint64_t seed) {
     CHECK_PTR(A);
     return guarded([&]() {
@@ -3175,6 +3190,7 @@ uint64_t B200_get_stat(const char *name) {
     if (n == "h2d_bytes") return c.h2d_bytes.load();
     if (n == "d2h_bytes") return c.d2h_bytes.load();
     if (n == "num_sms") return (uint64_t)c.num_sms;
+    if (n == "l2_bytes") return (uint64_t)c.l2_bytes;
     if (n == "host_bytes") return g_host_bytes.load();     // live bytes obtained through the GxB_init allocator hooks
     if (n == "host_allocs") return g_host_allocs.load();
     return ~0ULL;
@@ -3214,6 +3230,7 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "csr_push") c.opt_csr_push = value;
     else if (n == "fused_prep") c.opt_fused_prep = value;
     else if (n == "perm_push") c.opt_perm_push = value;
+    else if (n == "push_slices") c.opt_push_slices = value;
     else if (n == "union_accum") c.opt_union_accum = value;
     // retired: the pull, the count pass and the fill have a single kernel each now, and there is no persisting-L2 window; the
     // names stay accepted so callers that set them keep working

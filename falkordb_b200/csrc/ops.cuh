@@ -41,13 +41,14 @@ struct PullTables {   // per-matrix tables of the pull direction, cached with th
     std::shared_ptr<DevBuf<u32>> pvert, pperm; u64 perm_tag = 0;    // pvert[position] = vertex, pperm[vertex] = position
     DevBuf<u32> jp;                                    // col_idx of A' relabelled to hot-set slots (when packed)
     DevBuf<u32> ap;                                    // col_idx of A relabelled to positions (pperm[A.j], when packed): the CSR push's operand
+    bool ap_sorted = false;                            // every row of ap ascending by position: the push may cut it into destination slices
     // segment list: rows of A' longer than SMALL_ROW -- whole rows up to LONG_ROW entries, LONG_ROW-entry segments of longer ones --
     // longest first; bit 31 of s_len marks a segment of a long row (merged with RED.OR)
     DevBuf<u32> s_row, s_len; DevBuf<u64> s_start; u64 ns = 0;
     bool built = false;                                // the segment list is built
     void clear() {
         vert.release(); slot.release(); hdeg.release(); n1 = 0; packed = false; pvert.reset(); pperm.reset(); perm_tag = 0;
-        jp.release(); ap.release();
+        jp.release(); ap.release(); ap_sorted = false;
         s_row.release(); s_len.release(); s_start.release(); ns = 0;
         built = false;
     }

@@ -34,6 +34,7 @@ void ensure_init() {
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
     c.num_sms = prop.multiProcessorCount;
+    if (prop.l2CacheSize > 0) c.l2_bytes = (u64)prop.l2CacheSize;
     CUDA_TRY(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
     c.ready = true;
 }
@@ -258,6 +259,30 @@ void sort_pairs_u64(u64 *keys, u64 *vals, size_t n, int end_bit) {
     if (dk.Current() != keys) d2d(keys, dk.Current(), n);
     if (dv.Current() != vals) d2d(vals, dv.Current(), n);
     ctx().lib_launches += 8;
+}
+
+// Sorts the entries of every CSR row: one radix sort of (row, entry) keys over the row-index bits and the entry's 32.  Rows
+// keep their extents, so the sorted low words go straight back.  16 * nnz bytes of temporaries, released on return.
+__global__ void k_row_keys(const u64 *__restrict__ rowptr, u64 nrows, const u32 *__restrict__ cols, u64 *__restrict__ keys) {
+    const u64 nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
+    const u32 lane = threadIdx.x & 31;
+    for (u64 r = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nrows; r += nwarps)
+        for (u64 q = rowptr[r] + lane; q < rowptr[r + 1]; q += 32) keys[q] = (r << 32) | cols[q];
+}
+__global__ void k_keys_low(const u64 *__restrict__ keys, u64 n, u32 *__restrict__ out) {
+    u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    const u64 stride = (u64)gridDim.x * blockDim.x;
+    for (; q < n; q += stride) out[q] = (u32)keys[q];
+}
+void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz) {
+    if (nnz <= 1) return;
+    if (nrows > ((u64)1 << 32)) throw GrbError(-8, "sort_rows_u32: more than 2^32 rows not supported");
+    DevBuf<u64> keys(nnz);
+    LAUNCH(k_row_keys, grid_for(nrows * 32, 256, (u64)ctx().num_sms * 32), 256, 0, rowptr, nrows, cols, keys.ptr);
+    int row_bits = 1;
+    while (row_bits < 32 && ((u64)1 << row_bits) < nrows) row_bits++;
+    sort_keys_u64(keys.ptr, nnz, 32 + row_bits);
+    LAUNCH(k_keys_low, grid_for(nnz, 256, (u64)ctx().num_sms * 32), 256, 0, keys.ptr, nnz, cols);
 }
 
 u64 reduce_sum_u64(const u64 *in, size_t n) {

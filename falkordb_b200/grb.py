@@ -377,6 +377,15 @@ class Matrix:
         check(lib().B200_Matrix_prepare(self.h, int(want_transpose)))
         return self
 
+    def push_operand(self):
+        """(ap, pperm, sorted) of a prepared square matrix: col_idx relabelled to hot-set positions (laid out by the rowptr), the
+        vertex -> position table, and whether every row of ap is ascending -- B200_Matrix_push_operand."""
+        ap = np.zeros(self.nvals(), np.uint32)
+        pperm = np.zeros(self.ncols(), np.uint32)
+        srt = C.c_int(0)
+        check(lib().B200_Matrix_push_operand(self.h, ap.ctypes.data, pperm.ctypes.data, C.byref(srt)))
+        return ap, pperm, bool(srt.value)
+
 
 def rmat(scale, edge_factor=16, seed=1):
     h = P()

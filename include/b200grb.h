@@ -307,6 +307,10 @@ GrB_Info B200_Matrix_digest(GrB_Matrix A, uint64_t *digest3);
 GrB_Info B200_Matrix_device_view(GrB_Matrix A, const uint64_t **Ap, const uint32_t **Aj, const uint64_t **Ax);
 /* Pre-build the cached transpose mirror used by the pull direction (done lazily otherwise). */
 GrB_Info B200_Matrix_prepare(GrB_Matrix A, int want_transpose);
+/* The CSR push's operand of a prepared square matrix, for inspection: ap_out[nvals] = col_idx relabelled to hot-set positions,
+ * laid out by A's rowptr; pperm_out[ncols] = vertex -> position; *sorted = every row of ap ascending (the sliced push's
+ * condition).  Either array may be NULL.  GrB_INVALID_VALUE when the matrix has no such table. */
+GrB_Info B200_Matrix_push_operand(GrB_Matrix A, uint32_t *ap_out, uint32_t *pperm_out, int *sorted);
 /* Synthetic Graph500-style RMAT adjacency (a,b,c,d=.57,.19,.19,.05), dedupe + no self loops, built on
  * the device.  Benchmark / test input only. */
 GrB_Info B200_Matrix_rmat(GrB_Matrix *A, int scale, uint64_t edge_factor, uint64_t seed);

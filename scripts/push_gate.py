@@ -3,7 +3,8 @@
 Workload: bench.py's chain (RMAT-24, edge factor 16, seed 1, 512 sources per batch, the same seeded batches as bench.py's rank 0,
 warm-up batches included).  Hop 1 runs as in the bench (row-wise; its result is a CSR).  Then hop 2 runs from that CSR three ways,
 each followed by hop 3 under the default options, since the form hop 2 leaves decides hop 3's preparation:
-  csr  : csr_push = 2 -- the push straight from F's CSR entries (path 7), whatever the frontier
+  csr  : csr_push = 2 -- the push straight from F's CSR entries (path 7), whatever the frontier, in destination slices
+  csr0 : the same with push_slices = 0 -- its REDs in entry order
   bits : csr_push = 0 -- the frontier is built as a bit-matrix and the direction-optimising hop runs (push, path 2, below the gate)
   pull : pull_mode = 1 -- the bit-matrix pull (path 3)
   auto : the default dispatch (bits.cu: bits_push_from_csr decides between the CSR push and the bit-matrix hop)
@@ -37,7 +38,7 @@ def card():
         return {"error": str(e)}
 
 
-ARMS = {"csr": {"csr_push": 2}, "bits": {"csr_push": 0}, "pull": {"pull_mode": 1}, "auto": {}}
+ARMS = {"csr": {"csr_push": 2}, "csr0": {"csr_push": 2, "push_slices": 0}, "bits": {"csr_push": 0}, "pull": {"pull_mode": 1}, "auto": {}}
 
 
 def main():
@@ -83,7 +84,7 @@ def main():
         ev[1].record(strm)
         path, fl = fb.get_stat("last_path"), fb.get_stat("last_flops")
         for k in ARMS[arm]:
-            fb.set_option(k, {"csr_push": 1, "pull_mode": -1}[k])
+            fb.set_option(k, {"csr_push": 1, "pull_mode": -1, "push_slices": -1}[k])
         G.lmxm(A)
         ev[2].record(strm)
         ev[2].synchronize()
