@@ -9,17 +9,9 @@
 // device and only travel to the host when something observes them (GraphBLAS non-blocking mode:
 // matrix.rs:116-131 initialises GrB_NONBLOCKING).  There is NO CPU implementation of any bulk
 // operation in this file: without a GPU they fail with GxB_GPU_ERROR.
-#include "../../include/b200grb.h"
-#include "common.cuh"
-#include "ops.cuh"
-#include <algorithm>
+#include "handle.cuh"
 #include <cstring>
 #include <memory>
-#include <mutex>
-#include <string>
-#include <vector>
-
-using namespace b200;
 
 // ------------------------------------------------------------------------------------------------ opaque types
 struct GB_Type_opaque { int code; size_t size; const char *name; };
@@ -30,7 +22,6 @@ struct GB_Global_opaque { int x; };
 struct GB_Descriptor_opaque { bool t0, t1, comp, structure, replace; };
 struct GB_Scalar_opaque { int type; bool has; uint64_t val; };   // allocated with the C++ allocator: 24 bytes, short-lived
 
-enum { T_BOOL = 1, T_UINT64 = 2, T_INT64 = 3, T_UINT32 = 4, T_FP64 = 5 };   // FP64 values travel as IEEE-754 bit patterns in the u64 arrays
 enum { OP_ANY_BOOL = 1, OP_SECOND_UINT64 = 2, OP_ANY_UINT64 = 3, OP_PLUS_FP64 = 4 };
 enum { SR_ANY_PAIR = 1, SR_PLUS_TIMES_FP64 = 2, SR_PLUS_SECOND_FP64 = 3 };
 
@@ -65,28 +56,11 @@ DESC(RSC, 1, 1, 1, 0, 0) DESC(RSCT1, 1, 1, 1, 0, 1) DESC(RSCT0, 1, 1, 1, 1, 0) D
 // memory accounting and QUERY_MEM_CAPACITY see this library's host footprint).  Every host container of a handle (tuple
 // stores, pending lists, vector payloads, iterator snapshots) and the handles themselves use it; so do the buffers handed
 // to the caller (unloaded arrays, blobs), which the caller frees with the same allocator (vector.rs:171-172).
-static void *(*g_user_malloc)(size_t) = malloc;
+void *(*g_user_malloc)(size_t) = malloc;
 static void *(*g_user_calloc)(size_t, size_t) = calloc;
 static void *(*g_user_realloc)(void *, size_t) = realloc;
-static void (*g_user_free)(void *) = free;
-static std::atomic<uint64_t> g_host_bytes{0}, g_host_allocs{0};     // live bytes / allocation calls through the hooks
-template <class T> struct UAlloc {
-    typedef T value_type;
-    UAlloc() noexcept {}
-    template <class U> UAlloc(const UAlloc<U> &) noexcept {}
-    T *allocate(size_t n) {
-        if (n > (size_t)-1 / sizeof(T)) throw std::bad_alloc();
-        const size_t bytes = n * sizeof(T);
-        void *p = g_user_malloc(bytes > 0 ? bytes : 1);
-        if (!p) throw std::bad_alloc();
-        g_host_bytes += n * sizeof(T); g_host_allocs++;
-        return (T *)p;
-    }
-    void deallocate(T *p, size_t n) noexcept { g_host_bytes -= n * sizeof(T); g_user_free(p); }
-    template <class U> bool operator==(const UAlloc<U> &) const noexcept { return true; }
-    template <class U> bool operator!=(const UAlloc<U> &) const noexcept { return false; }
-};
-template <class T> using uvec = std::vector<T, UAlloc<T>>;
+void (*g_user_free)(void *) = free;
+std::atomic<uint64_t> g_host_bytes{0}, g_host_allocs{0};     // live bytes / allocation calls through the hooks
 static void *user_zalloc(size_t bytes) {        // zero-initialised block (the container struct); calloc hook when the caller gave one
     void *p = g_user_calloc ? g_user_calloc(1, bytes) : g_user_malloc(bytes);
     if (p && !g_user_calloc) memset(p, 0, bytes);
@@ -100,54 +74,6 @@ static void *user_grow(void *old, size_t old_bytes, size_t new_bytes) {   // rea
 }
 // the hooks as the host-side mirror and the tests see them
 extern "C" void *B200_user_realloc(void *p, size_t old_bytes, size_t new_bytes) { return user_grow(p, old_bytes, new_bytes); }
-// handles: operator new / delete through the same hooks
-struct UObject {
-    static void *operator new(size_t n) {
-        void *p = g_user_malloc(n);
-        if (!p) throw std::bad_alloc();
-        g_host_bytes += n; g_host_allocs++;
-        return p;
-    }
-    static void operator delete(void *p, size_t n) noexcept { if (p) { g_host_bytes -= n; g_user_free(p); } }
-};
-
-struct HostStore {
-    uvec<u64> hrow; // ascending ids of the non-empty rows
-    uvec<u64> hptr; // hrow.size()+1
-    uvec<u64> hcol; // ascending inside a row
-    uvec<u64> hval; // empty for pattern-only (BOOL)
-    void clear() { hrow.clear(); hptr.assign(1, 0); hcol.clear(); hval.clear(); }
-    u64 nnz() const { return hcol.size(); }
-};
-struct PendingOp { u64 i, j, v; u64 seq; bool del; };
-
-static const u32 MAGIC = 0xB200A7u;
-
-struct GB_Matrix_opaque : UObject {
-    u32 magic = MAGIC;
-    int type = T_BOOL;
-    u64 nrows = 0, ncols = 0;
-    std::mutex mu;
-    bool host_valid = true;
-    HostStore host;
-    uvec<PendingOp> pending;
-    bool dev_valid = false;
-    DevCSR dev;
-    bool bits_valid = false;
-    u64 bits_nv = ~0ULL;   // nvals of `bits` once counted (~0 = not yet)
-    int diag_state = -1;   // -1 unknown, 0 no, 1 the device CSR is a diagonal matrix (label matrix): mxm by it is a column filter
-    DevBits bits;
-    bool devT_valid = false;
-    DevCSR devT;
-    PullTables pt;   // pull-direction tables of devT (bits.cu)
-    DevBuf<u32> bfs_deg; u64 bfs_edges = 0; bool bfs_deg_valid = false;   // out-degree table of the BFS engine (bfs_do.cu)
-    DevIdStore ids;  // device copy of the host store, for a Tensor's multi-edge layers (B200_expand_edges)
-    int sparsity_control = GxB_HYPERSPARSE | GxB_SPARSE | GxB_BITMAP | GxB_FULL;
-    int hyper_hash = 1;
-    int orientation = GrB_ROWMAJOR;
-    GB_Matrix_opaque() { host.clear(); }
-    bool valued() const { return type != T_BOOL; }
-};
 
 struct GB_Vector_opaque : UObject {
     u32 magic = MAGIC;
@@ -187,58 +113,8 @@ struct GB_Iterator_opaque : UObject {
 };
 
 // ------------------------------------------------------------------------------------------------ errors
-static thread_local std::string tl_error;
-static std::mutex g_gpu_mu; // serialises GPU submission across caller threads
-// Holds g_gpu_mu for one bulk operation.  If the operation unwinds with an exception, small reads whose destinations lived on
-// the abandoned stack are forgotten BEFORE the mutex is released: once another thread owns the mutex its sync_stream() would
-// otherwise deliver into dead frames.
-struct GpuLock {
-    std::unique_lock<std::mutex> lk;
-    int entry;
-    GpuLock() : lk(g_gpu_mu), entry(std::uncaught_exceptions()) {}
-    ~GpuLock() { if (std::uncaught_exceptions() > entry) drop_small_reads(); }
-};
-
-template <class F>
-static GrB_Info guarded(F &&f) {
-    // an exception may unwind past a small read whose destination lived on the abandoned stack: forget such reads
-    // (drop_small_reads) so that the next sync_stream() does not deliver into dead frames
-    try {
-        return f();
-    } catch (const GrbError &e) {
-        drop_small_reads();
-        tl_error = e.what();
-        return (GrB_Info)e.info;
-    } catch (const CudaError &e) {
-        drop_small_reads();
-        tl_error = e.what();
-        if (e.code == cudaErrorMemoryAllocation) return GrB_OUT_OF_MEMORY;
-        return GxB_GPU_ERROR;
-    } catch (const std::bad_alloc &) {
-        drop_small_reads();
-        tl_error = "host allocation failed";
-        return GrB_OUT_OF_MEMORY;
-    } catch (const std::exception &e) {
-        drop_small_reads();
-        tl_error = e.what();
-        return GrB_PANIC;
-    }
-}
-#define CHECK_PTR(p) do { if (!(p)) { tl_error = "null pointer: " #p; return GrB_NULL_POINTER; } } while (0)
-#define CHECK_MAT(m) do { if (!(m)) { tl_error = "null matrix: " #m; return GrB_NULL_POINTER; } \
-                          if ((m)->magic != MAGIC) { tl_error = "invalid matrix: " #m; return GrB_INVALID_OBJECT; } } while (0)
-
-struct MultiLock {
-    uvec<std::unique_lock<std::mutex>> locks;
-    MultiLock(std::initializer_list<GrB_Matrix> ms) : MultiLock(ms.begin(), ms.end()) {}
-    template <class It> MultiLock(It first, It last) {
-        uvec<GrB_Matrix> v;
-        for (; first != last; ++first) if (*first) v.push_back(*first);
-        std::sort(v.begin(), v.end());
-        v.erase(std::unique(v.begin(), v.end()), v.end());
-        for (GrB_Matrix m : v) locks.emplace_back(m->mu);
-    }
-};
+thread_local std::string tl_error;
+std::mutex g_gpu_mu; // serialises GPU submission across caller threads
 
 // ------------------------------------------------------------------------------------------------ form management
 static void invalidate_aux(GrB_Matrix A) {
@@ -252,7 +128,7 @@ static void invalidate_aux(GrB_Matrix A) {
     A->ids.clear();
 }
 
-static void set_dev(GrB_Matrix A, DevCSR &&d) {
+void set_dev(GrB_Matrix A, DevCSR &&d) {
     A->dev = std::move(d);
     A->dev.nrows = A->nrows; A->dev.ncols = A->ncols;
     // type discipline: BOOL is pattern-only, UINT64/INT64 always carry a value array
@@ -270,7 +146,7 @@ static void set_dev(GrB_Matrix A, DevCSR &&d) {
     invalidate_aux(A);
 }
 
-static void set_bits(GrB_Matrix A, DevBits &&b) {
+void set_bits(GrB_Matrix A, DevBits &&b) {
     A->bits = std::move(b);
     A->bits_nv = ~0ULL;
     A->bits_valid = true;
@@ -300,7 +176,7 @@ static void set_empty(GrB_Matrix A) {
 static void download_to_host(GrB_Matrix A); // fwd
 
 // apply queued setElement / removeElement onto the host store (GrB_Matrix_wait, matrix.rs:781-796)
-static void finish_pending(GrB_Matrix A) {
+void finish_pending(GrB_Matrix A) {
     if (A->pending.empty()) return;
     if (!A->host_valid) download_to_host(A);
     uvec<PendingOp> &p = A->pending;
@@ -379,7 +255,7 @@ static void upload_to_dev(GrB_Matrix A) {
     A->dev_valid = true;
 }
 
-static void ensure_dev(GrB_Matrix A) {
+void ensure_dev(GrB_Matrix A) {
     finish_pending(A);
     if (A->dev_valid) return;
     if (A->bits_valid) {
@@ -417,12 +293,12 @@ static void download_to_host(GrB_Matrix A) {
     A->host_valid = true;
 }
 
-static void ensure_host(GrB_Matrix A) {
+void ensure_host(GrB_Matrix A) {
     if (!A->host_valid) download_to_host(A);
     finish_pending(A);
 }
 
-static void ensure_bits(GrB_Matrix A) {
+void ensure_bits(GrB_Matrix A) {
     finish_pending(A);
     if (A->bits_valid) { natural_bits(A); return; }
     ensure_dev(A);
@@ -433,7 +309,7 @@ static void ensure_bits(GrB_Matrix A) {
     A->bits_valid = true;
 }
 
-static void ensure_devT(GrB_Matrix A) {
+void ensure_devT(GrB_Matrix A) {
     ensure_dev(A);
     if (!A->devT_valid) {
         DevCSR t;
@@ -444,7 +320,7 @@ static void ensure_devT(GrB_Matrix A) {
     // pull-direction auxiliaries (hot-set packing, CSR-stream form, long-row lists) are built lazily by bits_hop
 }
 
-static u64 matrix_nvals(GrB_Matrix A) {
+u64 matrix_nvals(GrB_Matrix A) {
     finish_pending(A);
     if (A->host_valid) return A->host.nnz();
     if (A->dev_valid) return A->dev.nnz;
@@ -453,7 +329,6 @@ static u64 matrix_nvals(GrB_Matrix A) {
 }
 
 // ------------------------------------------------------------------------------------------------ write-back
-struct Desc { bool t0 = false, t1 = false, comp = false, structure = false, replace = false; };
 static Desc get_desc(GrB_Descriptor d) {
     Desc r;
     if (d) { r.t0 = d->t0; r.t1 = d->t1; r.comp = d->comp; r.structure = d->structure; r.replace = d->replace; }
@@ -496,7 +371,7 @@ static void write_back(GrB_Matrix C, DevCSR &&T, GrB_Matrix M, const Desc &d, bo
 // eWiseAdd / eWiseMult / masked-copy calls, so those three set operations exist on the hypersparse host form.  This is
 // NOT a fallback: device-capable operands never take this branch (see is_huge), and mxm on such matrices is refused.
 struct HTup { u64 r, c, v; };
-static bool is_huge(GrB_Matrix A) { return A && (A->nrows >= ((u64)1 << 32) || A->ncols >= ((u64)1 << 32)); }
+bool is_huge(GrB_Matrix A) { return A && (A->nrows >= ((u64)1 << 32) || A->ncols >= ((u64)1 << 32)); }
 static uvec<HTup> host_tuples(GrB_Matrix A) {
     ensure_host(A);
     const HostStore &h = A->host;
@@ -1033,7 +908,7 @@ static bool bits_legal(GrB_Matrix C, GrB_Matrix M, GrB_Matrix A, GrB_Matrix B, c
 // Y = A*B through the frontier dispatch: the push straight from A's entries while A is still a small CSR, the diagonal filter, or
 // the direction-optimising push / pull.  pt_ok: the CSR push may write Y in B's hot-set order.  Returns true when Y came from
 // A's CSR form (A then has no bit form).  acc (union hops): Y |= A*B into a natural-order Y that holds earlier operands' products.
-static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y, u64 *fl, int *path, bool acc = false) {
+extern "C++" bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y, u64 *fl, int *path, bool acc) {
     Context &cx = ctx();
     ensure_dev(B);
     if (B->diag_state < 0) B->diag_state = csr_is_diagonal(B->dev) ? 1 : 0;   // cached until B changes
@@ -1061,8 +936,8 @@ static bool frontier_product(GrB_Matrix A, GrB_Matrix B, bool pt_ok, DevBits &Y,
 // Returns false when the path does not apply (not legal, switched off, or the automatic choice prefers the general row-wise
 // path); C is then unchanged.  dm / dp (B200_Matrix_delta_lmxm): device-resident deltas of B whose terms are applied to the
 // product before it replaces C, while A's frontier is still intact: C = (A*B AND NOT A*dm) OR A*dp.
-static bool frontier_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_Matrix A, GrB_Matrix B, const Desc &d, bool accum,
-                         const DevCSR *dm = nullptr, const DevCSR *dp = nullptr) {
+extern "C++" bool frontier_mxm(GrB_Matrix C, GrB_Matrix Mask, GrB_Matrix A, GrB_Matrix B, const Desc &d, bool accum,
+                               const DevCSR *dm, const DevCSR *dp) {
     Context &cx = ctx();
     if (accum || d.t0 || d.t1 || cx.opt_bits_mode == 0 || !bits_legal(C, Mask, A, B, d)) return false;
     bool use_bits = (cx.opt_bits_mode == 1);
@@ -1820,9 +1695,9 @@ int LAGraph_cdlp(GrB_Vector *CDLP_handle, LAGraph_Graph G, int itermax, char *ms
 // (the same rows of A') the direction-optimising engine runs, its out-degree table cached on A; without it (one GPU, lo = 0)
 // the top-down bfs_run.  Both give level and minimum-id parent.  dest >= 0 stops once that vertex is reached.  dirty (one GPU,
 // B200_bfs_delta): the engine walks those operands instead of A, with deg / total_edges from bfs_delta_degrees.
-static void bfs_staged(GrB_Matrix A, const DevCSR *AT, u64 n, u64 lo, BfsComm *comm, u64 src, i64 max_level, i64 dest,
-                       i64 *level, i64 *parent, int location, B200_BfsInfo *info_out,
-                       const std::vector<BfsOperand> *dirty = nullptr, const u32 *deg = nullptr, u64 total_edges = 0) {
+extern "C++" void bfs_staged(GrB_Matrix A, const DevCSR *AT, u64 n, u64 lo, BfsComm *comm, u64 src, i64 max_level, i64 dest,
+                             i64 *level, i64 *parent, int location, B200_BfsInfo *info_out,
+                             const std::vector<BfsOperand> *dirty, const u32 *deg, u64 total_edges) {
     const u64 nloc = A->nrows, hi = lo + nloc;
     DevBuf<i64> dl, dp;
     i64 *d_level = level, *d_parent = parent;
@@ -2262,903 +2137,6 @@ GrB_Info B200_Matrix_rmat_block(GrB_Matrix *A, int scale, uint64_t edge_factor, 
     });
 }
 
-// ---- unions of relationship operands with pending writes: E = U_t (m[t] \ dm[t]) u dp[t], pattern only ----
-// What the reference builds for a hop or a var-len walk over several relationship types (build_relationship_matrix_unrestricted,
-// graph.rs:2520-2550: extract(T_1), then set_pattern(<!dm_t> m_t) and set_pattern(dp_t) per further type).  The union is exact:
-// an entry that one type contributes survives another type's dm, and within a type dp wins over dm.  Walked by
-// B200_reach_batch_delta and multiplied by the union hops of B200_Matrix_union_lmxm / B200_traverse_batch_union.
-struct UnionOperand {
-    GrB_Matrix m = nullptr, dp = nullptr, dm = nullptr;
-    const DevCSR *ddp = nullptr;                 // dp's device form when it holds entries
-    RepairPlan rp;                               // dm's repair plan (rp.ns == 0: nothing to repair)
-};
-
-static std::vector<UnionOperand> union_operands(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
-    std::vector<UnionOperand> ops(nops);
-    for (int t = 0; t < nops; t++) { ops[t].m = m[t]; ops[t].dp = dp ? dp[t] : nullptr; ops[t].dm = dm ? dm[t] : nullptr; }
-    return ops;
-}
-
-// Y = F * E in frontier form (F at most 1024 rows), under the submission lock; *fl += sum_t flops(F * m[t]) + flops(F * dp[t]).
-// The first operand with a repair plan goes first: it writes Y fresh and has the columns its dm touches recomputed in place
-// (bits_repair overwrites columns, so it cannot accumulate).  Every further clean operand ORs into the same natural-order Y: the
-// pushes skip zeroing Y and the pull ORs each row into the stored record.  A further operand with a repair plan (or every further
-// operand with union_accum = 0) gets a bit-matrix of its own that is repaired, naturalised and ORed in.  pt_ok applies to a single
-// operand only: the CSR push may then leave Y in the operand's hot-set order, as GrB_mxm does.
-static void union_product(GrB_Matrix F, std::vector<UnionOperand> &ops, bool pt_ok, DevBits &Y, u64 *fl, int *path) {
-    Context &cx = ctx();
-    const size_t nops = ops.size();
-    finish_pending(F);
-    std::vector<UnionOperand *> order;
-    for (UnionOperand &o : ops) if (o.rp.ns) { order.push_back(&o); break; }
-    for (UnionOperand &o : ops) if (order.empty() || &o != order[0]) order.push_back(&o);
-    DevBits Xcsr;
-    for (size_t i = 0; i < nops; i++) {
-        UnionOperand &o = *order[i];
-        const bool own = i > 0 && (o.rp.ns || !cx.opt_union_accum);
-        DevBits Z;
-        DevBits &T = own ? Z : Y;
-        u64 f = 0;
-        const bool from_csr = frontier_product(F, o.m, nops == 1 && pt_ok, T, &f, path, i > 0 && !own);
-        if (o.rp.ns) {
-            // the repair gathers from F in bit form: a frontier still in CSR form is converted for it
-            if (from_csr && !Xcsr.valid()) bits_from_csr(F->dev, Xcsr);
-            ensure_devT(o.m);
-            bits_repair(from_csr ? Xcsr : F->bits, o.m->devT, o.rp, T);
-        }
-        if (o.ddp) f += bits_apply_deltas(from_csr ? nullptr : &F->bits, from_csr ? &F->dev : nullptr, nullptr, o.ddp, T);
-        *fl += f;
-        if (own) { bits_naturalise(Z); bits_or(Y, Z); }
-    }
-}
-
-// *U = a new BOOL matrix holding the union over the operands of their induced effective layers ((m \ dm) u dp restricted to the
-// kept vertices and renumbered by rank, adj.cu), and with symmetric its union with its transpose.  keep null: vertices below n_out,
-// U is n_out x n_out; else the strictly ascending keep[0 .. nkeep), U is nkeep x nkeep.  Arguments checked by the caller.
-static GrB_Info effective_adjacency(GrB_Matrix *U, const std::vector<UnionOperand> &ops, u64 n_out, const GrB_Index *keep, u64 nkeep,
-                                    bool symmetric) {
-    const u64 rows = keep ? nkeep : n_out;
-    GrB_Info info = GrB_Matrix_new(U, GrB_BOOL, rows, rows);
-    if (info) return info;
-    info = guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (const UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-        all.push_back(*U);
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        DevBuf<u64> dkeep;
-        DevBuf<u32> rank;
-        if (keep) {
-            dkeep.alloc(nkeep ? nkeep : 1);
-            h2d(dkeep.ptr, (const u64 *)keep, nkeep);
-            adj_rank_table(dkeep.ptr, nkeep, ops[0].m->ncols, rank);
-        }
-        DevCSR S;
-        bool have = false;
-        for (const UnionOperand &o : ops) {
-            ensure_dev(o.m);
-            const DevCSR *ddm = nullptr;
-            if (o.dm) { ensure_dev(o.dm); if (o.dm->dev.nnz) ddm = &o.dm->dev; }
-            DevCSR E;
-            adj_layer(o.m->dev, ddm, n_out, keep ? dkeep.ptr : nullptr, rank.ptr, nkeep, E);
-            if (o.dp) {
-                ensure_dev(o.dp);
-                if (o.dp->dev.nnz) {                 // dp's layer is merged in whole: within a type dp wins over dm
-                    DevCSR D, T;
-                    adj_layer(o.dp->dev, nullptr, n_out, keep ? dkeep.ptr : nullptr, rank.ptr, nkeep, D);
-                    ewise_union(E, D, false, T);
-                    E = std::move(T);
-                }
-            }
-            if (!have) { S = std::move(E); have = true; }
-            else { DevCSR T; ewise_union(S, E, false, T); S = std::move(T); }
-        }
-        if (symmetric) {
-            DevCSR ST, T;
-            transpose_csr(S, ST, false);
-            ewise_union(S, ST, false, T);
-            S = std::move(T);
-        }
-        set_dev(*U, std::move(S));
-        return GrB_SUCCESS;
-    });
-    if (info) GrB_Matrix_free(U);
-    return info;
-}
-
-// U = the union of every operand's effective pattern (m \ dm) u dp over all n vertices
-static GrB_Info reach_materialise(GrB_Matrix *U, std::vector<UnionOperand> &ops, u64 n) {
-    return effective_adjacency(U, ops, n, nullptr, 0, false);
-}
-
-// per call, for the frontier form: deltas' pending tuples finished, dp's device form, and dm's repair plan (dm' and the repaired
-// segments of m', the base's mirror built at commit)
-static GrB_Info union_plan(std::vector<UnionOperand> &ops) {
-    return guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        for (UnionOperand &o : ops) {
-            if (o.dp) { ensure_dev(o.dp); if (o.dp->dev.nnz) o.ddp = &o.dp->dev; }
-            if (!o.dm) continue;
-            ensure_dev(o.dm);
-            if (!o.dm->dev.nnz) continue;
-            ensure_devT(o.m);
-            bits_repair_plan(o.dm->dev, o.m->devT, o.rp);
-        }
-        return GrB_SUCCESS;
-    });
-}
-
-// the plans' device buffers go back to the pool
-static void union_release(std::vector<UnionOperand> &ops) { guarded([&]() { GpuLock g; ops.clear(); return GrB_SUCCESS; }); }
-
-// ---- union hops: F <- F * E, exact (no delta_lmxm over-masking) ----
-// A union hop is prepared once per call: with F in frontier form (a BOOL F of at most 1024 rows and bits_mode != 0) the operands'
-// repair plans, otherwise the union materialised once (reach_materialise) for the general GrB_mxm -- the reference's cost, paid
-// per call rather than per hop.  last_flops of a union hop = sum_t flops(F * m[t]) + flops(F * dp[t]) on either path: the work
-// the frontier form does, independent of how the operands overlap.
-struct UnionHop {
-    std::vector<UnionOperand> ops;
-    GrB_Matrix U = nullptr;                      // the materialised union (row-wise path)
-};
-
-static bool union_frontier(u64 rows, u64 n) {
-    return ctx().opt_bits_mode != 0 && bits_words_for(rows) != 0 && n < ((u64)1 << 32);
-}
-
-static GrB_Info union_hop_prepare(UnionHop &uh, bool frontier, u64 n) {
-    return frontier ? union_plan(uh.ops) : reach_materialise(&uh.U, uh.ops, n);
-}
-
-static void union_hop_release(UnionHop &uh) {
-    GrB_Matrix_free(&uh.U);
-    union_release(uh.ops);
-}
-
-static GrB_Info union_hop_apply(GrB_Matrix F, UnionHop &uh) {
-    uvec<GrB_Matrix> all = {F};
-    for (UnionOperand &o : uh.ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-    if (uh.U) {
-        u64 fl = 0;
-        GrB_Info info = guarded([&]() {
-            GpuLock g;
-            MultiLock lk(all.begin(), all.end());
-            ensure_init();
-            ensure_dev(F);
-            for (UnionOperand &o : uh.ops) {
-                ensure_dev(o.m);
-                fl += spgemm_flops(F->dev, o.m->dev);
-                if (o.dp) { ensure_dev(o.dp); fl += spgemm_flops(F->dev, o.dp->dev); }
-            }
-            return GrB_SUCCESS;
-        });
-        if (!info) info = GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, uh.U, nullptr);
-        if (!info) { Context &cx = ctx(); cx.total_flops -= cx.last_flops.load(); cx.total_flops += fl; cx.last_flops = fl; }
-        return info;
-    }
-    return guarded([&]() {
-        GpuLock g;
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        Context &cx = ctx();
-        DevBits Y;
-        u64 fl = 0;
-        int path = 0;
-        union_product(F, uh.ops, true, Y, &fl, &path);
-        cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
-        set_bits(F, std::move(Y));
-        if (cx.opt_sync_after_op) sync_stream();
-        return GrB_SUCCESS;
-    });
-}
-
-// nops >= 1 operands and their deltas: square, of one size, device-resident
-static GrB_Info union_check(const char *what, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
-    CHECK_PTR(m);
-    if (nops < 1) { tl_error = std::string(what) + ": nops < 1"; return GrB_INVALID_VALUE; }
-    for (int t = 0; t < nops; t++) {
-        CHECK_MAT(m[t]);
-        if (dp && dp[t]) CHECK_MAT(dp[t]);
-        if (dm && dm[t]) CHECK_MAT(dm[t]);
-    }
-    const u64 n = m[0]->nrows;
-    for (int t = 0; t < nops; t++)
-        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
-            if (X && (X->nrows != n || X->ncols != n)) {
-                tl_error = std::string(what) + ": operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-            }
-    for (int t = 0; t < nops; t++)
-        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
-            if (X && is_huge(X)) { tl_error = std::string(what) + ": host-resident operand"; return GrB_NOT_IMPLEMENTED; }
-    return GrB_SUCCESS;
-}
-
-static GrB_Info device_ready() { return guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; }); }
-
-// The union hop as one call, the counterpart of B200_Matrix_delta_lmxm: F <- F * U_t (m[t] \ dm[t]) u dp[t].
-GrB_Info B200_Matrix_union_lmxm(GrB_Matrix F, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
-    CHECK_MAT(F);
-    GrB_Info info = union_check("union_lmxm", m, dp, dm, nops);
-    if (info) return info;
-    const u64 n = m[0]->nrows;
-    if (F->ncols != n) { tl_error = "union_lmxm: F * m does not fit F"; return GrB_DIMENSION_MISMATCH; }
-    if (is_huge(F)) { tl_error = "union_lmxm: host-resident frontier"; return GrB_NOT_IMPLEMENTED; }
-    info = device_ready();                       // no device: fail before any host work
-    if (info) return info;
-    UnionHop uh;
-    uh.ops = union_operands(m, dp, dm, nops);
-    info = union_hop_prepare(uh, F->type == T_BOOL && union_frontier(F->nrows, n), n);
-    if (!info) info = union_hop_apply(F, uh);
-    union_hop_release(uh);
-    return info;
-}
-
-// ---- delta_lmxm as ONE C call (matrix.rs:1317-1402): F <- (F*m AND NOT F*dm) OR F*dp over GxB_ANY_PAIR_BOOL ----
-// The reference composes three GrB_mxm calls and an eWiseAdd, each of which builds or rewrites a whole |F| x n bit-matrix.  In
-// frontier form only the deltas' entries are touched here: F*m runs through GrB_mxm's frontier path unchanged, then the dm and dp
-// terms are applied to the product in place (bits_apply_deltas) before it replaces F.  Where the frontier path does not apply
-// (bits_mode 0, more than 1024 rows, or the automatic choice takes the general row-wise path) the three-call composition runs.
-// last_flops = flops(F*m) + flops(F*dp) + flops(F*dm), as the composition reports them.
-static GrB_Info delta_compose(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_Matrix dm) {
-    GrB_Index np = 0, nm = 0;
-    GrB_Info info = GrB_SUCCESS;
-    if (dp) info = GrB_Matrix_nvals(&np, dp);
-    if (!info && dm) info = GrB_Matrix_nvals(&nm, dm);
-    if (info) return info;
-    if (!np && !nm) return GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, m, nullptr);
-    GrB_Matrix mk = nullptr, ac = nullptr;
-    u64 flops = 0;
-    auto product = [&](GrB_Matrix *out, GrB_Matrix D) {        // *out = F * D, dropped when empty
-        GrB_Index nv = 0;
-        GrB_Info e = GrB_Matrix_new(out, GrB_BOOL, F->nrows, m->ncols);
-        if (!e) e = GrB_mxm(*out, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, D, nullptr);
-        if (!e) { flops += ctx().last_flops.load(); e = GrB_Matrix_nvals(&nv, *out); }
-        if (!e && !nv) GrB_Matrix_free(out);
-        return e;
-    };
-    if (nm) info = product(&mk, dm);
-    if (!info && np) info = product(&ac, dp);
-    if (!info) info = GrB_mxm(F, mk, nullptr, GxB_ANY_PAIR_BOOL, F, m, mk ? GrB_DESC_RSC : nullptr);
-    if (!info) flops += ctx().last_flops.load();
-    if (!info && ac) info = GrB_Matrix_eWiseAdd_BinaryOp(F, nullptr, nullptr, GxB_ANY_BOOL, F, ac, nullptr);
-    GrB_Matrix_free(&mk);
-    GrB_Matrix_free(&ac);
-    if (!info) ctx().last_flops = flops;
-    return info;
-}
-
-GrB_Info B200_Matrix_delta_lmxm(GrB_Matrix F, GrB_Matrix m, GrB_Matrix dp, GrB_Matrix dm) {
-    CHECK_MAT(F); CHECK_MAT(m);
-    if (dp) CHECK_MAT(dp);
-    if (dm) CHECK_MAT(dm);
-    if (F->ncols != m->nrows || F->ncols != m->ncols) { tl_error = "delta_lmxm: F * m does not fit F"; return GrB_DIMENSION_MISMATCH; }
-    for (GrB_Matrix D : {dp, dm})
-        if (D && (D->nrows != m->nrows || D->ncols != m->ncols)) { tl_error = "delta_lmxm: delta dimensions differ from m"; return GrB_DIMENSION_MISMATCH; }
-    if (!dp && !dm) return GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, m, nullptr);
-    bool done = false;
-    GrB_Info info = guarded([&]() {
-        GpuLock g;
-        MultiLock lk{F, m, dp, dm};
-        for (GrB_Matrix X : {F, m, dp, dm})
-            if (is_huge(X)) throw GrbError(GrB_NOT_IMPLEMENTED, "delta_lmxm: host-resident matrix");
-        ensure_init();
-        const DevCSR *ddm = nullptr, *ddp = nullptr;
-        if (dm) { ensure_dev(dm); if (dm->dev.nnz) ddm = &dm->dev; }      // pending tuples finish first (dm.wait())
-        if (dp) { ensure_dev(dp); if (dp->dev.nnz) ddp = &dp->dev; }
-        done = frontier_mxm(F, nullptr, F, m, Desc(), false, ddm, ddp);
-        return GrB_SUCCESS;
-    });
-    if (info || done) return info;
-    return delta_compose(F, m, dp, dm);
-}
-
-// ---- the coalesced traversal as ONE C call (SURVEY 8f-1: CondTraverseOp's batch coalescing, cond_traverse.rs:600-608, 1264-1285) ----
-// F(i, sources[i]) = 1;  F <- F * hops[0] * ... * hops[nhops-1] over GxB_ANY_PAIR_BOOL;  result rows to HOST memory.
-//   B200_OUT_BITMAP : out_bits[row * words_per_row + (col >> 6)], one bit per slot.  The batch is processed in 128-row slices and
-//                     slice k's device-to-host copy (second stream) overlaps slice k+1's hops; page-locked out_bits makes the
-//                     copies asynchronous.
-//   B200_OUT_CSR    : out_p[nsrc + 1], out_j[<= out_j_capacity]; GrB_INSUFFICIENT_SPACE (with *nvals_out = entries needed) when the
-//                     buffer is too small.
-//   B200_OUT_AUTO   : bitmap when the result holds more than one entry per 32 slots (fewer bytes over PCIe), else CSR; the choice
-//                     is reported in *format_out.  Needs both output buffers.
-// Composed from the public entry points (each takes the submission lock for its own duration), so other threads' calls interleave.
-// Operands are hop-major: hop h owns hop_nops[h] consecutive entries of hops / dp / dm (hop_nops NULL: one each).  A delta hop
-// (hop_union NULL or hop_union[h] == 0, one operand k) is B200_Matrix_delta_lmxm(F, hops[k], dp[k], dm[k]); a union hop is
-// B200_Matrix_union_lmxm over its operands, prepared once per call (union_hop_prepare).  dp / dm NULL (B200_traverse_batch) or
-// holding NULL entries: clean operands.
-static GrB_Info traverse_impl(const GrB_Index *sources, GrB_Index nsrc, const int *hop_nops, const int *hop_union,
-                              const GrB_Matrix *hops, const GrB_Matrix *dp, const GrB_Matrix *dm, int nhops, int format,
-                              uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
-                              uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
-    CHECK_PTR(hops);
-    if (nsrc) CHECK_PTR(sources);
-    if (nhops < 1) { tl_error = "traverse_batch: nhops < 1"; return GrB_INVALID_VALUE; }
-    std::vector<int> first(nhops + 1, 0);        // hop h's operands: [first[h], first[h + 1]) (hop_nops checked by the caller)
-    for (int h = 0; h < nhops; h++) first[h + 1] = first[h] + (hop_nops ? hop_nops[h] : 1);
-    const int nopd = first[nhops];
-    for (int k = 0; k < nopd; k++) {
-        CHECK_MAT(hops[k]);
-        if (dp && dp[k]) CHECK_MAT(dp[k]);
-        if (dm && dm[k]) CHECK_MAT(dm[k]);
-    }
-    if (format != B200_OUT_BITMAP && format != B200_OUT_CSR && format != B200_OUT_AUTO) { tl_error = "traverse_batch: unknown format"; return GrB_INVALID_VALUE; }
-    if ((format != B200_OUT_CSR && !out_bits) || (format != B200_OUT_BITMAP && (!out_p || (!out_j && out_j_capacity)))) {
-        tl_error = "traverse_batch: output buffer missing for the requested format"; return GrB_NULL_POINTER;
-    }
-    const u64 inner = hops[0]->nrows, ncols = hops[nopd - 1]->ncols;
-    const u64 wpr = (ncols + 63) / 64;
-    if (format != B200_OUT_CSR && words_per_row != wpr) { tl_error = "traverse_batch: words_per_row must be ceil(ncols / 64)"; return GrB_DIMENSION_MISMATCH; }
-    // GrB_mxm(C = F, A = F, B) needs C's dimensions to match the product: a chain over square n x n operands (what the reference
-    // stores, graph.rs:1191, 1211) keeps them; rectangular chains are rejected up front
-    for (int k = 0; k < nopd; k++) {
-        if (hops[k]->nrows != inner || hops[k]->ncols != inner) { tl_error = "traverse_batch: operands must be square and equally sized"; return GrB_DIMENSION_MISMATCH; }
-        for (GrB_Matrix D : {dp ? dp[k] : nullptr, dm ? dm[k] : nullptr})
-            if (D && (D->nrows != inner || D->ncols != inner)) { tl_error = "traverse_batch: delta dimensions differ from the hop's"; return GrB_DIMENSION_MISMATCH; }
-    }
-    GrB_Scalar one = nullptr;
-    GrB_Info info = GrB_Scalar_new(&one, GrB_BOOL);
-    if (info) return info;
-    GrB_Scalar_setElement_BOOL(one, true);
-    // union hops: plans (frontier form, for the rows of one F: a 128-row slice or the whole batch) or the materialised union
-    std::vector<UnionHop> uhops(hop_union ? nhops : 0);
-    const bool ufrontier = union_frontier(format == B200_OUT_BITMAP ? std::min<u64>(nsrc, 128) : nsrc, inner);
-    for (int h = 0; h < (int)uhops.size() && !info; h++)
-        if (hop_union[h]) {
-            uhops[h].ops = union_operands(hops + first[h], dp ? dp + first[h] : nullptr, dm ? dm + first[h] : nullptr, first[h + 1] - first[h]);
-            info = union_hop_prepare(uhops[h], ufrontier, inner);
-        }
-    u64 flops = 0, nvals = 0;
-    int chosen = format;
-    std::vector<B200_Ticket> tickets;
-    auto run_hops = [&](GrB_Matrix F, u64 r0, u64 r1) -> GrB_Info {
-        uvec<u64> rows(r1 - r0);
-        for (u64 i = 0; i < r1 - r0; i++) rows[i] = i;
-        GrB_Info e = GxB_Matrix_build_Scalar(F, rows.data(), sources + r0, one, r1 - r0);
-        for (int h = 0; h < nhops && !e; h++) {
-            const int k = first[h];
-            e = (hop_union && hop_union[h]) ? union_hop_apply(F, uhops[h])
-                                            : B200_Matrix_delta_lmxm(F, hops[k], dp ? dp[k] : nullptr, dm ? dm[k] : nullptr);
-            if (!e) flops += ctx().last_flops.load();
-            if (!e && h + 1 < nhops && F->ncols != hops[first[h + 1]]->nrows) { tl_error = "traverse_batch: hop dimensions do not chain"; e = GrB_DIMENSION_MISMATCH; }
-        }
-        return e;
-    };
-    auto fresh = [&](GrB_Matrix *F, u64 rows) -> GrB_Info {
-        // the frontier's column dimension follows the hops: n0 x n1 x ... (rectangular label ranges are n x n in the reference)
-        return GrB_Matrix_new(F, GrB_BOOL, rows, inner);
-    };
-    if (!info && (format == B200_OUT_AUTO || format == B200_OUT_CSR)) {
-        // density is known only after the hops: run the whole batch once, then pick the hand-off
-        GrB_Matrix F = nullptr;
-        info = fresh(&F, nsrc);
-        if (!info) info = run_hops(F, 0, nsrc);
-        if (!info) info = GrB_Matrix_nvals(&nvals, F);
-        if (!info) {
-            if (format == B200_OUT_AUTO) chosen = (nvals * 32 > nsrc * ncols) ? B200_OUT_BITMAP : B200_OUT_CSR;
-            if (chosen == B200_OUT_BITMAP) info = B200_Matrix_export_bitmap(F, out_bits, wpr, nullptr, B200_LOC_HOST);
-            else if (nvals > out_j_capacity) { tl_error = "traverse_batch: out_j too small"; info = GrB_INSUFFICIENT_SPACE; }
-            else {
-                info = GrB_Matrix_wait(F, GrB_MATERIALIZE);
-                if (!info) info = B200_Matrix_export_CSR(F, out_p, out_j, nullptr, B200_LOC_HOST);
-            }
-        }
-        GrB_Matrix_free(&F);
-    } else if (!info) {
-        const u64 per = 128;
-        for (u64 r0 = 0; r0 < nsrc && !info; r0 += per) {
-            const u64 r1 = std::min<u64>(nsrc, r0 + per);
-            GrB_Matrix F = nullptr;
-            info = fresh(&F, r1 - r0);
-            if (!info) info = run_hops(F, r0, r1);
-            B200_Ticket t = nullptr;
-            if (!info) info = B200_Matrix_export_bitmap_async(F, out_bits + r0 * wpr, wpr, &t);
-            if (!info) tickets.push_back(t);
-            GrB_Matrix_free(&F);
-        }
-        for (B200_Ticket &t : tickets) { GrB_Info e = B200_Ticket_wait(&t); if (!info) info = e; }
-        nvals = ~0ULL;       // not counted on this path (a popcount pass per slice would only serve this number)
-    }
-    for (UnionHop &uh : uhops) union_hop_release(uh);
-    GrB_Scalar_free(&one);
-    if (nvals_out) *nvals_out = nvals;
-    if (flops_out) *flops_out = flops;
-    if (format_out) *format_out = chosen;
-    return info;
-}
-
-GrB_Info B200_traverse_batch(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *hops, int nhops, int format,
-                             uint64_t *out_bits, uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
-                             uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
-    return traverse_impl(sources, nsrc, nullptr, nullptr, hops, nullptr, nullptr, nhops, format, out_bits, words_per_row, out_p, out_j,
-                         out_j_capacity, nvals_out, flops_out, format_out);
-}
-
-// The same traversal over operands with pending writes: hop h is (m[h], dp[h], dm[h]) through B200_Matrix_delta_lmxm.
-GrB_Info B200_traverse_batch_delta(const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
-                                   const GrB_Matrix *dm, int nhops, int format, uint64_t *out_bits, uint64_t words_per_row,
-                                   uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity, uint64_t *nvals_out, uint64_t *flops_out,
-                                   int *format_out) {
-    return traverse_impl(sources, nsrc, nullptr, nullptr, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j,
-                         out_j_capacity, nvals_out, flops_out, format_out);
-}
-
-// The same traversal over hop groups: hop h is a delta hop (hop_union[h] == 0, hop_nops[h] == 1) or a union hop over its
-// hop_nops[h] operands (B200_Matrix_union_lmxm).  Operands, validation and errors as B200_Matrix_union_lmxm.
-GrB_Info B200_traverse_batch_union(const GrB_Index *sources, GrB_Index nsrc, const int *hop_nops, const int *hop_union, int nhops,
-                                   const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int format, uint64_t *out_bits,
-                                   uint64_t words_per_row, uint64_t *out_p, uint32_t *out_j, uint64_t out_j_capacity,
-                                   uint64_t *nvals_out, uint64_t *flops_out, int *format_out) {
-    CHECK_PTR(hop_nops); CHECK_PTR(hop_union);
-    if (nsrc) CHECK_PTR(sources);
-    if (nhops < 1) { tl_error = "traverse_batch: nhops < 1"; return GrB_INVALID_VALUE; }
-    int nopd = 0;
-    for (int h = 0; h < nhops; h++) {
-        if (hop_nops[h] < 1) { tl_error = "traverse_batch: a hop has no operand"; return GrB_INVALID_VALUE; }
-        if (hop_nops[h] > 1 && !hop_union[h]) { tl_error = "traverse_batch: a delta hop takes one operand"; return GrB_INVALID_VALUE; }
-        nopd += hop_nops[h];
-    }
-    GrB_Info info = union_check("traverse_batch_union", m, dp, dm, nopd);
-    if (!info) info = device_ready();           // no device: fail before any host work
-    if (info) return info;
-    return traverse_impl(sources, nsrc, hop_nops, hop_union, m, dp, dm, nhops, format, out_bits, words_per_row, out_p, out_j,
-                         out_j_capacity, nvals_out, flops_out, format_out);
-}
-
-// ---- multi-source reachability as ONE C call (SURVEY 8f-1: the multiplicity-insensitive core of CondVarLenTraverse with
-// emit_path = false, cond_var_len_traverse.rs:196, and of AllShortestPaths' BFS phase, all_shortest_paths.rs:7-25) ----
-// Row i of *reached = every vertex reachable from sources[i] by a walk of 1..max_hops edges of A (max_hops < 0: until no row finds
-// a new vertex); with include_sources the zero-length walk (i, sources[i]) belongs to the result and is never re-discovered.
-// Each level is F<!R, replace, struct> = F*A (GrB_DESC_RSC, matrix.rs:1386) followed by R = R u F (matrix.rs:1398-1400); both stay
-// in device frontier form for <= 1024 sources.  Composed from the public entry points.  *reached is a new nsrc x n BOOL matrix.
-//
-// B200_reach_batch_delta walks A = U_t (m[t] \ dm[t]) u dp[t] exactly (no delta_lmxm over-masking).  One operand without deltas
-// (B200_reach_batch) issues the calls above unchanged.  Otherwise a level in frontier form is reach_hop: Y = F * A through
-// union_product (per operand Y = F*m[t] through the usual dispatch, the columns dm[t] touches recomputed from m[t]'s transpose
-// mirror without the deleted in-edges (bits_repair), then the dp[t] term, the operands' products ORed into one Y), and only then is
-// the reached set masked out, so a dp edge cannot re-add a vertex already reached.  With bits_mode -1 the dirty reach stays in frontier form whenever it is legal (a tiny
-// hop-1 frontier takes the CSR push there): the row-wise path would first need every dirty operand rewritten, O(nnz(m)) per call.
-// Where the frontier path does not apply (bits_mode 0, more than 1024 sources) every dirty operand is materialised once per call
-// by the adjacency builder (effective_adjacency, identity form) and the level runs the calls above over their union.
-
-// One level in frontier form: F <- (F * A) AND NOT R (R only when masked).  F has at most 1024 rows.  Runs under the submission
-// lock.  One operand and no mask: the CSR push may leave Y in the operand's hot-set order, as GrB_mxm does.
-static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<UnionOperand> &ops) {
-    Context &cx = ctx();
-    DevBits acc;
-    u64 fl = 0;
-    int path = 0;
-    union_product(F, ops, !masked, acc, &fl, &path);
-    if (masked) {
-        bits_naturalise(acc);
-        ensure_bits(R);
-        bits_andnot(acc, R->bits);
-    }
-    cx.last_flops = fl; cx.total_flops += fl; cx.last_path = (u64)path;
-    set_bits(F, std::move(acc));
-    if (cx.opt_sync_after_op) sync_stream();
-}
-
-static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
-                           const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources, int64_t *levels_out) {
-    const u64 n = m[0]->ncols;
-    bool clean = nops == 1;
-    for (int t = 0; t < nops && clean; t++)
-        for (GrB_Matrix D : {dp ? dp[t] : nullptr, dm ? dm[t] : nullptr}) {
-            GrB_Index nv = 0;
-            if (!D) continue;
-            GrB_Info e = GrB_Matrix_nvals(&nv, D);
-            if (e) return e;
-            if (nv) clean = false;
-        }
-    GrB_Matrix U = nullptr;                      // the materialised union, when a level runs the row-wise calls
-    GrB_Info info = GrB_SUCCESS;
-    std::vector<UnionOperand> ops = union_operands(m, dp, dm, nops);
-    const bool frontier = ctx().opt_bits_mode != 0 && bits_words_for(nsrc) != 0;
-    if (!clean && !frontier) info = reach_materialise(&U, ops, n);
-    else if (!clean) info = union_plan(ops);
-    GrB_Matrix A = U ? U : m[0];                 // the operand of the row-wise calls
-    GrB_Scalar one = nullptr;
-    GrB_Matrix F = nullptr, R = nullptr;
-    if (!info) info = GrB_Scalar_new(&one, GrB_BOOL);
-    if (!info) info = GrB_Scalar_setElement_BOOL(one, true);
-    if (!info) info = GrB_Matrix_new(&F, GrB_BOOL, nsrc, n);
-    if (!info) info = GrB_Matrix_new(&R, GrB_BOOL, nsrc, n);
-    if (!info && nsrc) {
-        uvec<u64> rows(nsrc);
-        for (u64 i = 0; i < nsrc; i++) rows[i] = i;
-        info = GxB_Matrix_build_Scalar(F, rows.data(), sources, one, nsrc);
-        if (!info && include_sources) info = GxB_Matrix_build_Scalar(R, rows.data(), sources, one, nsrc);
-    }
-    int64_t level = 0;
-    while (!info && nsrc && (max_hops < 0 || level < max_hops)) {
-        GrB_Index rn = 0, fn = 0;
-        info = GrB_Matrix_nvals(&rn, R);
-        if (info) break;
-        if (!clean && !U) {
-            info = guarded([&]() {
-                GpuLock g;
-                uvec<GrB_Matrix> all = {F, R};
-                for (UnionOperand &o : ops) { all.push_back(o.m); all.push_back(o.dp); all.push_back(o.dm); }
-                MultiLock lk(all.begin(), all.end());
-                ensure_init();
-                reach_hop(F, R, rn != 0, ops);
-                return GrB_SUCCESS;
-            });
-        } else {
-            info = rn ? GrB_mxm(F, R, nullptr, GxB_ANY_PAIR_BOOL, F, A, GrB_DESC_RSC)
-                      : GrB_mxm(F, nullptr, nullptr, GxB_ANY_PAIR_BOOL, F, A, nullptr);
-        }
-        if (!info) info = GrB_Matrix_nvals(&fn, F);
-        if (info || fn == 0) break;
-        info = GrB_Matrix_eWiseAdd_BinaryOp(R, nullptr, nullptr, GxB_ANY_BOOL, R, F, nullptr);
-        level++;
-    }
-    GrB_Scalar_free(&one);
-    GrB_Matrix_free(&F);
-    GrB_Matrix_free(&U);
-    if (!clean) union_release(ops);
-    if (info) { GrB_Matrix_free(&R); return info; }
-    if (levels_out) *levels_out = level;
-    *reached = R;
-    return GrB_SUCCESS;
-}
-
-GrB_Info B200_reach_batch(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, GrB_Matrix A, int64_t max_hops,
-                          int include_sources, int64_t *levels_out) {
-    CHECK_PTR(reached); CHECK_MAT(A);
-    if (nsrc) CHECK_PTR(sources);
-    if (A->nrows != A->ncols) { tl_error = "reach_batch: A must be square"; return GrB_DIMENSION_MISMATCH; }
-    return reach_impl(reached, sources, nsrc, &A, nullptr, nullptr, 1, max_hops, include_sources, levels_out);
-}
-
-GrB_Info B200_reach_batch_delta(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m,
-                                const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources,
-                                int64_t *levels_out) {
-    CHECK_PTR(reached); CHECK_PTR(m);
-    if (nsrc) CHECK_PTR(sources);
-    if (nops < 1) { tl_error = "reach_batch_delta: nops < 1"; return GrB_INVALID_VALUE; }
-    for (int t = 0; t < nops; t++) {
-        CHECK_MAT(m[t]);
-        if (dp && dp[t]) CHECK_MAT(dp[t]);
-        if (dm && dm[t]) CHECK_MAT(dm[t]);
-    }
-    const u64 n = m[0]->nrows;
-    for (int t = 0; t < nops; t++)
-        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
-            if (X && (X->nrows != n || X->ncols != n)) {
-                tl_error = "reach_batch_delta: operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-            }
-    if (is_huge(m[0])) { tl_error = "reach_batch_delta: host-resident operand"; return GrB_NOT_IMPLEMENTED; }
-    GrB_Info info = guarded([&]() { GpuLock g; ensure_init(); return GrB_SUCCESS; });   // no device: fail before any host work
-    if (info) return info;
-    return reach_impl(reached, sources, nsrc, m, dp, dm, nops, max_hops, include_sources, levels_out);
-}
-
-// ---- single-source BFS over relationship operands with pending writes (algo.BFS, algo_procedures.rs:1021-1166) ----
-// The reference builds A = U_t (m[t] \ dm[t]) u dp[t] afresh on every call (build_adjacency_matrix, graph.rs:3870-3893) and runs
-// LAGr_BreadthFirstSearch_Extended on it.  Here the direction-optimising engine walks the operands in place: each base's transpose
-// mirror and out-degree table are cached on its handle (ensure_devT, bfs_deg) and reused until the base changes; only the deltas'
-// transposes are built per call.  One operand without deltas is exactly B200_Matrix_prepare(A, 1) + B200_bfs_ex.
-GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index src, int64_t max_level,
-                        int64_t dest, int64_t *level, int64_t *parent, int location, B200_BfsInfo *info_out) {
-    CHECK_PTR(m); CHECK_PTR(level);
-    if (nops < 1) { tl_error = "bfs_delta: nops < 1"; return GrB_INVALID_VALUE; }
-    for (int t = 0; t < nops; t++) {
-        CHECK_MAT(m[t]);
-        if (dp && dp[t]) CHECK_MAT(dp[t]);
-        if (dm && dm[t]) CHECK_MAT(dm[t]);
-    }
-    const u64 n = m[0]->nrows;
-    for (int t = 0; t < nops; t++)
-        for (GrB_Matrix X : {m[t], dp ? dp[t] : nullptr, dm ? dm[t] : nullptr})
-            if (X && (X->nrows != n || X->ncols != n)) {
-                tl_error = "bfs_delta: operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-            }
-    if (is_huge(m[0])) { tl_error = "bfs_delta: host-resident operand"; return GrB_NOT_IMPLEMENTED; }
-    if (src >= n || (dest >= 0 && (u64)dest >= n)) { tl_error = "bfs_delta: src or dest out of range"; return GrB_INVALID_INDEX; }
-    GrB_Info info = device_ready();             // no device: fail before any host work
-    if (info) return info;
-    return guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (int t = 0; t < nops; t++) { all.push_back(m[t]); all.push_back(dp ? dp[t] : nullptr); all.push_back(dm ? dm[t] : nullptr); }
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        // the deltas that hold entries, on the device
-        std::vector<const DevCSR *> ddp(nops, nullptr), ddm(nops, nullptr);
-        bool clean = nops == 1;
-        for (int t = 0; t < nops; t++) {
-            GrB_Matrix P = dp ? dp[t] : nullptr, M = dm ? dm[t] : nullptr;
-            if (P && matrix_nvals(P)) { ensure_dev(P); ddp[t] = &P->dev; clean = false; }
-            if (M && matrix_nvals(M)) { ensure_dev(M); ddm[t] = &M->dev; clean = false; }
-        }
-        if (clean) {
-            ensure_devT(m[0]);
-            bfs_staged(m[0], &m[0]->devT, n, 0, nullptr, src, max_level, dest, level, parent, location, info_out);
-            return GrB_SUCCESS;
-        }
-        std::vector<DevCSR> dT(2 * nops);           // dp' and dm', built per call (the deltas change with every write)
-        std::vector<BfsOperand> ops(nops);
-        for (int t = 0; t < nops; t++) {
-            GrB_Matrix A = m[t];
-            ensure_devT(A);
-            if (!A->bfs_deg_valid) { bfs_build_degrees(A->dev, n, 0, n, nullptr, A->bfs_deg, &A->bfs_edges); A->bfs_deg_valid = true; }
-            if (ddp[t]) transpose_csr(*ddp[t], dT[2 * t], false);
-            if (ddm[t]) transpose_csr(*ddm[t], dT[2 * t + 1], false);
-            ops[t] = BfsOperand{&A->dev, &A->devT, ddp[t], ddp[t] ? &dT[2 * t] : nullptr, ddm[t], ddm[t] ? &dT[2 * t + 1] : nullptr,
-                                A->bfs_deg.ptr, A->bfs_edges};
-        }
-        DevBuf<u32> deg;
-        u64 total = 0;
-        bfs_delta_degrees(ops, n, deg, &total);
-        bfs_staged(m[0], nullptr, n, 0, nullptr, src, max_level, dest, level, parent, location, info_out, &ops, deg.ptr, total);
-        return GrB_SUCCESS;
-    });
-}
-
-// ---- the adjacency of algo.pageRank / algo.WCC / algo.labelPropagation over operands with pending writes ----
-// The reference builds it afresh on every call: build_adjacency_matrix or build_symmetric_adjacency_matrix, then dup + resize to
-// node_count + deleted_nodes_count (algo_procedures.rs:718-724, 816-822, 1207-1213), or, with a label filter, a host walk over every
-// edge of every named tensor remapped through a hash map (build_compact_adj_*_from_tensors, :535-670).  Here both are one device
-// call over the operands as they stand (effective_adjacency); only the kept rows of each layer are read.
-GrB_Info B200_adjacency_delta(GrB_Matrix *A, const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index n_out,
-                              const GrB_Index *keep, GrB_Index nkeep, int symmetric) {
-    CHECK_PTR(A);
-    GrB_Info info = union_check("adjacency_delta", m, dp, dm, nops);
-    if (info) return info;
-    const u64 n = m[0]->ncols;
-    if (keep) {
-        for (GrB_Index k = 0; k < nkeep; k++)
-            if (keep[k] >= n || (k && keep[k] <= keep[k - 1])) {
-                tl_error = "adjacency_delta: keep must be strictly ascending vertex ids below ncols(m)"; return GrB_INVALID_INDEX;
-            }
-    } else if (n_out >= ((u64)1 << 32)) {
-        tl_error = "adjacency_delta: n_out must be below 2^32"; return GrB_INVALID_VALUE;
-    }
-    info = device_ready();                       // no device: fail before any host work
-    if (info) return info;
-    std::vector<UnionOperand> ops = union_operands(m, dp, dm, nops);
-    return effective_adjacency(A, ops, n_out, keep, keep ? nkeep : 0, symmetric != 0);
-}
-
-// ---- relationship ids of a batch of rows (expand_row / bind_edge / ExpandInto's Tensor::get, cond_traverse.rs:663-702, 844-935,
-// expand_into.rs:121-258) in one call: edges.cu.  The me layers stay host-resident; their stores go to the device once per handle
-// and change (GB_Matrix_opaque::ids, dropped by invalidate_aux).
-static const DevIdStore *id_store(GrB_Matrix A) {
-    if (!A) return nullptr;
-    ensure_host(A);
-    if (!A->ids.valid) {
-        const HostStore &h = A->host;
-        A->ids.upload(h.hrow.data(), h.hptr.data(), h.hcol.data(), h.hrow.size());
-    }
-    return &A->ids;
-}
-
-GrB_Info B200_expand_edges(const GrB_Index *sources, const GrB_Index *targets, GrB_Index n, const B200_TensorLayers *types,
-                           int ntypes, int dir, int mode, uint64_t *out_p, uint32_t *out_node, uint64_t *out_edge,
-                           uint16_t *out_type, uint8_t *out_rev, uint64_t out_capacity, uint64_t *nout) {
-    CHECK_PTR(types); CHECK_PTR(out_p); CHECK_PTR(nout);
-    if (n) CHECK_PTR(sources);
-    if (out_capacity) { CHECK_PTR(out_node); CHECK_PTR(out_edge); }
-    if (ntypes < 1 || ntypes > 65536 || dir < B200_DIR_OUT || dir > B200_DIR_BOTH || mode < B200_EDGES_ALL || mode > B200_EDGES_FIRST) {
-        tl_error = "expand_edges: ntypes outside 1 .. 65536 (out_type is 16 bits), or dir / mode out of range"; return GrB_INVALID_VALUE;
-    }
-    for (int t = 0; t < ntypes; t++) {
-        const B200_TensorLayers &L = types[t];
-        CHECK_MAT(L.m);
-        for (GrB_Matrix X : {L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) if (X) CHECK_MAT(X);
-        if (dir != B200_DIR_OUT && !L.mt) { tl_error = "expand_edges: incoming edges need the transpose mt"; return GrB_NULL_POINTER; }
-        if (L.m->type != T_UINT64 || (L.dp && L.dp->type != T_UINT64)) {
-            tl_error = "expand_edges: the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
-        }
-    }
-    const u64 nv = types[0].m->nrows;
-    for (int t = 0; t < ntypes; t++) {
-        const B200_TensorLayers &L = types[t];
-        for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm})
-            if (X && (X->nrows != nv || X->ncols != nv)) {
-                tl_error = "expand_edges: forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-            }
-    }
-    if (is_huge(types[0].m)) { tl_error = "expand_edges: host-resident forward or transpose layers"; return GrB_NOT_IMPLEMENTED; }
-    for (u64 i = 0; i < n; i++)
-        if (sources[i] >= nv || (targets && targets[i] >= nv)) { tl_error = "expand_edges: vertex id out of range"; return GrB_INVALID_INDEX; }
-    GrB_Info info = device_ready();             // no device: fail before any host work
-    if (info) return info;
-    return guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (int t = 0; t < ntypes; t++) {
-            const B200_TensorLayers &L = types[t];
-            for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) all.push_back(X);
-        }
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
-        std::vector<EdgeTypeDev> td(ntypes);
-        for (int t = 0; t < ntypes; t++) {
-            const B200_TensorLayers &L = types[t];
-            const bool rev = dir != B200_DIR_OUT;
-            td[t] = EdgeTypeDev{dev(L.m), dev(L.dp), dev(L.dm), rev ? dev(L.mt) : nullptr, rev ? dev(L.mt_dp) : nullptr,
-                                rev ? dev(L.mt_dm) : nullptr, id_store(L.me), id_store(L.me_dp), id_store(L.me_dm)};
-        }
-        DevBuf<u64> ds(n), dtg(targets ? n : 0);
-        h2d(ds.ptr, (const u64 *)sources, n);
-        if (targets) h2d(dtg.ptr, (const u64 *)targets, n);
-        const u64 total = edge_expand(ds.ptr, targets ? dtg.ptr : nullptr, n, td, dir, mode, out_p, out_node, out_edge, out_type,
-                                      out_rev, out_capacity);
-        *nout = total;
-        if (total > out_capacity) { tl_error = "expand_edges: output capacity too small (*nout = entries needed)"; return GrB_INSUFFICIENT_SPACE; }
-        return GrB_SUCCESS;
-    });
-}
-
-// ---- CondVarLenTraverse's trails (cond_var_len_traverse.rs:152-386) for a batch of starts in one call: trails.cu.  The type
-// layers are read as B200_expand_edges reads them; the destination labels' (m, dp, dm) become one bitmap on the device.
-GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_Index nstarts, const B200_TensorLayers *types,
-                             int ntypes, int dir, uint64_t min_hops, uint64_t max_hops, const GrB_Matrix *lab_m,
-                             const GrB_Matrix *lab_dp, const GrB_Matrix *lab_dm, int nlabels, uint64_t tree_capacity,
-                             uint64_t *out_p, uint32_t *out_end, uint32_t *out_hops, uint64_t out_capacity,
-                             uint64_t *path_edge, uint32_t *path_node, uint64_t path_capacity, uint64_t *nout, uint64_t *npath) {
-    CHECK_PTR(types); CHECK_PTR(out_p); CHECK_PTR(nout); CHECK_PTR(npath);
-    if (nstarts) CHECK_PTR(starts);
-    if (out_end) CHECK_PTR(out_hops);
-    if (path_edge) CHECK_PTR(path_node);
-    if (ntypes < 1 || ntypes > 65536 || dir < B200_DIR_OUT || dir > B200_DIR_BOTH || nlabels < 0) {
-        tl_error = "var_len_trails: ntypes outside 1 .. 65536, dir out of range, or nlabels < 0"; return GrB_INVALID_VALUE;
-    }
-    if (nlabels) CHECK_PTR(lab_m);
-    for (int t = 0; t < ntypes; t++) {
-        const B200_TensorLayers &L = types[t];
-        CHECK_MAT(L.m);
-        for (GrB_Matrix X : {L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) if (X) CHECK_MAT(X);
-        if (dir != B200_DIR_OUT && !L.mt) { tl_error = "var_len_trails: incoming edges need the transpose mt"; return GrB_NULL_POINTER; }
-        if (L.m->type != T_UINT64 || (L.dp && L.dp->type != T_UINT64)) {
-            tl_error = "var_len_trails: the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
-        }
-    }
-    const u64 nv = types[0].m->nrows;
-    bool missing = false;
-    std::vector<GrB_Matrix> labs;                // (m, dp, dm) per present label
-    for (int k = 0; k < nlabels; k++) {
-        GrB_Matrix m = lab_m[k], dp = lab_dp ? lab_dp[k] : nullptr, dm = lab_dm ? lab_dm[k] : nullptr;
-        for (GrB_Matrix X : {m, dp, dm}) if (X) CHECK_MAT(X);
-        if (!m) { missing = true; continue; }
-        labs.insert(labs.end(), {m, dp, dm});
-    }
-    for (int t = 0; t < ntypes; t++) {
-        const B200_TensorLayers &L = types[t];
-        for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm})
-            if (X && (X->nrows != nv || X->ncols != nv)) {
-                tl_error = "var_len_trails: forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-            }
-    }
-    for (GrB_Matrix X : labs)
-        if (X && (X->nrows != nv || X->ncols != nv)) {
-            tl_error = "var_len_trails: label layers must be n x n"; return GrB_DIMENSION_MISMATCH;
-        }
-    if (is_huge(types[0].m)) { tl_error = "var_len_trails: host-resident forward or transpose layers"; return GrB_NOT_IMPLEMENTED; }
-    for (GrB_Matrix X : labs)
-        if (is_huge(X)) { tl_error = "var_len_trails: host-resident label layers"; return GrB_NOT_IMPLEMENTED; }
-    for (u64 i = 0; i < nstarts; i++)
-        if (starts[i] >= nv || (dests && dests[i] >= 0 && (u64)dests[i] >= nv)) {
-            tl_error = "var_len_trails: start or destination out of range"; return GrB_INVALID_INDEX;
-        }
-    if (nstarts == 0 || min_hops > max_hops) {
-        for (u64 i = 0; i <= nstarts; i++) out_p[i] = 0;
-        *nout = 0; *npath = 0;
-        return GrB_SUCCESS;
-    }
-    GrB_Info info = device_ready();             // no device: fail before any host work
-    if (info) return info;
-    return guarded([&]() {
-        GpuLock g;
-        uvec<GrB_Matrix> all;
-        for (int t = 0; t < ntypes; t++) {
-            const B200_TensorLayers &L = types[t];
-            for (GrB_Matrix X : {L.m, L.dp, L.dm, L.mt, L.mt_dp, L.mt_dm, L.me, L.me_dp, L.me_dm}) all.push_back(X);
-        }
-        for (GrB_Matrix X : labs) all.push_back(X);
-        MultiLock lk(all.begin(), all.end());
-        ensure_init();
-        if (missing) {                           // a label the graph lacks: every trail is walked, none emits (:162, :316)
-            for (u64 i = 0; i <= nstarts; i++) out_p[i] = 0;
-            *nout = 0; *npath = 0;
-            return GrB_SUCCESS;
-        }
-        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
-        std::vector<EdgeTypeDev> td(ntypes);
-        for (int t = 0; t < ntypes; t++) {
-            const B200_TensorLayers &L = types[t];
-            const bool rev = dir != B200_DIR_OUT;
-            td[t] = EdgeTypeDev{dev(L.m), dev(L.dp), dev(L.dm), rev ? dev(L.mt) : nullptr, rev ? dev(L.mt_dp) : nullptr,
-                                rev ? dev(L.mt_dm) : nullptr, id_store(L.me), id_store(L.me_dp), id_store(L.me_dm)};
-        }
-        std::vector<LabelDev> ld;
-        for (size_t k = 0; k < labs.size(); k += 3) ld.push_back(LabelDev{dev(labs[k]), dev(labs[k + 1]), dev(labs[k + 2])});
-        TrailsOut o{out_p, out_end, out_hops, path_edge, path_node, out_capacity, path_capacity};
-        const int r = var_len_trails((const u64 *)starts, (const i64 *)dests, nstarts, td, dir, min_hops, max_hops, ld, nv, tree_capacity, o);
-        if (r == 2) {
-            *nout = *npath = UINT64_MAX;
-            tl_error = "var_len_trails: the stored trail tree would exceed tree_capacity entries";
-            return GrB_INSUFFICIENT_SPACE;
-        }
-        *nout = o.nout; *npath = o.npath;
-        if (r == 1) { tl_error = "var_len_trails: output capacity too small (*nout / *npath = what is needed)"; return GrB_INSUFFICIENT_SPACE; }
-        return GrB_SUCCESS;
-    });
-}
-
-// ---- the read phase of a Tensor's relationship inserts and deletes (set_all_from_slices / remove_all, tensor.rs:333-629) for a
-// whole batch in one call: writes.cu.  Only reads the layers; their pending tuples are finished like any device read's.
-static_assert(B200_PLAN_COMMITTED == WP_COMMITTED && B200_PLAN_CANCEL == WP_CANCEL && B200_PLAN_MT_BASE == WP_MT_BASE &&
-              B200_PLAN_EMPTIED == WP_EMPTIED && B200_PLAN_DEMOTED == WP_DEMOTED && B200_PLAN_M_HAS == WP_M_HAS &&
-              B200_PLAN_M_EQ == WP_M_EQ, "plan flags");
-
-static GrB_Info write_plan(const char *what, bool insert, const B200_TensorLayers *t, const GrB_Index *a, const GrB_Index *b,
-                           const GrB_Index *c, GrB_Index n, uint64_t *rec_src, uint64_t *rec_dst, uint64_t *rec_val,
-                           uint8_t *rec_flags, uint64_t *nrec, uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
-    CHECK_PTR(t); CHECK_PTR(nrec); CHECK_PTR(nme);
-    if (n) {
-        CHECK_PTR(a); CHECK_PTR(b); CHECK_PTR(c);
-        CHECK_PTR(rec_src); CHECK_PTR(rec_dst); CHECK_PTR(rec_val); CHECK_PTR(rec_flags);
-        CHECK_PTR(me_key); CHECK_PTR(me_id); CHECK_PTR(me_base);
-    }
-    CHECK_MAT(t->m);
-    CHECK_MAT(t->mt);
-    for (GrB_Matrix X : {t->dp, t->dm, t->mt_dp, t->mt_dm, t->me, t->me_dp, t->me_dm}) if (X) CHECK_MAT(X);
-    if (t->m->type != T_UINT64 || (t->dp && t->dp->type != T_UINT64)) {
-        tl_error = std::string(what) + ": the forward layers m / dp must be UINT64 (edge ids)"; return GrB_DOMAIN_MISMATCH;
-    }
-    const u64 nv = t->m->nrows;
-    for (GrB_Matrix X : {t->m, t->dp, t->dm, t->mt, t->mt_dp, t->mt_dm})
-        if (X && (X->nrows != nv || X->ncols != nv)) {
-            tl_error = std::string(what) + ": forward and transpose layers must be square and equally sized"; return GrB_DIMENSION_MISMATCH;
-        }
-    if (is_huge(t->m)) { tl_error = std::string(what) + ": host-resident forward layers"; return GrB_NOT_IMPLEMENTED; }
-    // insert: (a, b, c) = (srcs, dsts, ids); remove: (ids, srcs, dsts)
-    const GrB_Index *src = insert ? a : b, *dst = insert ? b : c, *ids = insert ? c : a;
-    for (u64 k = 0; k < n; k++)
-        if (src[k] >= nv || dst[k] >= nv || ids[k] >= ((u64)1 << 60)) {
-            tl_error = std::string(what) + ": a vertex id >= n or an edge id >= 2^60"; return GrB_INVALID_INDEX;
-        }
-    *nrec = 0; *nme = 0;
-    if (n == 0) return GrB_SUCCESS;
-    GrB_Info info = device_ready();             // no device: fail before any host work
-    if (info) return info;
-    return guarded([&]() {
-        GpuLock g;
-        MultiLock lk{t->m, t->dp, t->dm, t->mt, t->mt_dp, t->mt_dm, t->me, t->me_dp, t->me_dm};
-        ensure_init();
-        auto dev = [&](GrB_Matrix X) -> const DevCSR * { if (!X) return nullptr; ensure_dev(X); return &X->dev; };
-        const EdgeTypeDev td{dev(t->m), dev(t->dp), dev(t->dm), dev(t->mt), nullptr, nullptr, id_store(t->me),
-                             insert ? nullptr : id_store(t->me_dp), insert ? nullptr : id_store(t->me_dm)};
-        DevBuf<u64> ds(n), dd(n), di(n);
-        h2d(ds.ptr, (const u64 *)src, n);
-        h2d(dd.ptr, (const u64 *)dst, n);
-        h2d(di.ptr, (const u64 *)ids, n);
-        WritePlan P{rec_src, rec_dst, rec_val, rec_flags, 0, me_key, me_id, me_base, 0};
-        if (insert) tensor_insert_plan(td, ds.ptr, dd.ptr, di.ptr, n, nv, P);
-        else tensor_remove_plan(td, di.ptr, ds.ptr, dd.ptr, n, nv, P);
-        *nrec = P.nrec; *nme = P.nme;
-        return GrB_SUCCESS;
-    });
-}
-
-GrB_Info B200_Tensor_insert_plan(const B200_TensorLayers *t, const GrB_Index *srcs, const GrB_Index *dsts, const GrB_Index *ids,
-                                 GrB_Index n, uint64_t *in_src, uint64_t *in_dst, uint64_t *in_val, uint8_t *in_flags, uint64_t *nin,
-                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
-    return write_plan("insert_plan", true, t, srcs, dsts, ids, n, in_src, in_dst, in_val, in_flags, nin, me_key, me_id, me_base, nme);
-}
-GrB_Info B200_Tensor_remove_plan(const B200_TensorLayers *t, const GrB_Index *ids, const GrB_Index *srcs, const GrB_Index *dsts,
-                                 GrB_Index n, uint64_t *pr_src, uint64_t *pr_dst, uint64_t *pr_val, uint8_t *pr_flags, uint64_t *npr,
-                                 uint64_t *me_key, uint64_t *me_id, uint8_t *me_base, uint64_t *nme) {
-    return write_plan("remove_plan", false, t, ids, srcs, dsts, n, pr_src, pr_dst, pr_val, pr_flags, npr, me_key, me_id, me_base, nme);
-}
 
 // returns every cached device block to the driver (the caching allocator otherwise keeps freed blocks for reuse)
 GrB_Info B200_pool_trim(void) {

@@ -128,14 +128,7 @@ struct EdgeExpansion {
 inline EdgeExpansion expand_edges(const std::vector<uint64_t> &srcs, const std::vector<uint64_t> *targets,
                                   const std::vector<const Tensor *> &types, int dir, int mode) {
     std::vector<B200_TensorLayers> ls;
-    for (const Tensor *t : types) {
-        t->wait();
-        t->fwd_m().wait(); t->fwd_dp().wait(); t->fwd_dm().wait();
-        const VersionedMatrix &mt = t->matrix_t(), &me = t->edge_versioned();
-        mt.wait_all(); me.wait_all();
-        ls.push_back(B200_TensorLayers{t->fwd_m().inner(), t->fwd_dp().inner(), t->fwd_dm().inner(), mt.m().inner(), mt.dp().inner(),
-                                       mt.dm().inner(), me.m().inner(), me.dp().inner(), me.dm().inner()});
-    }
+    for (const Tensor *t : types) ls.push_back(t->waited_layers());
     EdgeExpansion r;
     const size_t n = srcs.size();
     r.p.assign(n + 1, 0);

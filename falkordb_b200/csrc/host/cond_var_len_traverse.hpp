@@ -214,14 +214,7 @@ inline VarLenBatch var_len_trails(const std::vector<const Tensor *> &types, Edge
                                   const std::vector<const VersionedMatrix *> &labels, bool emit_path,
                                   uint64_t tree_capacity = UINT64_MAX) {
     std::vector<B200_TensorLayers> ls;
-    for (const Tensor *t : types) {
-        t->wait();
-        t->fwd_m().wait(); t->fwd_dp().wait(); t->fwd_dm().wait();
-        const VersionedMatrix &mt = t->matrix_t(), &me = t->edge_versioned();
-        mt.wait_all(); me.wait_all();
-        ls.push_back(B200_TensorLayers{t->fwd_m().inner(), t->fwd_dp().inner(), t->fwd_dm().inner(), mt.m().inner(), mt.dp().inner(),
-                                       mt.dm().inner(), me.m().inner(), me.dp().inner(), me.dm().inner()});
-    }
+    for (const Tensor *t : types) ls.push_back(t->waited_layers());
     std::vector<GrB_Matrix> lm, ldp, ldm;
     for (const VersionedMatrix *l : labels) {
         if (l) { l->wait(); l->wait_all(); }

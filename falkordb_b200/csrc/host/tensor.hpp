@@ -217,6 +217,13 @@ class Tensor {
         return B200_TensorLayers{fwd_m().inner(), fwd_dp().inner(), fwd_dm().inner(), mt_.m().inner(), mt_.dp().inner(), mt_.dm().inner(),
                                  me_.m().inner(), me_.dp().inner(), me_.dm().inner()};
     }
+    // layers() once every layer's pending work is applied, as B200_expand_edges and B200_var_len_trails read them
+    B200_TensorLayers waited_layers() const {
+        wait();
+        fwd_m().wait(); fwd_dp().wait(); fwd_dm().wait();
+        mt_.wait_all(); me_.wait_all();
+        return layers();
+    }
     // the six Delta counters: dp, dm, mt's dp, dm, me's dp, dm
     void counts(uint64_t *out6) const {
         out6[0] = dp_.get_count(); out6[1] = dm_.get_count();

@@ -44,6 +44,16 @@ def _u64arr(a):
     return np.ascontiguousarray(a, dtype=np.uint64)
 
 
+def _operands(ms, deltas):
+    """(m, dp, dm, n): the handle arrays of operands `ms` and of their deltas, one (dp, dm) pair per operand (either may be None;
+    `deltas` None: no pending writes)."""
+    n = len(ms)
+    deltas = [(None, None)] * n if deltas is None else list(deltas)
+    assert len(deltas) == n, "one (dp, dm) pair per operand"
+    arr = lambda xs: (C.c_void_p * max(1, n))(*[None if x is None else x.h for x in xs])
+    return arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), n
+
+
 class Matrix:
     """``Matrix<bool>`` (dtype=bool) or ``Matrix<u64>`` (dtype='u64')."""
 
@@ -275,11 +285,7 @@ class Matrix:
     def union_lmxm(self, ms, deltas=None):
         """B200_Matrix_union_lmxm: the union hop of `-[:R1|R2]->`, self <- self * U_t (ms[t] \\ dm_t) u dp_t, exact (no
         delta_lmxm over-masking, also for one operand).  `deltas`: one (dp, dm) pair per operand, either may be None."""
-        n = len(ms)
-        deltas = [(None, None)] * n if deltas is None else list(deltas)
-        assert len(deltas) == n, "one (dp, dm) pair per operand"
-        arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
-        check(lib().B200_Matrix_union_lmxm(self.h, arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), n))
+        check(lib().B200_Matrix_union_lmxm(self.h, *_operands(ms, deltas)))
 
     def element_wise_add(self, mask=None, a=None, b=None, descriptor=None):
         op = obj("GxB_ANY_BOOL") if self.dtype is bool else obj("GrB_SECOND_UINT64")
@@ -406,16 +412,13 @@ def bfs(A, src, max_level=-1, want_parent=True, deltas=None, dest=-1, info=None)
                              C.byref(edges)))
         return level, parent, edges.value
     ms = [A] if isinstance(A, Matrix) else list(A)
-    k = len(ms)
-    deltas = [(None, None)] * k if deltas is None else list(deltas)
-    assert len(deltas) == k, "one (dp, dm) pair per operand"
+    ops = _operands(ms, deltas)
     n = ms[0].nrows()
     level = np.empty(n, np.int64)
     parent = np.empty(n, np.int64) if want_parent else None
     rec = BfsInfo() if info is None else info
-    arr = lambda xs: (C.c_void_p * k)(*[None if x is None else x.h for x in xs])
-    check(lib().B200_bfs_delta(arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), k, src, max_level, dest,
-                               level.ctypes.data, None if parent is None else parent.ctypes.data, 0, C.byref(rec)))
+    check(lib().B200_bfs_delta(*ops, src, max_level, dest, level.ctypes.data, None if parent is None else parent.ctypes.data, 0,
+                               C.byref(rec)))
     return level, parent, rec.edges
 
 
@@ -470,19 +473,14 @@ def traverse_batch(sources, hop_matrices, fmt=OUT_AUTO, out_bitmap=None, out_p=N
             pairs += d
             nops.append(len(group))
             union.append(1 if isinstance(h, (list, tuple)) else 0)
-        n = len(ms)
-        arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
         info = lib().B200_traverse_batch_union(sources.ctypes.data, len(sources), (C.c_int * nh)(*nops), (C.c_int * nh)(*union), nh,
-                                               arr(ms), arr([d[0] for d in pairs]), arr([d[1] for d in pairs]), *outs)
+                                               *_operands(ms, pairs)[:3], *outs)
     elif deltas is None:
         hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
         info = lib().B200_traverse_batch(sources.ctypes.data, len(sources), hs, nh, *outs)
     else:
         assert len(deltas) == nh, "one (dp, dm) pair per hop"
-        dps = (C.c_void_p * nh)(*[None if d[0] is None else d[0].h for d in deltas])
-        dms = (C.c_void_p * nh)(*[None if d[1] is None else d[1].h for d in deltas])
-        hs = (C.c_void_p * nh)(*[m.h for m in hop_matrices])
-        info = lib().B200_traverse_batch_delta(sources.ctypes.data, len(sources), hs, dps, dms, nh, *outs)
+        info = lib().B200_traverse_batch_delta(sources.ctypes.data, len(sources), *_operands(hop_matrices, deltas), *outs)
     if info == -103:                     # GrB_INSUFFICIENT_SPACE: nv holds the entries needed
         raise BufferError(f"out_j holds {0 if out_j is None else len(out_j)} entries, the result has {nv.value}")
     check(info)
@@ -508,12 +506,8 @@ def reach_batch(sources, A, max_hops=None, include_sources=False, deltas=None):
                                      C.byref(lv)))
         return Matrix(0, 0, bool, _handle=h), lv.value
     ms = [A] if isinstance(A, Matrix) else list(A)
-    n = len(ms)
-    deltas = [(None, None)] * n if deltas is None else list(deltas)
-    assert len(deltas) == n, "one (dp, dm) pair per operand"
-    arr = lambda xs: (C.c_void_p * n)(*[None if x is None else x.h for x in xs])
-    check(lib().B200_reach_batch_delta(C.byref(h), sources.ctypes.data, len(sources), arr(ms), arr([d[0] for d in deltas]),
-                                       arr([d[1] for d in deltas]), n, hops, 1 if include_sources else 0, C.byref(lv)))
+    check(lib().B200_reach_batch_delta(C.byref(h), sources.ctypes.data, len(sources), *_operands(ms, deltas), hops,
+                                       1 if include_sources else 0, C.byref(lv)))
     return Matrix(0, 0, bool, _handle=h), lv.value
 
 
@@ -523,14 +517,9 @@ def adjacency(ms, deltas=None, n=None, keep=None, symmetric=False):
     restricted to the vertices below `n` (default ncols) or, given `keep` (strictly ascending ids), to those, renumbered 0 ..
     len(keep) - 1.  `symmetric`: that union with its transpose."""
     ms = [ms] if isinstance(ms, Matrix) else list(ms)
-    k = len(ms)
-    deltas = [(None, None)] * k if deltas is None else list(deltas)
-    assert len(deltas) == k, "one (dp, dm) pair per operand"
-    arr = lambda xs: (C.c_void_p * max(1, k))(*[None if x is None else x.h for x in xs])
     kp = None if keep is None else _u64arr(keep)
     h = P()
-    check(lib().B200_adjacency_delta(C.byref(h), arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), k,
-                                     (ms[0].ncols() if k else 0) if n is None else int(n),
+    check(lib().B200_adjacency_delta(C.byref(h), *_operands(ms, deltas), (ms[0].ncols() if ms else 0) if n is None else int(n),
                                      None if kp is None else kp.ctypes.data, 0 if kp is None else len(kp), 1 if symmetric else 0))
     return Matrix(0, 0, bool, _handle=h)
 
@@ -579,6 +568,16 @@ def _handle(x):
     return None if x is None else (x.h if isinstance(x, Matrix) else x)
 
 
+def _layers(types):
+    """a B200_TensorLayers array, one entry per type: a sequence or dict of the nine layers in TENSOR_LAYERS order"""
+    ls = (TensorLayers * max(1, len(types)))()
+    for k, t in enumerate(types):
+        vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
+        for name, x in zip(TENSOR_LAYERS, vals):
+            setattr(ls[k], name, _handle(x))
+    return ls
+
+
 def expand_edges(sources, types, dir=DIR_OUT, mode=EDGES_ALL, targets=None, capacity=None):
     """B200_expand_edges: the relationships of a batch of rows over relationship types, in one call.  `types`: one entry per type,
     a sequence or dict of the nine layers in TENSOR_LAYERS order (Matrix, raw handle or None; m required, mt for DIR_IN / DIR_BOTH).
@@ -590,11 +589,7 @@ def expand_edges(sources, types, dir=DIR_OUT, mode=EDGES_ALL, targets=None, capa
     if targets is not None:
         targets = _u64arr(targets)
         assert len(targets) == n, "one target per source"
-    ls = (TensorLayers * max(1, len(types)))()
-    for k, t in enumerate(types):
-        vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
-        for name, x in zip(TENSOR_LAYERS, vals):
-            setattr(ls[k], name, _handle(x))
+    ls = _layers(types)
     cap = max(1024, 4 * n) if capacity is None else int(capacity)
     p, nv = np.zeros(n + 1, np.uint64), U64(0)
     for attempt in (0, 1):
@@ -615,14 +610,6 @@ def expand_edges(sources, types, dir=DIR_OUT, mode=EDGES_ALL, targets=None, capa
 PLAN_COMMITTED, PLAN_CANCEL, PLAN_MT_BASE, PLAN_EMPTIED, PLAN_DEMOTED, PLAN_M_HAS, PLAN_M_EQ = 1, 2, 4, 8, 16, 32, 64
 
 
-def _layers1(t):
-    ls = TensorLayers()
-    vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
-    for name, x in zip(TENSOR_LAYERS, vals):
-        setattr(ls, name, _handle(x))
-    return ls
-
-
 def _plan(fn, t, a, b, c):
     a, b, c = _u64arr(a), _u64arr(b), _u64arr(c)
     n = len(a)
@@ -630,7 +617,7 @@ def _plan(fn, t, a, b, c):
     rs, rd, rv, rf = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint8)
     mk, mi, mb = np.zeros(max(2 * n, 1), np.uint64), np.zeros(max(2 * n, 1), np.uint64), np.zeros(max(2 * n, 1), np.uint8)
     nr, nm = U64(0), U64(0)
-    check(fn(C.byref(_layers1(t)), a.ctypes.data if n else None, b.ctypes.data if n else None, c.ctypes.data if n else None, n,
+    check(fn(_layers([t]), a.ctypes.data if n else None, b.ctypes.data if n else None, c.ctypes.data if n else None, n,
              rs.ctypes.data, rd.ctypes.data, rv.ctypes.data, rf.ctypes.data, C.byref(nr), mk.ctypes.data, mi.ctypes.data, mb.ctypes.data,
              C.byref(nm)))
     r, m = nr.value, nm.value
@@ -662,11 +649,7 @@ def var_len_trails(starts, types, dir=DIR_OUT, min_hops=1, max_hops=None, dests=
     n = len(starts)
     ds = None if dests is None else np.ascontiguousarray(dests, dtype=np.int64)
     assert ds is None or len(ds) == n, "one destination per start"
-    ls = (TensorLayers * max(1, len(types)))()
-    for k, t in enumerate(types):
-        vals = [t.get(name) for name in TENSOR_LAYERS] if isinstance(t, dict) else list(t) + [None] * (9 - len(t))
-        for name, x in zip(TENSOR_LAYERS, vals):
-            setattr(ls[k], name, _handle(x))
+    ls = _layers(types)
     nl = len(labels)
     lm, ldp, ldm = (P * max(1, nl))(), (P * max(1, nl))(), (P * max(1, nl))()
     for k, lab in enumerate(labels):
