@@ -830,8 +830,23 @@ __global__ void __launch_bounds__(256) k_or_all(const u64 *__restrict__ X, u64 n
     }
 }
 
-template <bool HINTS> __device__ __forceinline__ u32 ld_col(const u32 *p, u64 strm) { return HINTS ? ld_u32_stream(p, strm) : __ldg(p); }
-template <bool HINTS> __device__ __forceinline__ u64 ld_x(const u64 *p, u64 keep) { return HINTS ? ld_u64_hint(p, keep) : __ldg(p); }
+// The L2 policies of one pull launch with hints on.  The gather source X (the packed frontier, hot-set order: out-degree
+// descending) is evict_last over its first `hot` bytes and evict_first over the rest of its `tot` bytes, or evict_normal
+// everywhere when hot = 0.  streams != 0: A' col_idx and rowptr, the segment list and the stores of Y are evict_first, so the
+// 2 GB that pass through once do not push the hot records out.
+struct PullHints {
+    u32 hot = 0, tot = 0, streams = 0;
+#ifdef __CUDACC__
+    __device__ __forceinline__ u64 gather_policy(const void *X) const { return hot ? policy_range(X, hot, tot) : policy_normal(); }
+    __device__ __forceinline__ u64 stream_policy() const { return streams ? policy_stream() : policy_normal(); }
+#endif
+};
+
+// HINTS: every load of the pull kernels carries an L2 policy (PullHints).  A' col_idx and rowptr lines are shared by the loads of
+// neighbouring lanes and unroll steps, so they keep their L1 allocation; only their L2 priority changes
+template <bool HINTS> __device__ __forceinline__ u32 ld_col(const u32 *p, u64 strm) { return HINTS ? ld_nc_u32(p, strm) : __ldg(p); }
+template <bool HINTS> __device__ __forceinline__ u64 ld_ptr(const u64 *p, u64 strm) { return HINTS ? ld_nc_u64(p, strm) : __ldg(p); }
+template <bool HINTS> __device__ __forceinline__ u64 ld_x(const u64 *p, u64 keep) { return HINTS ? ld_nc_u64(p, keep) : __ldg(p); }
 // acc |= the W frontier words of one vertex: ONE 16-byte load per word pair (a W=4 vertex is a single 32 B sector), so the
 // number of L1TEX wavefronts per gathered vertex does not grow with W
 template <int W, bool HINTS> __device__ __forceinline__ void or_words(u64 (&acc)[W], const u64 *__restrict__ p, u64 keep) {
@@ -839,7 +854,7 @@ template <int W, bool HINTS> __device__ __forceinline__ void or_words(u64 (&acc)
     const ulonglong2 *q = reinterpret_cast<const ulonglong2 *>(p);
 #pragma unroll
     for (int w2 = 0; w2 < W / 2; w2++) {
-        ulonglong2 v = HINTS ? ld_v2_hint(q + w2, keep) : __ldg(q + w2);
+        ulonglong2 v = HINTS ? ld_nc_v2(q + w2, keep) : __ldg(q + w2);
         acc[2 * w2] |= v.x;
         acc[2 * w2 + 1] |= v.y;
     }
@@ -847,14 +862,23 @@ template <int W, bool HINTS> __device__ __forceinline__ void or_words(u64 (&acc)
 
 static const u32 SMALL_ROW = 8;
 
-template <int W> __device__ __forceinline__ void store_row(u64 *dst, const u64 (&acc)[W]) {
-    if constexpr (W == 1) { dst[0] = acc[0]; }
-    else {
+// HINTS: the store carries policy pol (Y is written once and read by the next pass, not by this kernel)
+template <int W, bool HINTS = false> __device__ __forceinline__ void store_row(u64 *dst, const u64 (&acc)[W], u64 pol = 0) {
+    if constexpr (W == 1) {
+        if (HINTS) st_u64_stream(dst, acc[0], pol);
+        else dst[0] = acc[0];
+    } else {
 #pragma unroll
-        for (int w2 = 0; w2 < W / 2; w2++) reinterpret_cast<ulonglong2 *>(dst)[w2] = make_ulonglong2(acc[2 * w2], acc[2 * w2 + 1]);
+        for (int w2 = 0; w2 < W / 2; w2++) {
+            ulonglong2 *q = reinterpret_cast<ulonglong2 *>(dst) + w2;
+            if (HINTS) st_v2_hint(q, make_ulonglong2(acc[2 * w2], acc[2 * w2 + 1]), pol);
+            else *q = make_ulonglong2(acc[2 * w2], acc[2 * w2 + 1]);
+        }
     }
 }
-template <int WL> __device__ __forceinline__ void store_part(u64 *dst, const u64 (&acc)[WL]) { store_row<WL>(dst, acc); }
+template <int WL, bool HINTS = false> __device__ __forceinline__ void store_part(u64 *dst, const u64 (&acc)[WL], u64 pol = 0) {
+    store_row<WL, HINTS>(dst, acc, pol);
+}
 // accumulate mode (union hops): dst |= acc, skipped when acc is empty.  Each record is owned by one lane (k_pull_small) or one
 // 8-lane group (a mid row of k_pull_seg), so a plain read-modify-write is race-free
 template <int WL> __device__ __forceinline__ void or_part(u64 *dst, u64 (&acc)[WL]) {
@@ -947,23 +971,23 @@ static void build_seg_list(const DevCSR &AT, PullTables &pt) {
 template <int W, bool HINTS, bool ACC>
 __global__ void __launch_bounds__(256)
 k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, const u64 *__restrict__ X,
-             u64 *__restrict__ Y, u32 hot_bytes, u32 tot_bytes) {
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0;
+             u64 *__restrict__ Y, PullHints ph) {
+    const u64 keep = HINTS ? ph.gather_policy(X) : 0, strm = HINTS ? ph.stream_policy() : 0;
     u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const u64 stride = (u64)gridDim.x * blockDim.x;
     // three-stage pipeline per lane: row pointers two rows ahead, first col_idx batch one row ahead, gathers now
     u64 s = 0, e = 0, s1 = 0, e1 = 0;
-    if (j < n) { s = __ldg(ATp + j); e = __ldg(ATp + j + 1); }
-    if (j + stride < n) { s1 = __ldg(ATp + j + stride); e1 = __ldg(ATp + j + stride + 1); }
+    if (j < n) { s = ld_ptr<HINTS>(ATp + j, strm); e = ld_ptr<HINTS>(ATp + j + 1, strm); }
+    if (j + stride < n) { s1 = ld_ptr<HINTS>(ATp + j + stride, strm); e1 = ld_ptr<HINTS>(ATp + j + stride + 1, strm); }
     u32 k[4];
 #pragma unroll
-    for (int u = 0; u < 4; u++) k[u] = (e - s <= SMALL_ROW && s + u < e) ? __ldg(ATj + s + u) : 0xFFFFFFFFu;
+    for (int u = 0; u < 4; u++) k[u] = (e - s <= SMALL_ROW && s + u < e) ? ld_col<HINTS>(ATj + s + u, strm) : 0xFFFFFFFFu;
     for (; j < n; j += stride) {
         u64 s2 = 0, e2 = 0;
-        if (j + 2 * stride < n) { s2 = __ldg(ATp + j + 2 * stride); e2 = __ldg(ATp + j + 2 * stride + 1); }
+        if (j + 2 * stride < n) { s2 = ld_ptr<HINTS>(ATp + j + 2 * stride, strm); e2 = ld_ptr<HINTS>(ATp + j + 2 * stride + 1, strm); }
         u32 kn[4];
 #pragma unroll
-        for (int u = 0; u < 4; u++) kn[u] = (e1 - s1 <= SMALL_ROW && s1 + u < e1) ? __ldg(ATj + s1 + u) : 0xFFFFFFFFu;
+        for (int u = 0; u < 4; u++) kn[u] = (e1 - s1 <= SMALL_ROW && s1 + u < e1) ? ld_col<HINTS>(ATj + s1 + u, strm) : 0xFFFFFFFFu;
         u64 acc[W];
 #pragma unroll
         for (int w = 0; w < W; w++) acc[w] = 0;
@@ -973,14 +997,14 @@ k_pull_small(const u64 *__restrict__ ATp, const u32 *__restrict__ ATj, u64 n, co
                 if (k[u] != 0xFFFFFFFFu) or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
             if (e - s > 4) {
 #pragma unroll
-                for (int u = 0; u < 4; u++) k[u] = (s + 4 + u < e) ? __ldg(ATj + s + 4 + u) : 0xFFFFFFFFu;
+                for (int u = 0; u < 4; u++) k[u] = (s + 4 + u < e) ? ld_col<HINTS>(ATj + s + 4 + u, strm) : 0xFFFFFFFFu;
 #pragma unroll
                 for (int u = 0; u < 4; u++)
                     if (k[u] != 0xFFFFFFFFu) or_words<W, HINTS>(acc, X + (u64)k[u] * W, keep);
             }
         }
         if (ACC) { if (e - s <= SMALL_ROW) or_part<W>(Y + j * W, acc); }
-        else if (e - s <= SMALL_ROW || e - s > LONG_ROW) store_row<W>(Y + j * W, acc);
+        else if (e - s <= SMALL_ROW || e - s > LONG_ROW) store_row<W, HINTS>(Y + j * W, acc, strm);
 #pragma unroll
         for (int u = 0; u < 4; u++) k[u] = kn[u];
         s = s1; e = e1; s1 = s2; e1 = e2;
@@ -996,14 +1020,14 @@ template <int W, bool HINTS, int U, bool EARLY, bool ACC>
 __global__ void __launch_bounds__(256)
 k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const u32 *__restrict__ s_len, u64 ns,
            const u32 *__restrict__ ATj, const u64 *__restrict__ X, u64 *__restrict__ Y, const u64 *__restrict__ Gp,
-           u32 hot_bytes, u32 tot_bytes) {
+           PullHints ph) {
     constexpr int WL = PullCfg<W>::WL, SPLIT = PullCfg<W>::SPLIT, VG = PullCfg<W>::VG;
     const u32 lane8 = threadIdx.x & 7;
     const u32 sub = (threadIdx.x & 31) >> 3;
     const u32 gmask = 0xFFu << (8 * sub);
     const u32 vi = lane8 / SPLIT, h = lane8 % SPLIT;
     const u64 *Xh = X + h * WL;
-    const u64 keep = HINTS ? policy_range(X, hot_bytes, tot_bytes) : 0, strm = policy_stream();
+    const u64 keep = HINTS ? ph.gather_policy(X) : 0, strm = HINTS ? ph.stream_policy() : 0;
     u64 G[WL];
 #pragma unroll
     for (int w = 0; w < WL; w++) G[w] = (EARLY && Gp) ? Gp[h * WL + w] : ~0ULL;
@@ -1013,7 +1037,13 @@ k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const
     auto entry = [&](u64 t) -> u64 { return t * ngroups + ((t & 1) ? ngroups - 1 - g : g); };
     auto fetch = [&](u64 t, u64 &s, u64 &e) {
         s = 0; e = 0;
-        if (t < steps) { u64 i = entry(t); if (i < ns) { s = s_start[i]; e = s + (s_len[i] & ~SEG_ATOMIC); } }
+        if (t < steps) {
+            u64 i = entry(t);
+            if (i < ns) {   // each entry is fetched once: with hints its lines skip L1
+                s = HINTS ? ld_nc_once_u64(s_start + i, strm) : s_start[i];
+                e = s + ((HINTS ? ld_nc_once_u32(s_len + i, strm) : s_len[i]) & ~SEG_ATOMIC);
+            }
+        }
     };
     u64 s0, e0, s1, e1;
     fetch(0, s0, e0);
@@ -1075,12 +1105,12 @@ k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const
         }
         if (e0 > s0 && vi == 0) {
             const u64 i = entry(t);
-            u64 *dst = Y + (u64)s_row[i] * W + h * WL;
-            if (s_len[i] & SEG_ATOMIC) {
+            u64 *dst = Y + (u64)(HINTS ? ld_nc_once_u32(s_row + i, strm) : s_row[i]) * W + h * WL;
+            if ((HINTS ? ld_nc_once_u32(s_len + i, strm) : s_len[i]) & SEG_ATOMIC) {
 #pragma unroll
                 for (int w = 0; w < WL; w++) if (acc[w]) atomicOr((unsigned long long *)(dst + w), acc[w]);
             } else if (ACC) or_part<WL>(dst, acc);
-            else store_part<WL>(dst, acc);
+            else store_part<WL, HINTS>(dst, acc, strm);
         }
         s0 = s1; e0 = e1; s1 = s2; e1 = e2;
     }
@@ -1090,25 +1120,32 @@ k_pull_seg(const u32 *__restrict__ s_row, const u64 *__restrict__ s_start, const
 // The pull gathers X[k] with k distributed like the out-degree of k.  Relabel k -> slot, slots ordered by out-degree
 // descending and restricted to vertices that have out-edges at all (sinks are never gathered): the hot part of the
 // frontier words becomes contiguous (L1/L2 resident), and the gather footprint shrinks from 8*W*n to 8*W*n1 bytes.
-__global__ void k_degree_keys(const u64 *__restrict__ Ap, u64 n, u64 *__restrict__ keys, u64 *__restrict__ n1) {
+// shuffle (measurement, hot_shuffle): vertices with out-edges in the order of a hash of their id instead, so the gather
+// source has no hot prefix at all; sinks stay last either way
+__global__ void k_degree_keys(const u64 *__restrict__ Ap, u64 n, u64 *__restrict__ keys, u64 *__restrict__ n1, bool shuffle) {
     u64 v = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
     u64 cnt = 0;
     for (; v < n; v += stride) {
         u64 d = Ap[v + 1] - Ap[v];
         if (d > 0xFFFFFFFEULL) d = 0xFFFFFFFEULL;
-        keys[v] = ((0xFFFFFFFFULL - d) << 32) | v;   // ascending sort => degree descending, then vertex id ascending
+        u64 hi = 0xFFFFFFFFULL - d;
+        if (shuffle && d) { u32 h = (u32)v * 0x9E3779B1u; h ^= h >> 15; h *= 0x85EBCA77u; h ^= h >> 13; hi = h >> 1; }
+        keys[v] = (hi << 32) | v;   // ascending sort => degree descending, then vertex id ascending
         cnt += d != 0;
     }
     if (cnt) atomicAdd((unsigned long long *)n1, cnt);
 }
-__global__ void k_slots_from_keys(const u64 *__restrict__ keys, u64 n, u64 n1, u32 *__restrict__ vert, u32 *__restrict__ slot,
-                                  u32 *__restrict__ hdeg) {
+__global__ void k_slots_from_keys(const u64 *__restrict__ keys, const u64 *__restrict__ Ap, u64 n, u64 n1, u32 *__restrict__ vert,
+                                  u32 *__restrict__ slot, u32 *__restrict__ hdeg) {
     u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
     for (; s < n; s += stride) {
         u32 v = (u32)(keys[s] & 0xFFFFFFFFULL);
-        if (s < n1) { vert[s] = v; slot[v] = (u32)s; hdeg[s] = 0xFFFFFFFFu - (u32)(keys[s] >> 32); } else slot[v] = 0xFFFFFFFFu;
+        if (s < n1) {
+            const u64 d = Ap[v + 1] - Ap[v];
+            vert[s] = v; slot[v] = (u32)s; hdeg[s] = d > 0xFFFFFFFEULL ? 0xFFFFFFFEu : (u32)d;
+        } else slot[v] = 0xFFFFFFFFu;
     }
 }
 __global__ void k_full_order(const u64 *__restrict__ keys, u64 n, u32 *__restrict__ pvert, u32 *__restrict__ pperm) {
@@ -1222,14 +1259,14 @@ static void build_hot_pack(const DevCSR &A, const DevCSR &AT, PullTables &pt) {
     if (n == 0 || AT.nnz == 0 || n >= 0xFFFFFFFFULL) return;
     DevBuf<u64> keys(n), cnt(1);
     cnt.zero();
-    LAUNCH(k_degree_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, A.p.ptr, n, keys.ptr, cnt.ptr);
+    LAUNCH(k_degree_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, A.p.ptr, n, keys.ptr, cnt.ptr, ctx().opt_hot_shuffle != 0);
     sort_keys_u64(keys.ptr, n, 64);
     u64 n1 = read_scalar(cnt.ptr);
     pt.n1 = n1;
     pt.vert.alloc(n1 ? n1 : 1);
     pt.slot.alloc(n);
     pt.hdeg.alloc(n1 ? n1 : 1);
-    LAUNCH(k_slots_from_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, n, n1, pt.vert.ptr, pt.slot.ptr, pt.hdeg.ptr);
+    LAUNCH(k_slots_from_keys, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, keys.ptr, A.p.ptr, n, n1, pt.vert.ptr, pt.slot.ptr, pt.hdeg.ptr);
     // the order over ALL vertices (the sort already put the sinks last, by id): frontiers may be stored in it (permuted form)
     pt.pvert = std::make_shared<DevBuf<u32>>(n);
     pt.pperm = std::make_shared<DevBuf<u32>>(n);
@@ -1272,20 +1309,34 @@ static void build_pull_tables(const DevCSR &A, const DevCSR &AT, PullTables &pt)
 // SMs busy to the end.
 template <int W, bool HINTS, bool ACC>
 static void launch_pull(const DevCSR &AT, const PullTables &pt, u64 m, const u32 *gj, const u64 *gx, u64 *Y, const u64 *Gp,
-                        u32 hot_bytes, u32 tot_bytes) {
+                        PullHints ph) {
     Context &cx = ctx();
-    LAUNCH((k_pull_small<W, HINTS, ACC>), grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT.p.ptr, gj, m, gx, Y, hot_bytes, tot_bytes);
+    LAUNCH((k_pull_small<W, HINTS, ACC>), grid_for(m, 256, (u64)cx.num_sms * 32), 256, 0, AT.p.ptr, gj, m, gx, Y, ph);
     if (!pt.ns) return;
     auto seg = [&](auto kern) {
         int per_sm = 0;
         CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, 0));
         if (per_sm < 1) per_sm = 1;
         if (cx.opt_pull_grid > 0) per_sm = (int)cx.opt_pull_grid;
-        LAUNCH(kern, (u32)cx.num_sms * (u32)per_sm, 256, 0, pt.s_row.ptr, pt.s_start.ptr, pt.s_len.ptr, pt.ns, gj, gx, Y, Gp, hot_bytes,
-               tot_bytes);
+        LAUNCH(kern, (u32)cx.num_sms * (u32)per_sm, 256, 0, pt.s_row.ptr, pt.s_start.ptr, pt.s_len.ptr, pt.ns, gj, gx, Y, Gp, ph);
     };
     if (Gp) seg(k_pull_seg<W, HINTS, 4, true, ACC>);
     else seg(k_pull_seg<W, HINTS, 4, false, ACC>);
+}
+
+// The pull's L2 policies, as measured on the H100 (scripts/pull_l2.py, DESIGN §4.8): from W = 2 up, the first half of the L2 of
+// the gather source is evict_last and the rest evict_first (0.41 ms off a 4.6 ms W = 8 pull); the streams are evict_first only at
+// W = 2 and 4, where that gains another 0.08 ms -- at W = 8 and 16 it costs 0.07-0.16 ms.  At W = 1 no policy pays.
+// The prefix never exceeds the source.  (createpolicy.range takes 32-bit sizes: a source past 4 GB has its first 4 GB in the range.)
+static bool pull_hints_on(int W) { const i64 o = ctx().opt_hints; return o > 0 || (o < 0 && W >= 2); }
+static PullHints pull_hints(int W, u64 x_bytes) {
+    const Context &cx = ctx();
+    PullHints ph;
+    ph.tot = x_bytes > 0xFFFFFFF0ULL ? 0xFFFFFFF0u : (u32)x_bytes;
+    const u64 hot = cx.opt_hot_bytes >= 0 ? (u64)cx.opt_hot_bytes : cx.l2_bytes / 2;
+    ph.hot = hot < ph.tot ? (u32)hot : ph.tot;
+    ph.streams = cx.opt_hint_streams >= 0 ? cx.opt_hint_streams != 0 : (W == 2 || W == 4);
+    return ph;
 }
 
 template <int W>
@@ -1397,15 +1448,13 @@ static void hop_impl(const DevBits &Xin, const DevCSR &A, const DevCSR *AT, Pull
         // compulsory traffic: stream A' col_idx + rowptr, read X once, write Y once (X gathers hit L2).  Accumulating ("bits_pull_acc"),
         // Y is also read once: an upper bound, rows with nothing to add skip the read and the write.
         TimedScope ts(acc ? TK_BITS_PULL_ACC : TK_BITS_PULL, 4 * AT->nnz + 8 * (m + 1) + 8ULL * W * gn + (acc ? 16ULL : 8ULL) * W * m);
-        u64 totb = gn * W * 8;
-        const u32 tot_bytes = totb > 0xFFFFFFF0ULL ? 0xFFFFFFF0u : (u32)totb;
-        const u32 hot_bytes = (u64)cx.opt_hot_bytes < tot_bytes ? (u32)cx.opt_hot_bytes : tot_bytes;
-        const bool hints = cx.opt_hints > 0 || (cx.opt_hints < 0 && W <= 2);
+        const PullHints ph = pull_hints(W, gn * W * 8);
+        const bool hints = pull_hints_on(W);
         if (acc) {
-            if (hints) launch_pull<W, true, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-            else launch_pull<W, false, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-        } else if (hints) launch_pull<W, true, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
-        else launch_pull<W, false, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, hot_bytes, tot_bytes);
+            if (hints) launch_pull<W, true, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, ph);
+            else launch_pull<W, false, true>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, ph);
+        } else if (hints) launch_pull<W, true, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, ph);
+        else launch_pull<W, false, false>(*AT, *pt, m, gj, gx, Y.w.ptr, Gp, ph);
     }
     if (path_out) *path_out = 3;
 }

@@ -58,8 +58,10 @@ struct Context {
     i64 opt_bfs_direction = 0;     // 0 = direction-optimising, 1 = top-down only, 2 = bottom-up only (test hooks)
     i64 opt_bfs_sparse_exchange = 1;   // partitioned BFS: ship discovered-vertex lists instead of bitmaps when the frontier is sparse
     i64 opt_early_exit = 1;        // stop a pull row once it holds the OR monoid's terminal value (exact)
-    i64 opt_hints = -1;            // L2 createpolicy hints in the pull kernels: -1 = auto (on for W <= 2), 0 / 1 = off / on
-    i64 opt_hot_bytes = 64 << 20;  // size of that hot prefix
+    i64 opt_hints = -1;            // L2 cache policies in the pull kernels: -1 = as measured (on for W >= 2; bits.cu: pull_hints), 0 / 1 = off / on
+    i64 opt_hint_streams = -1;     // with hints on, the pull's streams (A' col_idx and rowptr, segment list, Y) are evict_first: -1 = as measured (W = 2, 4), 0 / 1
+    i64 opt_hot_bytes = -1;        // evict_last prefix of the pull's gather source: -1 = half of l2_bytes, 0 = the gathers are evict_normal
+    i64 opt_hot_shuffle = 0;       // measurement: pull tables built from now on order their hot set by a hash, not by out-degree
     i64 opt_hot_pack = 1;          // gather through the degree-sorted, sink-free relabelling of the frontier
     i64 opt_fused_prep = 1;        // pull hops: pack the frontier, count flops / edges and OR it in one pass
     i64 opt_csr_push = 1;          // small CSR frontiers push straight from their entries (no O(n*W) bit-matrix passes); 2 = whatever their size (measurement)
@@ -217,19 +219,29 @@ __device__ __forceinline__ u64 policy_range(const void *base, u32 primary_bytes,
     asm volatile("createpolicy.range.L2::evict_last.L2::evict_first.b64 %0, [%1], %2, %3;" : "=l"(p) : "l"(base), "r"(primary_bytes), "r"(total_bytes));
     return p;
 }
-__device__ __forceinline__ ulonglong2 ld_v2_hint(const ulonglong2 *p, u64 pol) {
+__device__ __forceinline__ u64 policy_normal() { u64 p; asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p)); return p; }
+// Read-only loads with an L2 policy.  They are non-volatile asm on the non-coherent path (ld.global.nc, what __ldg issues), so
+// the compiler schedules them as freely as __ldg: a kernel's software pipeline keeps its loads in flight across each other.
+// Only for data that nothing writes while the kernel runs.  _once: L1::no_allocate, for lines no later load of the thread reuses.
+__device__ __forceinline__ ulonglong2 ld_nc_v2(const ulonglong2 *p, u64 pol) {
     ulonglong2 v;
-    asm volatile("ld.global.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(v.x), "=l"(v.y) : "l"(p), "l"(pol));
+    asm("ld.global.nc.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(v.x), "=l"(v.y) : "l"(p), "l"(pol));
     return v;
 }
-__device__ __forceinline__ u64 ld_u64_hint(const u64 *p, u64 pol) {
-    u64 v; asm volatile("ld.global.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
+__device__ __forceinline__ u64 ld_nc_u64(const u64 *p, u64 pol) {
+    u64 v; asm("ld.global.nc.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
 }
-__device__ __forceinline__ u64 ld_u64_stream(const u64 *p, u64 pol) {
-    u64 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
+__device__ __forceinline__ u32 ld_nc_u32(const u32 *p, u64 pol) {
+    u32 v; asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
 }
-__device__ __forceinline__ u32 ld_u32_stream(const u32 *p, u64 pol) {
-    u32 v; asm volatile("ld.global.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
+__device__ __forceinline__ u64 ld_nc_once_u64(const u64 *p, u64 pol) {
+    u64 v; asm("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
+}
+__device__ __forceinline__ u32 ld_nc_once_u32(const u32 *p, u64 pol) {
+    u32 v; asm("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol)); return v;
+}
+__device__ __forceinline__ void st_v2_hint(ulonglong2 *p, ulonglong2 v, u64 pol) {
+    asm volatile("st.global.L2::cache_hint.v2.u64 [%0], {%1, %2}, %3;" ::"l"(p), "l"(v.x), "l"(v.y), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void st_u64_stream(u64 *p, u64 v, u64 pol) {
     asm volatile("st.global.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(p), "l"(v), "l"(pol) : "memory");

@@ -2202,6 +2202,8 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "hints") c.opt_hints = value;
     else if (n == "hot_pack") c.opt_hot_pack = value;
     else if (n == "hot_bytes") c.opt_hot_bytes = value;
+    else if (n == "hint_streams") c.opt_hint_streams = value;
+    else if (n == "hot_shuffle") c.opt_hot_shuffle = value;
     else if (n == "early_exit") c.opt_early_exit = value;
     else if (n == "pull_grid") c.opt_pull_grid = value;
     else if (n == "diag_filter") c.opt_diag_filter = value;

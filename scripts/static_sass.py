@@ -12,8 +12,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "falkordb_b200", "libb200grb.so")
 # demangled-name prefixes of the instantiations the 512-source chain (W = 8), the BFS engine and the side kernels launch
 WANT = [
-    ("hop, pull (mid + long-row segments), W = 8", r"k_pull_seg<8, false, 4, false>"),
-    ("hop, pull (rows <= 8), W = 8", r"k_pull_small<8, false>"),
+    ("hop, pull (mid + long-row segments), W = 8, L2 policies", r"k_pull_seg<8, true, 4, false, false>"),
+    ("hop, pull (rows <= 8), W = 8, L2 policies", r"k_pull_small<8, true, false>"),
     ("hop 2, CSR push", r"k_csr_push<8"),
     ("frontier totals in gather order", r"k_ordered_flops<8>"),
     ("materialise, count (carry-save)", r"k_bits_count_csa<8>"),
