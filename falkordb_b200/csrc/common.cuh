@@ -58,7 +58,7 @@ struct Context {
     i64 opt_bfs_direction = 0;     // 0 = direction-optimising, 1 = top-down only, 2 = bottom-up only (test hooks)
     i64 opt_bfs_sparse_exchange = 1;   // partitioned BFS: ship discovered-vertex lists instead of bitmaps when the frontier is sparse
     i64 opt_early_exit = 1;        // stop a pull row once it holds the OR monoid's terminal value (exact)
-    i64 opt_hints = -1;            // L2 cache policies in the pull kernels: -1 = as measured (on for W >= 2; bits.cu: pull_hints), 0 / 1 = off / on
+    i64 opt_hints = -1;            // L2 cache policies in the pull kernels: -1 = as measured (on for W >= 2; bits_hop.cu: pull_hints), 0 / 1 = off / on
     i64 opt_hint_streams = -1;     // with hints on, the pull's streams (A' col_idx and rowptr, segment list, Y) are evict_first: -1 = as measured (W = 2, 4), 0 / 1
     i64 opt_hot_bytes = -1;        // evict_last prefix of the pull's gather source: -1 = half of l2_bytes, 0 = the gathers are evict_normal
     i64 opt_hot_shuffle = 0;       // measurement: pull tables built from now on order their hot set by a hash, not by out-degree
@@ -195,7 +195,7 @@ struct DevBits {
     u64 nrows = 0, ncols = 0;
     u32 W = 0;
     DevBuf<u64> w;
-    // Permuted form (bits.cu, "hot-set order"): the words of vertex v live at position pos(v) instead of v, pos = the degree-sorted
+    // Permuted form (bits_hop.cu, "hot-set order"): the words of vertex v live at position pos(v) instead of v, pos = the degree-sorted
     // gather order of the matrix this frontier is about to be multiplied by (PullTables::pperm), so the pull of the next hop gathers
     // straight from it with no packing pass.  pvert[position] = vertex undoes it; perm_tag names the permutation (0 = natural).
     // pperm[vertex] = position addresses single vertices in place (the delta terms of a dirty hop).

@@ -158,7 +158,7 @@ void set_bits(GrB_Matrix A, DevBits &&b) {
     invalidate_aux(A);
 }
 
-// a frontier kept in another matrix's hot-set order (bits.cu: permuted form) goes back to natural vertex order before anything
+// a frontier kept in another matrix's hot-set order (bits_hop.cu: permuted form) goes back to natural vertex order before anything
 // but the pull it was ordered for looks at it
 static void natural_bits(GrB_Matrix A) {
     if (A->bits_valid && A->bits.permuted()) bits_naturalise(A->bits);

@@ -75,7 +75,7 @@ struct GB_Matrix_opaque : UObject {
     DevBits bits;
     bool devT_valid = false;
     DevCSR devT;
-    PullTables pt;   // pull-direction tables of devT (bits.cu)
+    PullTables pt;   // pull-direction tables of devT (bits_hop.cu)
     DevBuf<u32> bfs_deg; u64 bfs_edges = 0; bool bfs_deg_valid = false;   // out-degree table of the BFS engine (bfs_do.cu)
     DevIdStore ids;  // device copy of the host store, for a Tensor's multi-edge layers (B200_expand_edges)
     int sparsity_control = GxB_HYPERSPARSE | GxB_SPARSE | GxB_BITMAP | GxB_FULL;

@@ -18,22 +18,33 @@ void rmat_block_csr(int scale, u64 edge_factor, u64 seed, u64 lo, u64 hi, int by
 void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out);
 u64 spgemm_flops(const DevCSR &A, const DevCSR &B);
 
-struct PullTables;
-// bits.cu : frontier bit-matrix path for short-fat left operands (<= 1024 rows)
+// bits.cu : the frontier bit-matrix's form, for short-fat left operands (<= 1024 rows)
 u32 bits_words_for(u64 nrows);
 void bits_from_csr(const DevCSR &F, DevBits &X);
 void bits_to_csr(const DevBits &X, DevCSR &C);
 u64 bits_nvals(const DevBits &X);
-// Y = F * A expanded straight from F's CSR (small frontiers); false = the frontier touches enough of A that the pull should take
-// it (edges * 4 > nnz(A)), nothing was done.  pt (optional): A's pull tables; when they carry a vertex order the result is
-// written in it (permuted form).  acc: Y |= F * A, Y holding a natural-order product of the same shape (pt is then ignored)
-bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr,
-                        bool acc = false);
 void bits_naturalise(DevBits &X);                                // permuted form -> natural vertex order (no-op when natural)
 bool csr_is_diagonal(const DevCSR &A);                          // square, every entry (i,i)
 void bits_diag(const DevBits &X, const DevCSR &A, DevBits &Y, u64 *flops_out);   // Y = X * A for diagonal A
 void bits_to_rowmajor(const DevBits &X, u64 *out, u64 wpr);   // out[row * wpr + (col >> 6)], every word written
 void csr_to_rowmajor(const DevCSR &A, u64 *out, u64 wpr);     // out must be zero on entry
+void bits_andnot(DevBits &Y, const DevBits &M); // Y &= ~M
+void bits_or(DevBits &Y, const DevBits &Z);     // Y |= Z
+void bits_copy(const DevBits &X, DevBits &Y);
+
+struct PullTables;
+// csr_push.cu : the push straight from a CSR frontier, and the delta terms of delta_lmxm
+// Y = F * A expanded straight from F's CSR (small frontiers); false = the frontier touches enough of A that the pull should take
+// it (edges * 4 > nnz(A)), nothing was done.  pt (optional): A's pull tables; when they carry a vertex order the result is
+// written in it (permuted form).  acc: Y |= F * A, Y holding a natural-order product of the same shape (pt is then ignored)
+bool bits_push_from_csr(const DevCSR &F, const DevCSR &A, DevBits &Y, u64 *flops_out, const PullTables *pt = nullptr,
+                        bool acc = false);
+// The delta terms of delta_lmxm applied in place to Y = X * m:  Y = (Y AND NOT X * dm) OR X * dp, one pass over each delta's
+// entries.  The left operand is the bit-matrix Xb, or the CSR Xc when Y came from bits_push_from_csr (Xb null).  dm / dp may be
+// null.  X and Y stay in the vertex order they are stored in.  Returns flops(X * dm) + flops(X * dp).
+u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y);
+
+// bits_hop.cu : the bit-matrix hop (push or pull) and the exact dirty-hop repair
 struct PullTables {   // per-matrix tables of the pull direction, cached with the transpose mirror
     // hot-set order: vertices with out-edges, by out-degree descending
     DevBuf<u32> vert, slot, hdeg; u64 n1 = 0; bool packed = false;   // hdeg[s] = out-degree of vert[s]
@@ -58,13 +69,6 @@ struct PullTables {   // per-matrix tables of the pull direction, cached with th
 void bits_hop(const DevBits &X, const DevCSR &A, const DevCSR *AT, PullTables *pt, DevBits &Y, u64 *flops_out,
               int *path_out, bool acc = false);
 void bits_prepare_pull(const DevCSR &A, const DevCSR &AT, PullTables &pt);   // square A: build the pull tables now
-void bits_andnot(DevBits &Y, const DevBits &M); // Y &= ~M
-void bits_or(DevBits &Y, const DevBits &Z);     // Y |= Z
-void bits_copy(const DevBits &X, DevBits &Y);
-// The delta terms of delta_lmxm applied in place to Y = X * m:  Y = (Y AND NOT X * dm) OR X * dp, one pass over each delta's
-// entries.  The left operand is the bit-matrix Xb, or the CSR Xc when Y came from bits_push_from_csr (Xb null).  dm / dp may be
-// null.  X and Y stay in the vertex order they are stored in.  Returns flops(X * dm) + flops(X * dp).
-u64 bits_apply_deltas(const DevBits *Xb, const DevCSR *Xc, const DevCSR *dm, const DevCSR *dp, DevBits &Y);
 // The exact dirty hop's deleted-edge term.  For every column j that dm touches, Y[j] = OR of X[k] over the in-edges k of m(:, j)
 // that are not in dm (Y = X * (m \ dm) on those columns; every other column of X * m is already exact).  The plan is built once
 // per operand and call: dmT = dm', and the repaired columns of m' (m's transpose mirror, natural column ids) cut into segments of

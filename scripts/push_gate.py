@@ -7,7 +7,7 @@ each followed by hop 3 under the default options, since the form hop 2 leaves de
   csr0 : the same with push_slices = 0 -- its REDs in entry order
   bits : csr_push = 0 -- the frontier is built as a bit-matrix and the direction-optimising hop runs (push, path 2, below the gate)
   pull : pull_mode = 1 -- the bit-matrix pull (path 3)
-  auto : the default dispatch (bits.cu: bits_push_from_csr decides between the CSR push and the bit-matrix hop)
+  auto : the default dispatch (csr_push.cu: bits_push_from_csr decides between the CSR push and the bit-matrix hop)
 Then the same for synthetic hop-2 frontiers whose rows repeat hubs (--synthetic): a pool of vertices of out-degree >= 256 whose
 degrees sum to a target `edges`, each of the --sources rows holding each pool vertex with probability ratio / sources, so that
 flops / edges is about `ratio`.  Frontiers of more than 2^20 entries (beyond the CSR push's probe) are skipped.

@@ -1,4 +1,4 @@
-"""The CSR push's gate (bits.cu: csr_push_wins) and its relabelled operand (PullTables::ap).  A CSR frontier pushes straight from
+"""The CSR push's gate (csr_push.cu: csr_push_wins) and its relabelled operand (PullTables::ap).  A CSR frontier pushes straight from
 its entries when flops * 4 <= nnz(A), or when the bit-matrix hop would push too (edges * 4 <= nnz(A), edges = the out-degrees
 summed over the DISTINCT columns of F) and the duplicate flops it would merge stay under n * W / 2.  Frontiers here are built with
 a known duplication: edges from a pool of vertices, flops - edges from placing some of them in further rows.  Through a prepared

@@ -1,4 +1,4 @@
-"""The pull kernels under their L2 cache policies (bits.cu: k_pull_small, k_pull_seg, PullHints).  A policy only says how long a
+"""The pull kernels under their L2 cache policies (bits_hop.cu: k_pull_small, k_pull_seg, PullHints).  A policy only says how long a
 line stays in the L2, so no product may depend on it: every instantiation -- W = 1 ... 16, plain and accumulating, with and
 without early exit -- runs with hints off and on, with an evict_last prefix of nothing, of part of the gather source and of more
 than all of it, and must give the oracle's product bit for bit.  The graph has small rows, mid rows and rows of A' long enough to

@@ -1,4 +1,4 @@
-"""The sliced CSR push (bits.cu: csr_push_sliced).  Through a prepared operand whose relabelled col_idx (PullTables::ap) has every
+"""The sliced CSR push (csr_push.cu: csr_push_sliced).  Through a prepared operand whose relabelled col_idx (PullTables::ap) has every
 row ascending by position, the push cuts the positions into destination slices and issues the same REDs slice by slice.  Nothing
 about the product may depend on the slice count, so chains run with push_slices forced to 1, 3, 7 and more slices than vertices
 and are compared with the oracle by digest and by exported CSR; the routes that never slice (accumulating union hops, the delta

@@ -1,4 +1,4 @@
-"""Hot-set-ordered frontiers (bits.cu: permuted form): every observer of an ordered intermediate.  The 3-hop chain through this path
+"""Hot-set-ordered frontiers (bits_hop.cu: permuted form): every observer of an ordered intermediate.  The 3-hop chain through this path
 is also checked by bench.py's all-rows digest parity; this test adds the other observers.  Last in the `pytest -x` order."""
 import ctypes as C
 
@@ -95,7 +95,7 @@ def test_frontier_in_hot_set_order_between_push_and_pull(nsrc):
             F = two_hops()
             wr = np.repeat(np.arange(nsrc), np.diff(F2.p))
             assert list(F.iter()) == list(zip(wr.tolist(), F2.j.tolist())), "row iterator over an ordered frontier"
-        # the CSR push takes a hop iff its expansion is small against A (flops * 4 <= nnz(A), bits.cu: bits_push_from_csr)
+        # the CSR push takes a hop iff its expansion is small against A (flops * 4 <= nnz(A), csr_push.cu: bits_push_from_csr)
         expect_push = int(np.diff(A.p)[F1.j].sum()) * 4 <= A.nnz
         assert all(p == expect_push for p in pushed), (expect_push, pushed)
         if nsrc <= 6:
