@@ -79,7 +79,7 @@ inline cudaStream_t stream() { return ctx().stream; }
 enum TimedId { TK_BITS_PULL = 0, TK_BITS_PUSH, TK_HEAVY_ACC, TK_SMALL_ROWS, TK_BITS_FILL, TK_BITS_COUNT,
                TK_BITMAP_EXPAND, TK_BFS_EXPAND, TK_UNION, TK_FILTER, TK_MXV, TK_MASKED, TK_TRANSPOSE, TK_BITS_DELTA,
                TK_BITS_REPAIR, TK_BITS_PULL_ACC, TK_BITS_PUSH_ACC, TK_EDGE_EXPAND, TK_BFS_DELTA, TK_ADJ_BUILD,
-               TK_TENSOR_WRITE, TK_VAR_LEN_TRAILS, TK_COUNT_ };
+               TK_TENSOR_WRITE, TK_VAR_LEN_TRAILS, TK_VAR_LEN_REACH_BOTH, TK_COUNT_ };
 const char *timed_name(int id);
 void timed_begin(int id);
 void timed_end(int id, u64 algorithmic_bytes) noexcept;

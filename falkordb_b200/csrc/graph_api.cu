@@ -12,6 +12,7 @@ struct UnionOperand {
     GrB_Matrix m = nullptr, dp = nullptr, dm = nullptr;
     const DevCSR *ddp = nullptr;                 // dp's device form when it holds entries
     RepairPlan rp;                               // dm's repair plan (rp.ns == 0: nothing to repair)
+    bool planned = false;                        // ddp and rp are set (union_plan)
 };
 
 static std::vector<UnionOperand> union_operands(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops) {
@@ -125,6 +126,7 @@ static GrB_Info union_plan(std::vector<UnionOperand> &ops) {
         MultiLock lk = lock_all(ops);
         ensure_init();
         for (UnionOperand &o : ops) {
+            o.planned = true;
             if (o.dp) { ensure_dev(o.dp); if (o.dp->dev.nnz) o.ddp = &o.dp->dev; }
             if (!o.dm) continue;
             ensure_dev(o.dm);
@@ -489,8 +491,11 @@ static void reach_hop(GrB_Matrix F, GrB_Matrix R, bool masked, std::vector<Union
     if (cx.opt_sync_after_op) sync_stream();
 }
 
+// planned (optional): on success, receives the operands' frontier-form plan when the reach built one (left empty otherwise), so a
+// caller that runs further levels over the same operands need not plan them again; it releases them with union_release.
 static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_Index nsrc, const GrB_Matrix *m, const GrB_Matrix *dp,
-                           const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources, int64_t *levels_out) {
+                           const GrB_Matrix *dm, int nops, int64_t max_hops, int include_sources, int64_t *levels_out,
+                           std::vector<UnionOperand> *planned = nullptr) {
     const u64 n = m[0]->ncols;
     bool clean = nops == 1;
     for (int t = 0; t < nops && clean; t++)
@@ -505,7 +510,8 @@ static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_In
     GrB_Info info = GrB_SUCCESS;
     std::vector<UnionOperand> ops = union_operands(m, dp, dm, nops);
     const bool frontier = ctx().opt_bits_mode != 0 && bits_words_for(nsrc) != 0;
-    if (!clean && !frontier) info = reach_materialise(&U, ops, n);
+    const bool U_built = !clean && !frontier;
+    if (U_built) info = reach_materialise(&U, ops, n);
     else if (!clean) info = union_plan(ops);
     GrB_Matrix A = U ? U : m[0];                 // the operand of the row-wise calls
     GrB_Matrix F = nullptr, R = nullptr;
@@ -537,7 +543,8 @@ static GrB_Info reach_impl(GrB_Matrix *reached, const GrB_Index *sources, GrB_In
     }
     GrB_Matrix_free(&F);
     GrB_Matrix_free(&U);
-    if (!clean) union_release(ops);
+    if (!info && planned && !clean && !U_built) *planned = std::move(ops);
+    else if (!clean) union_release(ops);
     if (info) { GrB_Matrix_free(&R); return info; }
     if (levels_out) *levels_out = level;
     *reached = R;
@@ -800,6 +807,98 @@ GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_
         if (r == 1) { tl_error = "var_len_trails: output capacity too small (*nout / *npath = what is needed)"; return GrB_INSUFFICIENT_SPACE; }
         return GrB_SUCCESS;
     });
+}
+
+// ---- CondVarLenTraverse's DISTINCT endpoints of a bidirectional pattern (a)-[*min..max]-(b), min <= 1, for a batch of starts.
+// Every v != s: B200_reach_batch_delta's walk over each type's forward and transpose layers (a shortest walk is a path, hence a
+// trail); the start itself: a cycle through it of at most max_hops edges (var_len_reach.cu), whose longer cases run masked
+// levels of reach_hop over the same operands in closure rows of at most 1024.
+// ops: the reach's operands, planned by it (reach_impl's `planned`) or, when the reach materialised their union, not yet planned
+static GrB_Info reach_both_closure(GrB_Matrix R, const GrB_Index *starts, GrB_Index nstarts, const B200_TensorLayers *types,
+                                   int ntypes, std::vector<UnionOperand> &ops, uint64_t max_hops) {
+    const u64 n = types[0].m->nrows;
+    VlbPlan P;
+    GrB_Info info = guarded([&]() {
+        GpuLock g;
+        MultiLock lk = lock_all(types, ntypes);
+        ensure_init();
+        vlb_plan((const u64 *)starts, nstarts, edge_types_dev(types, ntypes, B200_DIR_BOTH), max_hops, P);
+        return GrB_SUCCESS;
+    });
+    if (!info && P.rows && !ops.front().planned) info = union_plan(ops);
+    for (u64 r0 = 0; r0 < P.rows && !info; r0 += 1024) {
+        const u64 r1 = std::min<u64>(P.rows, r0 + 1024);
+        GrB_Matrix F = nullptr, V = nullptr;
+        info = GrB_Matrix_new(&F, GrB_BOOL, r1 - r0, n);
+        if (!info) info = GrB_Matrix_new(&V, GrB_BOOL, r1 - r0, n);
+        if (!info) info = guarded([&]() {
+            GpuLock g;
+            MultiLock lk = lock_all(ops, {F, V});
+            DevBits fb, vb;
+            vlb_seed(P, r0, r1, n, fb, vb);
+            set_bits(F, std::move(fb));
+            set_bits(V, std::move(vb));
+            // the middle of a cycle of g <= max_hops edges is a path of g - 2 edges
+            for (u64 level = 0; level + 2 < max_hops; level++) {
+                reach_hop(F, V, true, ops);
+                if (!vlb_level(P, r0, r1, F->bits)) break;
+                bits_or(V->bits, F->bits);
+            }
+            return GrB_SUCCESS;
+        });
+        GrB_Matrix_free(&F);
+        GrB_Matrix_free(&V);
+    }
+    union_release(ops);
+    if (!info) info = guarded([&]() {
+        GpuLock g;
+        MultiLock lk{R};
+        if (R->bits_valid) {
+            ensure_bits(R);
+            DevBits b = std::move(R->bits);
+            vlb_fix_bits(P, b);
+            set_bits(R, std::move(b));
+        } else {
+            ensure_dev(R);
+            DevCSR out;
+            vlb_fix_csr(P, R->dev, out);
+            set_dev(R, std::move(out));
+        }
+        return GrB_SUCCESS;
+    });
+    guarded([&]() { GpuLock g; P = VlbPlan(); return GrB_SUCCESS; });   // the plan's buffers go back to the pool
+    return info;
+}
+
+GrB_Info B200_var_len_reach_both(GrB_Matrix *reached, const GrB_Index *starts, GrB_Index nstarts, const B200_TensorLayers *types,
+                                 int ntypes, uint64_t min_hops, uint64_t max_hops) {
+    CHECK_PTR(reached); CHECK_PTR(types);
+    if (nstarts) CHECK_PTR(starts);
+    if (ntypes < 1 || ntypes > 65536) { tl_error = "var_len_reach_both: ntypes outside 1 .. 65536"; return GrB_INVALID_VALUE; }
+    GrB_Info info = layers_check("var_len_reach_both", types, ntypes, true);
+    if (info) return info;
+    const u64 nv = types[0].m->nrows;
+    for (u64 i = 0; i < nstarts; i++)
+        if (starts[i] >= nv) { tl_error = "var_len_reach_both: start out of range"; return GrB_INVALID_INDEX; }
+    if (min_hops > 1) { tl_error = "var_len_reach_both: min_hops > 1 is not a reach (a walk is not a trail)"; return GrB_NOT_IMPLEMENTED; }
+    if (nstarts == 0 || min_hops > max_hops) return GrB_Matrix_new(reached, GrB_BOOL, nstarts, nv);
+    info = device_ready();                       // no device: fail before any host work
+    if (info) return info;
+    std::vector<GrB_Matrix> m, dp, dm;           // each type's forward layers, then its transpose's: the pattern of G'
+    for (int t = 0; t < ntypes; t++) {
+        const B200_TensorLayers &L = types[t];
+        m.insert(m.end(), {L.m, L.mt}); dp.insert(dp.end(), {L.dp, L.mt_dp}); dm.insert(dm.end(), {L.dm, L.mt_dm});
+    }
+    GrB_Matrix R = nullptr;
+    std::vector<UnionOperand> ops;               // the reach's plan, reused by the closure's levels
+    info = reach_impl(&R, starts, nstarts, m.data(), dp.data(), dm.data(), 2 * ntypes,
+                      max_hops > (uint64_t)INT64_MAX ? -1 : (int64_t)max_hops, 1, nullptr, min_hops == 0 ? nullptr : &ops);
+    if (info || min_hops == 0) { if (!info) *reached = R; return info; }
+    if (ops.empty()) ops = union_operands(m.data(), dp.data(), dm.data(), 2 * ntypes);
+    info = reach_both_closure(R, starts, nstarts, types, ntypes, ops, max_hops);
+    if (info) { GrB_Matrix_free(&R); return info; }
+    *reached = R;
+    return GrB_SUCCESS;
 }
 
 // ---- the read phase of a Tensor's relationship inserts and deletes (set_all_from_slices / remove_all, tensor.rs:333-629) for a

@@ -182,6 +182,21 @@ inline Matrix<bool> var_len_reach(const std::vector<const Tensor *> &types, Edge
     return Matrix<bool>::adopt(raw, false);
 }
 
+// The same fast path for a bidirectional pattern, as one B200_var_len_reach_both call over every type's live layers: row i holds
+// the DISTINCT nodes the trail DFS reaches from starts[i] under Both.  The reach over A u A' is exact for v != s; the start itself
+// is decided by the shortest cycle through it, which the call finds.  min_hops > 1 is refused: such a pattern keeps the DFS.
+inline Matrix<bool> var_len_reach_both(const std::vector<const Tensor *> &types, const std::vector<uint64_t> &starts, uint64_t min_hops,
+                                       uint64_t max_hops) {
+    if (min_hops > 1) throw std::invalid_argument("var_len_reach_both: min_hops > 1 is not a reach");
+    if (types.empty()) throw std::invalid_argument("var_len_reach_both: no relationship type");
+    std::vector<B200_TensorLayers> ls;
+    for (const Tensor *t : types) ls.push_back(t->waited_layers());
+    GrB_Matrix raw = nullptr;
+    grb_ok(B200_var_len_reach_both(&raw, starts.data(), starts.size(), ls.data(), (int)ls.size(), min_hops, max_hops),
+           "B200_var_len_reach_both");
+    return Matrix<bool>::adopt(raw, false);
+}
+
 // The trails of a batch of starts: start i's results are r[p[i] .. p[i+1]).
 struct VarLenBatch { std::vector<uint64_t> p{0}; std::vector<VarLenResult> r; };
 

@@ -803,6 +803,63 @@ static void t_var_len_reach_matches_trails() {   // device
     }
 }
 
+// var_len_reach_both (one B200_var_len_reach_both call) against the DISTINCT nodes the trail DFS reaches under Both, over the same
+// kind of tensors: self-loops in the base and in dp, deleted ones, multi-edge pairs, reciprocal pairs, a pair shared by two types.
+static void t_var_len_reach_both_matches_trails() {   // device
+    const uint64_t n = 750, used = 740;              // vertices 740.. have no edges
+    uint64_t x = 777;
+    auto rnd = [&]() { x = x * 6364136223846793005ULL + 1442695040888963407ULL; return x >> 33; };
+    std::vector<uint64_t> starts;
+    auto make = [&](uint64_t id) {
+        Tensor t(n, n);
+        std::vector<uint64_t> S, D, I;
+        for (uint64_t k = 0; k < 320; k++) { S.push_back(rnd() % used); D.push_back(rnd() % used); I.push_back(id++); }
+        for (uint64_t v = 0; v < used; v += 37) { S.push_back(v); D.push_back(v); I.push_back(id++); }   // self-loops
+        S.push_back(10); D.push_back(11); I.push_back(id++);                                               // a reciprocal pair
+        S.push_back(11); D.push_back(10); I.push_back(id++);
+        t.set_all_from_slices(S, D, I);
+        t.wait();
+        t.fold_oversized();
+        std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> rm;
+        for (size_t k = 0; k < S.size(); k += 6) rm.push_back(std::make_tuple(I[k], S[k], D[k]));     // deletes from the base
+        t.remove_all(rm);
+        std::vector<uint64_t> S2, D2, I2;
+        for (size_t k = 0; k < rm.size(); k += 3) { S2.push_back(std::get<1>(rm[k])); D2.push_back(std::get<2>(rm[k])); I2.push_back(id++); }
+        for (uint64_t k = 0; k < 30; k++) { S2.push_back(rnd() % used); D2.push_back(rnd() % used); I2.push_back(id++); }
+        for (size_t k = 1; k < 40; k += 13) { S2.push_back(S[k]); D2.push_back(D[k]); I2.push_back(id++); }   // multi-edge pairs
+        S2.push_back(5); D2.push_back(5); I2.push_back(id++);                                                 // a new self-loop
+        t.set_all_from_slices(S2, D2, I2);
+        t.wait();
+        REQUIRE(t.fwd_dp().nvals() > 0 && t.fwd_dm().nvals() > 0, "test setup: the forward deltas are not empty");
+        for (size_t k = 0; k < 40; k += 4) starts.push_back(S[k]);
+        return t;
+    };
+    Tensor a = make(0), b = make(100000);
+    for (uint64_t s : {741ULL, 5ULL, 10ULL, 37ULL, 749ULL, 5ULL}) starts.push_back(s);
+    typedef std::set<std::pair<uint64_t, uint64_t>> Pairs;
+    for (const std::vector<const Tensor *> &types : {std::vector<const Tensor *>{&a}, std::vector<const Tensor *>{&a, &b}})
+        for (uint64_t lo : {0ULL, 1ULL})
+            for (uint64_t hi : {0ULL, 1ULL, 2ULL, 3ULL, 4ULL}) {
+                Matrix<bool> R = var_len_reach_both(types, starts, lo, hi);
+                Pairs got, want;
+                auto it = R.iter();
+                std::tuple<uint64_t, uint64_t> e;
+                while (it.next(e)) got.insert({std::get<0>(e), std::get<1>(e)});
+                for (size_t i = 0; i < starts.size(); i++) {
+                    VarLenIterT<TensorsAdjacency> dfs(TensorsAdjacency{types}, lo, hi, false, true, -1, false);
+                    dfs.begin_start_node(starts[i]);
+                    VarLenResult r;
+                    while (dfs.next(r)) want.insert({(uint64_t)i, r.to});
+                }
+                REQUIRE(got == want && R.nrows() == starts.size(), "bidirectional reach differs from the trail DFS: types " << types.size()
+                        << " min " << lo << " max " << hi << " (" << got.size() << " vs " << want.size() << " pairs)");
+                REQUIRE(hi != 3 || lo != 1 || want.size() >= 40, "test setup: the starts reach something");
+            }
+    bool threw = false;
+    try { var_len_reach_both({&a}, starts, 2, 3); } catch (const std::invalid_argument &) { threw = true; }
+    REQUIRE(threw, "min_hops > 1 keeps the DFS");
+}
+
 // ---- the C-compatible RDB form of a Tensor (tensor.rs:1049-1204) and of a VersionedMatrix (versioned_matrix.rs:1082-1113) ----
 typedef std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> EdgeList;
 static EdgeList sorted_edges(const Tensor &t) {
@@ -1053,6 +1110,7 @@ static TestEntry TESTS[] = {
     {"traverse_over_tensor_operand", t_traverse_over_tensor_operand},
     {"coalesced_traverse_over_tensor_operand", t_coalesced_traverse_over_tensor_operand},
     {"var_len_reach_matches_trails", t_var_len_reach_matches_trails},
+    {"var_len_reach_both_matches_trails", t_var_len_reach_both_matches_trails},
     {"union_traverse_over_tensor_types", t_union_traverse_over_tensor_types},
     {"repack_output_batches", t_repack_output_batches},
     {"repack_logic", t_repack_logic},
@@ -1157,6 +1215,25 @@ int fdbh_var_len_reach(void **tensors, uint64_t ntypes, int dir, const uint64_t 
         if (dir != 0 && dir != 1) throw std::invalid_argument("var_len_reach: dir must be 0 (outgoing) or 1 (incoming)");
         Matrix<bool> R = var_len_reach(types, dir == 0 ? EdgeDirection::Outgoing : EdgeDirection::Incoming,
                                        std::vector<uint64_t>(starts, starts + nstarts), min_hops, max_hops);
+        std::vector<uint64_t> rows, nodes;
+        auto it = R.iter();
+        std::tuple<uint64_t, uint64_t> e;
+        while (it.next(e)) { rows.push_back(std::get<0>(e)); nodes.push_back(std::get<1>(e)); }
+        *nout = rows.size();
+        *out_rows = (uint64_t *)malloc(sizeof(uint64_t) * (rows.size() + 1));
+        *out_nodes = (uint64_t *)malloc(sizeof(uint64_t) * (rows.size() + 1));
+        memcpy(*out_rows, rows.data(), sizeof(uint64_t) * rows.size());
+        memcpy(*out_nodes, nodes.data(), sizeof(uint64_t) * rows.size());
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+// The bidirectional counterpart (var_len_reach_both): the (row, node) pairs in row order, malloc'ed; free with fdbh_free.
+int fdbh_var_len_reach_both(void **tensors, uint64_t ntypes, const uint64_t *starts, uint64_t nstarts, uint64_t min_hops,
+                            uint64_t max_hops, uint64_t **out_rows, uint64_t **out_nodes, uint64_t *nout) {
+    try {
+        std::vector<const Tensor *> types;
+        for (uint64_t k = 0; k < ntypes; k++) types.push_back((const Tensor *)tensors[k]);
+        Matrix<bool> R = var_len_reach_both(types, std::vector<uint64_t>(starts, starts + nstarts), min_hops, max_hops);
         std::vector<uint64_t> rows, nodes;
         auto it = R.iter();
         std::tuple<uint64_t, uint64_t> e;

@@ -171,6 +171,27 @@ struct TrailsOut {
 int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const std::vector<EdgeTypeDev> &types, int dir, u64 min_hops,
                    u64 max_hops, const std::vector<LabelDev> &labels, u64 nv, u64 tree_capacity, TrailsOut &o);
 
+// var_len_reach.cu : whether a bidirectional variable-length reach (B200_var_len_reach_both) emits each start itself, i.e. whether
+// the undirected multigraph of the types holds a cycle through it of at most max_hops edges
+struct VlbPlan {
+    u64 n = 0, nu = 0, Q = 0, rows = 0;           // starts, distinct starts, their distinct neighbours other than themselves, closure rows
+    DevBuf<u64> ds, u;                             // the starts; the distinct starts, ascending
+    DevBuf<u32> slot, dec;                         // per start its slot in u; per slot 1 = the start is emitted
+    DevBuf<u32> dn, dslot;                         // the distinct neighbours, slot-major, ascending within a slot
+    DevBuf<u64> nbase, rowbase;                    // per slot (nu + 1): its first distinct neighbour, its first closure row
+    u64 q0 = 0, q1 = 0;                            // the current chunk's distinct neighbours
+};
+// nstarts >= 1, starts < nv (checked by the caller); the short cycles (g <= 2) decided, the rows of the longer ones laid out
+void vlb_plan(const u64 *h_starts, u64 nstarts, const std::vector<EdgeTypeDev> &types, u64 max_hops, VlbPlan &P);
+// closure rows [r0, r1) (at most 1024): F = the seeds, R = the seeds and the start, W = bits_words_for(r1 - r0)
+void vlb_seed(VlbPlan &P, u64 r0, u64 r1, u64 n, DevBits &F, DevBits &R);
+// after a level of F: rows whose frontier meets their targets decide their start; every row of a decided start leaves F.
+// Returns the rows with a frontier left.
+u64 vlb_level(VlbPlan &P, u64 r0, u64 r1, DevBits &F);
+// (i, starts[i]) cleared in row i of the reach unless the start is emitted: the bit-matrix in place, or a CSR into out
+void vlb_fix_bits(const VlbPlan &P, DevBits &R);
+void vlb_fix_csr(const VlbPlan &P, const DevCSR &R, DevCSR &out);
+
 // adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
 // replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
 // and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.

@@ -678,3 +678,16 @@ def var_len_trails(starts, types, dir=DIR_OUT, min_hops=1, max_hops=None, dests=
     if paths:
         out["edges"], out["nodes"] = pe[:q], pn[:q + m]
     return out
+
+
+def var_len_reach_both(starts, types, min_hops=1, max_hops=None):
+    """B200_var_len_reach_both: the DISTINCT endpoints of the bidirectional pattern (a)-[*min_hops..max_hops]-(b), min_hops <= 1,
+    from each start over relationship types (`types` as expand_edges takes them; mt required).  Row i of the returned BOOL Matrix
+    (len(starts) x n) holds every b the trail DFS emits from starts[i]: each v != starts[i] within max_hops undirected edges, and
+    starts[i] itself when min_hops == 0 or a cycle of at most max_hops relationships runs through it.  max_hops None: unbounded."""
+    starts = _u64arr(starts)
+    n = len(starts)
+    h = P()
+    check(lib().B200_var_len_reach_both(C.byref(h), starts.ctypes.data if n else None, n, _layers(types), len(types), int(min_hops),
+                                        (1 << 64) - 1 if max_hops is None else int(max_hops)))
+    return Matrix(0, 0, bool, _handle=h)

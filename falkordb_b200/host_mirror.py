@@ -2,7 +2,7 @@
 Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending (through the reference's read phase
 or the device plans, B200_Tensor_insert_plan / B200_Tensor_remove_plan), and the routes that read its
 relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), CondVarLenTraverse's trails
-(B200_var_len_trails, or the reference's DFS), and the algo.BFS, algo.pageRank, algo.WCC
+(B200_var_len_trails, or the reference's DFS) and its bidirectional DISTINCT endpoints (B200_var_len_reach_both), and the algo.BFS, algo.pageRank, algo.WCC
 and algo.labelPropagation procedures over them."""
 import ctypes as C
 import os
@@ -49,6 +49,7 @@ def host():
     vl = [P, U64, C.c_int, P, P, U64, U64, U64, P, U64, C.c_int]
     L.fdbh_var_len_trails.argtypes = vl + [U64] + [P] * 5 + [C.POINTER(U64)] * 2
     L.fdbh_var_len_trails_dfs.argtypes = vl + [P] * 5 + [C.POINTER(U64)] * 2
+    L.fdbh_var_len_reach_both.argtypes = [P, U64, P, U64, U64, U64, C.POINTER(P), C.POINTER(P), C.POINTER(U64)]
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
     algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
     L.fdbh_algo_pagerank.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
@@ -199,6 +200,25 @@ def var_len_trails(tensors, starts, dir, min_hops=1, max_hops=None, dests=None, 
     out = {}
     for name, x, k in zip(("p", "end", "hops", "edges", "nodes"), ptrs, (len(src) + 1, m, m, q, q + m if emit_path else 0)):
         out[name] = np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64).copy() if k else np.zeros(0, np.uint64)
+        L.fdbh_free(x)
+    return out
+
+
+def var_len_reach_both(tensors, starts, min_hops=1, max_hops=None):
+    """CondVarLenTraverse's bidirectional fast path over Tensor objects (fdbh_var_len_reach_both, one B200_var_len_reach_both
+    call): the DISTINCT (row, node) pairs as a (k, 2) uint64 array in row order"""
+    L = host()
+    (src,) = _u64(starts)
+    ts = (C.c_void_p * max(1, len(tensors)))(*[t.h for t in tensors])
+    pr, pn, nv = C.c_void_p(), C.c_void_p(), U64(0)
+    if L.fdbh_var_len_reach_both(ts, len(tensors), src.ctypes.data, len(src), int(min_hops), (1 << 64) - 1 if max_hops is None else int(max_hops),
+                                 C.byref(pr), C.byref(pn), C.byref(nv)):
+        raise RuntimeError(L.fdbh_last_message().decode())
+    k = nv.value
+    out = np.zeros((k, 2), np.uint64)
+    for col, x in enumerate((pr, pn)):
+        if k:
+            out[:, col] = np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64)
         L.fdbh_free(x)
     return out
 

@@ -440,6 +440,19 @@ GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_
                              const GrB_Matrix *lab_dp, const GrB_Matrix *lab_dm, int nlabels, uint64_t tree_capacity,
                              uint64_t *out_p, uint32_t *out_end, uint32_t *out_hops, uint64_t out_capacity,
                              uint64_t *path_edge, uint32_t *path_node, uint64_t path_capacity, uint64_t *nout, uint64_t *npath);
+/* CondVarLenTraverse's DISTINCT endpoints of a bidirectional pattern (a)-[*min_hops..max_hops]-(b) with min_hops <= 1, from
+ * each starts[i], over ntypes tensors' live layers: *reached is a new nstarts x n BOOL matrix whose row i holds every b the trail
+ * DFS emits from starts[i] under B200_DIR_BOTH (B200_var_len_trails' endpoints, without multiplicity).  Over the undirected
+ * multigraph G' with one edge per live relationship (a self-loop once): v != starts[i] is in row i iff dist_G'(s, v) <= max_hops;
+ * starts[i] itself iff min_hops == 0 or G' holds a cycle through it of at most max_hops edges (a self-loop; two relationships to
+ * one neighbour, in either direction or of different types; or a longer cycle).  max_hops = UINT64_MAX: unbounded.  Every type
+ * needs mt.  Errors as B200_var_len_trails: NULL pointers or a NULL m / mt GrB_NULL_POINTER; ntypes outside 1 .. 65536
+ * GrB_INVALID_VALUE; m / dp not UINT64 GrB_DOMAIN_MISMATCH; layers not square of one size GrB_DIMENSION_MISMATCH; a start >= n
+ * GrB_INVALID_INDEX; host-resident layers, or min_hops > 1 (a walk is not a trail there: that pattern keeps the trail
+ * enumerator), GrB_NOT_IMPLEMENTED; with no device GxB_GPU_ERROR before any host work.  nstarts == 0 or min_hops > max_hops:
+ * empty rows, no device work.  No layer changes, apart from finishing pending tuples; no base is downloaded. */
+GrB_Info B200_var_len_reach_both(GrB_Matrix *reached, const GrB_Index *starts, GrB_Index nstarts, const B200_TensorLayers *types,
+                                 int ntypes, uint64_t min_hops, uint64_t max_hops);
 /* Flags of the write plans below. */
 #define B200_PLAN_COMMITTED 0x01 /* insert: m holds the pair, its value is to be reconciled (dm.erase) */
 #define B200_PLAN_CANCEL 0x02    /* insert: COMMITTED and m's value equals the new inline value (dp.erase instead of dp.insert) */
@@ -485,8 +498,9 @@ void B200_reset_stats(void);
  * accumulated device time (ms), launch count and algorithmic bytes of one kernel family since the last reset:
  * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", the accumulating
  * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", B200_bfs_delta's kernels over
- * dirty operands, "bfs_delta", B200_adjacency_delta's induced-layer kernels, "adj_build", and B200_var_len_trails' kernels,
- * "var_len_trails".  0 on success. */
+ * dirty operands, "bfs_delta", B200_adjacency_delta's induced-layer kernels, "adj_build", B200_var_len_trails' kernels,
+ * "var_len_trails", and B200_var_len_reach_both's own kernels (its reach and closure levels count under the hop families),
+ * "var_len_reach_both".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */

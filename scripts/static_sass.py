@@ -48,6 +48,10 @@ WANT = [
     ("trails, stored level fill", r"k_tr_fill"),
     ("trails, last-level emissions", r"k_tr_out_last"),
     ("trails, stored-level emissions", r"k_tr_out("),
+    ("bidirectional reach, closure hits", r"k_vb_hit"),
+    ("bidirectional reach, closure row mask", r"k_vb_mask"),
+    ("bidirectional reach, closure seeds", r"k_vb_seed("),
+    ("bidirectional reach, start fix-up (CSR)", r"k_vb_fix_copy"),
 ]
 OPS = [("LDG.*\\.256", r"\bLDG\.[A-Z0-9_.]*256"), ("LDG.*\\.128", r"\bLDG\.[A-Z0-9_.]*128"), ("LDG.*\\.64", r"\bLDG\.[A-Z0-9_.]*\.64\b"),
        ("LDG other", r"\bLDG\."), ("STG.*\\.256", r"\bSTG\.[A-Z0-9_.]*256"), ("STG.*\\.128", r"\bSTG\.[A-Z0-9_.]*128"), ("STG other", r"\bSTG\."),
