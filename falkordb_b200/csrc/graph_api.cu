@@ -901,6 +901,72 @@ GrB_Info B200_var_len_reach_both(GrB_Matrix *reached, const GrB_Index *starts, G
     return GrB_SUCCESS;
 }
 
+// ---- shortestPath((a)-[:R*min..max]->(b)) for a batch of bound pairs (ExprEval::eval_shortest_path, eval.rs:1296-1513) ----
+// The reference runs a bidirectional BFS per row over versioned row iterators.  Here the pairs other than src == dst run together
+// (shortest_path.cu): each side's neighbours are the union of its operands' effective rows, read from the layers as they stand.
+GrB_Info B200_shortest_path(const GrB_Index *src, const GrB_Index *dst, GrB_Index npairs, const GrB_Matrix *fm, const GrB_Matrix *fdp,
+                            const GrB_Matrix *fdm, int nf, const GrB_Matrix *bm, const GrB_Matrix *bdp, const GrB_Matrix *bdm, int nb,
+                            uint64_t min_hops, uint64_t max_hops, uint64_t *out_p, uint32_t *path_node, uint64_t node_capacity,
+                            uint64_t *nnodes) {
+    CHECK_PTR(out_p); CHECK_PTR(nnodes);
+    if (npairs) { CHECK_PTR(src); CHECK_PTR(dst); }
+    if (node_capacity) CHECK_PTR(path_node);
+    if (nf < 1 || nb < 1) { tl_error = "shortest_path: each side needs at least one operand"; return GrB_INVALID_VALUE; }
+    if (min_hops > 1) { tl_error = "shortest_path: min_hops must be 0 or 1"; return GrB_INVALID_VALUE; }
+    GrB_Info info = operands_check("shortest_path", fm, fdp, fdm, nf);
+    if (!info) info = operands_check("shortest_path", bm, bdp, bdm, nb);
+    if (info) return info;
+    const u64 n = fm[0]->nrows;
+    if (bm[0]->nrows != n) { tl_error = "shortest_path: operands and deltas must be square and equally sized"; return GrB_DIMENSION_MISMATCH; }
+    for (u64 i = 0; i < npairs; i++)
+        if (src[i] >= n || dst[i] >= n) { tl_error = "shortest_path: src or dst out of range"; return GrB_INVALID_INDEX; }
+    if (npairs == 0) { out_p[0] = 0; *nnodes = 0; return GrB_SUCCESS; }
+    info = device_ready();                       // no device: fail before any host work
+    if (info) return info;
+    std::vector<u64> ps, pd, pos;                // the pairs the BFS runs for, and their rows
+    for (u64 i = 0; i < npairs; i++)
+        if (src[i] != dst[i]) { ps.push_back(src[i]); pd.push_back(dst[i]); pos.push_back(i); }
+    std::vector<u64> len;
+    std::vector<u32> nodes;
+    info = guarded([&]() {
+        GpuLock g;
+        std::vector<UnionOperand> all = union_operands(fm, fdp, fdm, nf), b = union_operands(bm, bdp, bdm, nb);
+        all.insert(all.end(), std::make_move_iterator(b.begin()), std::make_move_iterator(b.end()));
+        MultiLock lk = lock_all(all);
+        ensure_init();
+        std::vector<SpOperand> sides[2];
+        for (int k = 0; k < nf + nb; k++)
+            sides[k >= nf].push_back(SpOperand{dev_or_null(all[k].m), dev_or_null(all[k].dp), dev_or_null(all[k].dm)});
+        const u64 fl = ps.empty() ? 0 : shortest_path(ps.data(), pd.data(), ps.size(), sides[0], sides[1], n, max_hops,
+                                                     (u64)std::max<i64>(0, ctx().opt_shortest_path_budget), len, nodes);
+        Context &cx = ctx();
+        cx.last_flops = fl; cx.total_flops += fl;
+        return GrB_SUCCESS;
+    });
+    if (info) return info;
+    // rows in input order: src == dst is the one-node path with min_hops == 0 and Null otherwise (eval.rs:1329, 1406)
+    std::vector<u64> first(ps.size() + 1, 0);
+    for (size_t k = 0; k < ps.size(); k++) first[k + 1] = first[k] + len[k];
+    u64 total = 0;
+    for (u64 i = 0, k = 0; i < npairs; i++) {
+        out_p[i] = total;
+        if (k < pos.size() && pos[k] == i) total += len[k++];
+        else total += min_hops == 0 ? 1 : 0;
+    }
+    out_p[npairs] = total;
+    *nnodes = total;
+    if (total > node_capacity) { tl_error = "shortest_path: node_capacity too small (*nnodes = nodes needed)"; return GrB_INSUFFICIENT_SPACE; }
+    for (u64 i = 0, k = 0; i < npairs; i++) {
+        if (k < pos.size() && pos[k] == i) {
+            std::copy(nodes.begin() + first[k], nodes.begin() + first[k + 1], path_node + out_p[i]);
+            k++;
+        } else if (min_hops == 0) {
+            path_node[out_p[i]] = (uint32_t)src[i];
+        }
+    }
+    return GrB_SUCCESS;
+}
+
 // ---- the read phase of a Tensor's relationship inserts and deletes (set_all_from_slices / remove_all, tensor.rs:333-629) for a
 // whole batch in one call: writes.cu.  Only reads the layers; their pending tuples are finished like any device read's.
 static_assert(B200_PLAN_COMMITTED == WP_COMMITTED && B200_PLAN_CANCEL == WP_CANCEL && B200_PLAN_MT_BASE == WP_MT_BASE &&

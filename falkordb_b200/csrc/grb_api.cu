@@ -2212,6 +2212,7 @@ GrB_Info B200_set_option(const char *name, int64_t value) {
     else if (n == "perm_push") c.opt_perm_push = value;
     else if (n == "push_slices") c.opt_push_slices = value;
     else if (n == "union_accum") c.opt_union_accum = value;
+    else if (n == "shortest_path_budget") c.opt_shortest_path_budget = value;
     // retired: the pull, the count pass and the fill have a single kernel each now, and there is no persisting-L2 window; the
     // names stay accepted so callers that set them keep working
     else if (n == "fill_kernel" || n == "fill_cap" || n == "pull_kernel" || n == "unroll" || n == "small_split" ||

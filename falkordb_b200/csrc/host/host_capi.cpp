@@ -5,6 +5,7 @@
 #include "cond_var_len_traverse.hpp"
 #include "algo_bfs.hpp"
 #include "algo_procs.hpp"
+#include "shortest_path.hpp"
 #include <functional>
 #include <map>
 #include <set>
@@ -1462,6 +1463,34 @@ int fdbh_algo_bfs(void *adj, void **all_types, uint64_t nall, void **named, uint
         };
         out(out_nodes, r.nodes); out(out_edges, r.edges);
         *nnodes = r.nodes.size(); *nedges = r.edges.size();
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
+// shortestPath (shortest_path.hpp).  adj: the adjacency VersionedMatrix; all_types / named: Tensor pointers (nnamed = 0: no type
+// named; a null entry: a named type the graph lacks); max_hops UINT64_MAX unbounded.  route 0: shortest_path (B200_shortest_path +
+// B200_expand_edges); 1: shortest_path_by_iter (the reference's NeighborIter BFS and Tensor::get).  Outputs (malloc'ed; free with
+// fdbh_free): p[npairs + 1] over nodes, ep[npairs + 1] over ids; a row with no node is Null.
+int fdbh_shortest_path(void *adj, void **all_types, uint64_t nall, void **named, uint64_t nnamed, int directed, uint64_t min_hops,
+                       uint64_t max_hops, const uint64_t *srcs, const uint64_t *dsts, uint64_t npairs, int route, uint64_t **out_p,
+                       uint64_t **out_nodes, uint64_t **out_ep, uint64_t **out_ids) {
+    try {
+        ShortestPathQuery q;
+        q.adj = (const VersionedMatrix *)adj;
+        for (uint64_t k = 0; k < nall; k++) q.all_types.push_back((const Tensor *)all_types[k]);
+        for (uint64_t k = 0; k < nnamed; k++) q.named.push_back((const Tensor *)named[k]);
+        q.directed = directed != 0; q.min_hops = min_hops; q.max_hops = max_hops;
+        if (npairs) { q.srcs.assign(srcs, srcs + npairs); q.dsts.assign(dsts, dsts + npairs); }
+        ShortestPathResult r;
+        if (route == 0) r = shortest_path(q);
+        else if (route == 1) r = shortest_path_by_iter(q);
+        else throw std::invalid_argument("shortest_path: unknown route");
+        auto out = [](uint64_t **dst, const std::vector<uint64_t> &v) {
+            *dst = (uint64_t *)malloc(sizeof(uint64_t) * (v.size() + 1));
+            if (!*dst) throw std::bad_alloc();
+            memcpy(*dst, v.data(), sizeof(uint64_t) * v.size());
+        };
+        out(out_p, r.p); out(out_nodes, r.nodes); out(out_ep, r.ep); out(out_ids, r.ids);
         return 0;
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
 }

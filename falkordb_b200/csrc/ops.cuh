@@ -192,6 +192,14 @@ u64 vlb_level(VlbPlan &P, u64 r0, u64 r1, DevBits &F);
 void vlb_fix_bits(const VlbPlan &P, DevBits &R);
 void vlb_fix_csr(const VlbPlan &P, const DevCSR &R, DevCSR &out);
 
+// shortest_path.cu : shortestPath's bidirectional BFS (B200_shortest_path) for np pairs with src != dst (< n, checked by the caller).
+// Each side is a union of operands (m \ dm) u dp, pattern only.  len[i] = nodes on pair i's path (0: Null); nodes = the paths,
+// concatenated, from src to dst.  budget: neighbour entries per piece of a round (0: from free memory).  Returns the neighbour
+// entries scanned.
+struct SpOperand { const DevCSR *m, *dp, *dm; };
+u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<SpOperand> &fwd, const std::vector<SpOperand> &bwd,
+                  u64 n, u64 max_hops, u64 budget, std::vector<u64> &len, std::vector<u32> &nodes);
+
 // adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
 // replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
 // and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.

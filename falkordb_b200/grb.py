@@ -46,11 +46,11 @@ def _u64arr(a):
 
 def _operands(ms, deltas):
     """(m, dp, dm, n): the handle arrays of operands `ms` and of their deltas, one (dp, dm) pair per operand (either may be None;
-    `deltas` None: no pending writes)."""
+    `deltas` None: no pending writes).  Matrix objects or raw handles."""
     n = len(ms)
     deltas = [(None, None)] * n if deltas is None else list(deltas)
     assert len(deltas) == n, "one (dp, dm) pair per operand"
-    arr = lambda xs: (C.c_void_p * max(1, n))(*[None if x is None else x.h for x in xs])
+    arr = lambda xs: (C.c_void_p * max(1, n))(*[_handle(x) for x in xs])
     return arr(ms), arr([d[0] for d in deltas]), arr([d[1] for d in deltas]), n
 
 
@@ -691,3 +691,27 @@ def var_len_reach_both(starts, types, min_hops=1, max_hops=None):
     check(lib().B200_var_len_reach_both(C.byref(h), starts.ctypes.data if n else None, n, _layers(types), len(types), int(min_hops),
                                         (1 << 64) - 1 if max_hops is None else int(max_hops)))
     return Matrix(0, 0, bool, _handle=h)
+
+
+def shortest_path(src, dst, fwd, bwd, min_hops=1, max_hops=None, fwd_deltas=None, bwd_deltas=None):
+    """B200_shortest_path: shortestPath((a)-[*min_hops..max_hops]->(b)) for the pairs (src[i], dst[i]).  `fwd` / `bwd`: the operands
+    each side walks (a Matrix or a list), `fwd_deltas` / `bwd_deltas` one (dp, dm) pair per operand (either may be None).  Returns one
+    entry per pair: the path's nodes from src to dst as a uint32 array, or None (Null).  max_hops None: unbounded."""
+    src, dst = _u64arr(src), _u64arr(dst)
+    assert len(src) == len(dst), "one dst per src"
+    n = len(src)
+    fwd = [fwd] if isinstance(fwd, Matrix) else list(fwd)
+    bwd = [bwd] if isinstance(bwd, Matrix) else list(bwd)
+    out_p = np.zeros(n + 1, np.uint64)
+    cap = max(16, n * (min(31, (1 << 64) - 1 if max_hops is None else int(max_hops)) + 1))   # fits every path of up to 31 edges
+    for _ in range(2):                               # a result larger than the first guess is rerun into its size
+        nodes = np.zeros(cap, np.uint32)
+        nn = U64(0)
+        info = lib().B200_shortest_path(src.ctypes.data if n else None, dst.ctypes.data if n else None, n, *_operands(fwd, fwd_deltas),
+                                        *_operands(bwd, bwd_deltas), int(min_hops), (1 << 64) - 1 if max_hops is None else int(max_hops),
+                                        out_p.ctypes.data, nodes.ctypes.data, cap, C.byref(nn))
+        if info != -103:
+            break
+        cap = nn.value
+    check(info)
+    return [nodes[out_p[i]:out_p[i + 1]].copy() if out_p[i + 1] > out_p[i] else None for i in range(n)]

@@ -2,7 +2,8 @@
 Tensor built by GRAPH.BULK's device-side load and changed by batched writes that stay pending (through the reference's read phase
 or the device plans, B200_Tensor_insert_plan / B200_Tensor_remove_plan), and the routes that read its
 relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), CondVarLenTraverse's trails
-(B200_var_len_trails, or the reference's DFS) and its bidirectional DISTINCT endpoints (B200_var_len_reach_both), and the algo.BFS, algo.pageRank, algo.WCC
+(B200_var_len_trails, or the reference's DFS) and its bidirectional DISTINCT endpoints (B200_var_len_reach_both), the shortestPath
+expression (B200_shortest_path, or the reference's NeighborIter BFS), and the algo.BFS, algo.pageRank, algo.WCC
 and algo.labelPropagation procedures over them."""
 import ctypes as C
 import os
@@ -16,6 +17,7 @@ _L = None
 
 ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
 BFS_DEVICE, BFS_BY_EXTRACT = 0, 1
+SP_DEVICE, SP_BY_ITER = 0, 1
 ALGO_DEVICE, ALGO_BY_EXTRACT = 0, 1
 WRITE_REFERENCE, WRITE_DEVICE = 0, 1
 
@@ -50,6 +52,7 @@ def host():
     L.fdbh_var_len_trails.argtypes = vl + [U64] + [P] * 5 + [C.POINTER(U64)] * 2
     L.fdbh_var_len_trails_dfs.argtypes = vl + [P] * 5 + [C.POINTER(U64)] * 2
     L.fdbh_var_len_reach_both.argtypes = [P, U64, P, U64, U64, U64, C.POINTER(P), C.POINTER(P), C.POINTER(U64)]
+    L.fdbh_shortest_path.argtypes = [P, P, U64, P, U64, C.c_int, U64, U64, P, P, U64, C.c_int] + [C.POINTER(P)] * 4
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
     algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
     L.fdbh_algo_pagerank.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
@@ -298,6 +301,30 @@ def algo_bfs(adj, all_types, named, src, max_depth=-1, want_edges=True, deleted=
         out.append(np.frombuffer((C.c_char * (8 * k)).from_address(x.value), np.uint64).copy() if k else np.zeros(0, np.uint64))
         L.fdbh_free(x)
     return tuple(out)
+
+
+def shortest_path(adj, all_types, named, srcs, dsts, directed=True, min_hops=1, max_hops=None, route=SP_DEVICE):
+    """fdbh_shortest_path: shortestPath((a)-[:named*min_hops..max_hops]->(b)) per pair (srcs[i], dsts[i]) over `named` Tensors (None
+    entries: types the graph lacks), or over the adjacency VersionedMatrix `adj` when none is named; relationship ids from `named`,
+    or from `all_types` when none is named.  Returns one entry per pair: (nodes, ids) as lists, or None (Null)."""
+    L = host()
+    s, d = _u64(srcs, dsts)
+    arr = lambda xs: (C.c_void_p * max(1, len(xs)))(*[None if x is None else x.h for x in xs])
+    named = list(named or ())
+    ptrs = [C.c_void_p() for _ in range(4)]
+    rc = L.fdbh_shortest_path(None if adj is None else adj.h, arr(all_types), len(all_types), arr(named), len(named), 1 if directed else 0,
+                              int(min_hops), (1 << 64) - 1 if max_hops is None else int(max_hops), s.ctypes.data, d.ctypes.data, len(s),
+                              route, *[C.byref(x) for x in ptrs])
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    n = len(s)
+    p = np.frombuffer((C.c_char * (8 * (n + 1))).from_address(ptrs[0].value), np.uint64).copy()
+    ep = np.frombuffer((C.c_char * (8 * (n + 1))).from_address(ptrs[2].value), np.uint64).copy()
+    nodes = np.frombuffer((C.c_char * (8 * int(p[-1]))).from_address(ptrs[1].value), np.uint64).tolist() if p[-1] else []
+    ids = np.frombuffer((C.c_char * (8 * int(ep[-1]))).from_address(ptrs[3].value), np.uint64).tolist() if ep[-1] else []
+    for x in ptrs:
+        L.fdbh_free(x)
+    return [(nodes[p[i]:p[i + 1]], ids[ep[i]:ep[i + 1]]) if p[i + 1] > p[i] else None for i in range(n)]
 
 
 def _algo(fn, dt, adj, all_types, named, labels, node_count, deleted, route, *extra):

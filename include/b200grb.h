@@ -499,8 +499,8 @@ void B200_reset_stats(void);
  * "bits_pull", "bits_push", "heavy_accumulate", "bits_fill", "bits_count", "bits_delta", "bits_repair", the accumulating
  * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", B200_bfs_delta's kernels over
  * dirty operands, "bfs_delta", B200_adjacency_delta's induced-layer kernels, "adj_build", B200_var_len_trails' kernels,
- * "var_len_trails", and B200_var_len_reach_both's own kernels (its reach and closure levels count under the hop families),
- * "var_len_reach_both".  0 on success. */
+ * "var_len_trails", B200_var_len_reach_both's own kernels (its reach and closure levels count under the hop families),
+ * "var_len_reach_both", and B200_shortest_path's, "shortest_path".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
@@ -529,6 +529,25 @@ GrB_Info B200_bfs_ex(GrB_Matrix A, GrB_Index src, int64_t max_level, int64_t des
  * GxB_GPU_ERROR before any host work. */
 GrB_Info B200_bfs_delta(const GrB_Matrix *m, const GrB_Matrix *dp, const GrB_Matrix *dm, int nops, GrB_Index src,
                         int64_t max_level, int64_t dest, int64_t *level, int64_t *parent, int location, B200_BfsInfo *info);
+/* The shortestPath((a)-[:R1|R2*min_hops..max_hops]->(b)) expression for npairs bound pairs (ExprEval::eval_shortest_path,
+ * eval.rs:1296-1513): the reference's bidirectional BFS, path for path.  The forward side walks the union of its nf operands
+ * (fm, fdp, fdm) and the backward side that of its nb operands (bm, bdp, bdm), each with B200_reach_batch_delta's operand rules
+ * (m / dp may be UINT64; within an operand dp wins over dm; an entry one operand holds survives another operand's dm; dp / dm may
+ * be NULL arrays or hold NULL entries).  Each round expands the side with the smaller front (the forward one on a tie); a new
+ * vertex's parent is its lowest-ranked front neighbour, the next front is ordered by (parent rank, vertex), and the meet is the
+ * least (other side's depth, parent rank, vertex).  src == dst: the one-node path when min_hops == 0, else Null.
+ * max_hops = UINT64_MAX: unbounded.  Row i is path_node[out_p[i] .. out_p[i+1]), from src[i] to dst[i]; an empty row is Null.
+ * out_p (npairs + 1 entries) and *nnodes are always written; nodes only when they fit node_capacity, else GrB_INSUFFICIENT_SPACE
+ * with *nnodes = the nodes needed.  The relationships between consecutive nodes are B200_expand_edges(DIR_BOTH, targets,
+ * EDGES_FIRST)'s first entry per row.  Errors: nf or nb < 1, or min_hops > 1, GrB_INVALID_VALUE; operands not square of one size
+ * GrB_DIMENSION_MISMATCH; an endpoint >= n GrB_INVALID_INDEX; host-resident operands GrB_NOT_IMPLEMENTED; with no device
+ * GxB_GPU_ERROR before any host work.  npairs == 0: success with no device work.  last_flops = the neighbour entries scanned.
+ * No layer changes, apart from finishing pending tuples; no base is downloaded.  Option "shortest_path_budget": neighbour entries
+ * per piece of a round (0: sized from free device memory). */
+GrB_Info B200_shortest_path(const GrB_Index *src, const GrB_Index *dst, GrB_Index npairs, const GrB_Matrix *fm, const GrB_Matrix *fdp,
+                            const GrB_Matrix *fdm, int nf, const GrB_Matrix *bm, const GrB_Matrix *bdp, const GrB_Matrix *bdm, int nb,
+                            uint64_t min_hops, uint64_t max_hops, uint64_t *out_p, uint32_t *path_node, uint64_t node_capacity,
+                            uint64_t *nnodes);
 /* The adjacency the algorithm procedures run on (algo.pageRank / algo.WCC / algo.labelPropagation, algo_procedures.rs:718-732,
  * 816-832, 1207-1223), built on the device in one call over relationship operands with pending writes.  *A is a new BOOL, iso
  * matrix: the union over t of the induced effective layer (m[t] \ dm[t]) u dp[t], restricted to the kept vertices (rows and

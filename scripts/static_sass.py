@@ -52,6 +52,9 @@ WANT = [
     ("bidirectional reach, closure row mask", r"k_vb_mask"),
     ("bidirectional reach, closure seeds", r"k_vb_seed("),
     ("bidirectional reach, start fix-up (CSR)", r"k_vb_fix_copy"),
+    ("shortest path, neighbour emission", r"k_sp_emit"),
+    ("shortest path, distinct entries and meets", r"k_sp_classify"),
+    ("shortest path, path write", r"k_sp_write"),
 ]
 OPS = [("LDG.*\\.256", r"\bLDG\.[A-Z0-9_.]*256"), ("LDG.*\\.128", r"\bLDG\.[A-Z0-9_.]*128"), ("LDG.*\\.64", r"\bLDG\.[A-Z0-9_.]*\.64\b"),
        ("LDG other", r"\bLDG\."), ("STG.*\\.256", r"\bSTG\.[A-Z0-9_.]*256"), ("STG.*\\.128", r"\bSTG\.[A-Z0-9_.]*128"), ("STG other", r"\bSTG\."),
