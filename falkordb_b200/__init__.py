@@ -6,4 +6,4 @@ used by the tests and the benchmark.  There is no CPU fallback: importing works 
 (so the symbol table can be checked), every bulk call fails loudly without one.
 """
 from ._lib import lib, GrbError, check, LIB_PATH, INFO  # noqa: F401
-from .grb import Matrix, Descriptor, init, rmat, get_stat, reset_stats, set_option, sync, bfs, wait_ticket, traverse_to_host, traverse_batch, multi_source_reach, reach_batch, adjacency, OUT_AUTO, OUT_BITMAP, OUT_CSR, expand_edges, DIR_OUT, DIR_IN, DIR_BOTH, EDGES_ALL, EDGES_FIRST, insert_plan, remove_plan, var_len_trails, var_len_reach_both, shortest_path  # noqa: F401
+from .grb import Matrix, Descriptor, init, rmat, get_stat, reset_stats, set_option, sync, bfs, wait_ticket, traverse_to_host, traverse_batch, multi_source_reach, reach_batch, adjacency, OUT_AUTO, OUT_BITMAP, OUT_CSR, expand_edges, DIR_OUT, DIR_IN, DIR_BOTH, EDGES_ALL, EDGES_FIRST, insert_plan, remove_plan, var_len_trails, var_len_reach_both, shortest_path, all_shortest_paths  # noqa: F401

@@ -106,6 +106,7 @@ def lib():
                                 C.POINTER(U64), C.POINTER(U64)],
         "B200_var_len_reach_both": [C.POINTER(P), P, U64, P, C.c_int, U64, U64],
         "B200_shortest_path": [P, P, U64, P, P, P, C.c_int, P, P, P, C.c_int, U64, U64, P, P, U64, C.POINTER(U64)],
+        "B200_all_shortest_paths": [P, P, U64, P, C.c_int, C.c_int, U64, P, P, P, P, P, P, U64, C.POINTER(U64)],
         "B200_comm_unique_id": [P], "B200_comm_init": [C.POINTER(P), C.c_int, C.c_int, P], "B200_comm_free": [C.POINTER(P)],
         "B200_bfs_partitioned": [P, P, U64, U64, P, U64, I64, I64, P, P, C.c_int, P],
     }

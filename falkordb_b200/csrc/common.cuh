@@ -69,7 +69,7 @@ struct Context {
     i64 opt_diag_filter = 1;       // frontier-form mxm by a diagonal (label) matrix runs as an elementwise column filter
     i64 opt_pull_grid = 0;         // CTAs per SM of the segment pull kernel (0 = occupancy: one resident wave)
     i64 opt_union_accum = 1;       // union hops: clean extra operands OR into one product (0 = a product per operand plus an OR pass; measurement)
-    i64 opt_shortest_path_budget = 0;   // B200_shortest_path: neighbour entries per piece of a round (0 = a sixteenth of free memory's worth, shortest_path.cu)
+    i64 opt_shortest_path_budget = 0;   // B200_shortest_path / B200_all_shortest_paths: neighbour entries per piece of a round or level (0 = a sixteenth of free memory's worth)
 };
 Context &ctx();
 void ensure_init();
@@ -80,7 +80,8 @@ inline cudaStream_t stream() { return ctx().stream; }
 enum TimedId { TK_BITS_PULL = 0, TK_BITS_PUSH, TK_HEAVY_ACC, TK_SMALL_ROWS, TK_BITS_FILL, TK_BITS_COUNT,
                TK_BITMAP_EXPAND, TK_BFS_EXPAND, TK_UNION, TK_FILTER, TK_MXV, TK_MASKED, TK_TRANSPOSE, TK_BITS_DELTA,
                TK_BITS_REPAIR, TK_BITS_PULL_ACC, TK_BITS_PUSH_ACC, TK_EDGE_EXPAND, TK_BFS_DELTA, TK_ADJ_BUILD,
-               TK_TENSOR_WRITE, TK_VAR_LEN_TRAILS, TK_VAR_LEN_REACH_BOTH, TK_SHORTEST_PATH, TK_COUNT_ };
+               TK_TENSOR_WRITE, TK_VAR_LEN_TRAILS, TK_VAR_LEN_REACH_BOTH, TK_SHORTEST_PATH, TK_ALL_SHORTEST_PATHS,
+               TK_COUNT_ };
 const char *timed_name(int id);
 void timed_begin(int id);
 void timed_end(int id, u64 algorithmic_bytes) noexcept;

@@ -88,8 +88,9 @@ __device__ u64 merged_ids(const EType &t, u64 key, F f) {
 // edges.cu: the adjacency of n >= 1 distinct nodes d_src (device) over T types dt (device), in Graph::get_node_relationships_by_type's
 // order (graph.rs:1797-1835): per node, types in order; per type the outgoing half (neighbour ascending, ids ascending), then the
 // incoming half (source ascending); under dir 2 a self-loop once, in the outgoing half.  Device outputs: node i covers
-// p[i] .. p[i+1] of node (the neighbour) and edge (the id).  Returns the entries; adds the passes' compulsory bytes to *bytes.
+// p[i] .. p[i+1] of node (the neighbour) and edge (the id); with tb, per entry its type << 1 | 1 for the incoming half.  Returns
+// the entries; adds the passes' compulsory bytes to *bytes.
 u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
-                   u64 *bytes);
+                   u64 *bytes, DevBuf<u32> *tb = nullptr);
 
 } // namespace b200

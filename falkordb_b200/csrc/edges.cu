@@ -175,7 +175,7 @@ __global__ void k_ee_fill(EArgs A, const u64 *__restrict__ lstart, const u64 *__
 // list and in the other layer of its (type, block) -- one binary search.  A base entry and a delta-plus entry never both count.
 __global__ void k_ee_ref_fill(EArgs A, const u64 *__restrict__ lstart, const u64 *__restrict__ lo, const u64 *__restrict__ len,
                               const u64 *__restrict__ val, const u32 *__restrict__ cnt, const u64 *__restrict__ pos,
-                              u32 *__restrict__ node, u64 *__restrict__ edge) {
+                              u32 *__restrict__ node, u64 *__restrict__ edge, u32 *__restrict__ tb) {
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < A.E; e += (u64)gridDim.x * blockDim.x) {
         const u32 c = cnt[e];
         if (!c) continue;
@@ -200,6 +200,7 @@ __global__ void k_ee_ref_fill(EArgs A, const u64 *__restrict__ lstart, const u64
         auto put = [&](u64 k, u64 id) {
             node[o + k] = x;
             edge[o + k] = id;
+            if (tb) tb[o + k] = L.t << 1 | (L.rev ? 1 : 0);
             return k + 1 < c;
         };
         if (v != EE_MULTI) put(0, v);
@@ -242,7 +243,7 @@ struct EeBatch {
 };
 
 u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
-                   u64 *bytes) {
+                   u64 *bytes, DevBuf<u32> *tb) {
     const u32 nb = dir == 2 ? 2 : 1, grid = (u32)ctx().num_sms * 8;
     EeBatch B(EArgs{d_src, nullptr, dt, n, n * nb * T * 2, 0, T, nb, dir});
     B.prepare(0, grid);
@@ -252,10 +253,11 @@ u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, Dev
     d2h(&total, p.ptr + n, 1);
     sync_stream();
     node.alloc(total); edge.alloc(total);
+    if (tb) tb->alloc(total);
     if (total)
         LAUNCH(k_ee_ref_fill, grid_for(B.A.E, 256, grid), 256, 0, B.A, B.lstart.ptr, B.lo.ptr, B.llen.ptr, B.val.ptr, B.fin, B.pos.ptr,
-               node.ptr, edge.ptr);
-    *bytes += B.bytes() + 12 * total;
+               node.ptr, edge.ptr, tb ? tb->ptr : nullptr);
+    *bytes += B.bytes() + (tb ? 16 : 12) * total;
     return total;
 }
 

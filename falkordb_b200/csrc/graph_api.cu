@@ -901,6 +901,44 @@ GrB_Info B200_var_len_reach_both(GrB_Matrix *reached, const GrB_Index *starts, G
     return GrB_SUCCESS;
 }
 
+// ---- allShortestPaths((a)-[:R*..max]->(b)) for a batch of bound pairs (AllShortestPathsOp::expand_row,
+// all_shortest_paths.rs:82-302): all_shortest_paths.cu.  The type layers are read as B200_expand_edges reads them, the transpose
+// of every type included: the paths are recovered from dst over incoming edges.
+GrB_Info B200_all_shortest_paths(const GrB_Index *src, const GrB_Index *dst, GrB_Index npairs, const B200_TensorLayers *types,
+                                 int ntypes, int dir, uint64_t max_hops, const uint64_t *first, uint64_t *out_count, uint32_t *out_len,
+                                 uint64_t *out_p, uint64_t *path_edge, uint32_t *path_node, uint64_t edge_capacity, uint64_t *nedges) {
+    CHECK_PTR(types); CHECK_PTR(out_p); CHECK_PTR(nedges);
+    if (npairs) { CHECK_PTR(src); CHECK_PTR(dst); CHECK_PTR(out_count); CHECK_PTR(out_len); }
+    if (path_edge) CHECK_PTR(path_node);
+    if (ntypes < 1 || ntypes > 65536 || (dir != B200_DIR_OUT && dir != B200_DIR_BOTH)) {
+        tl_error = "all_shortest_paths: ntypes outside 1 .. 65536, or dir not OUT / BOTH"; return GrB_INVALID_VALUE;
+    }
+    GrB_Info info = layers_check("all_shortest_paths", types, ntypes, true);
+    if (info) return info;
+    const u64 nv = types[0].m->nrows;
+    for (u64 i = 0; i < npairs; i++)
+        if (src[i] >= nv || dst[i] >= nv) { tl_error = "all_shortest_paths: src or dst out of range"; return GrB_INVALID_INDEX; }
+    if (npairs == 0 || max_hops == 0) {          // no path: empty rows
+        for (u64 i = 0; i < npairs; i++) { out_count[i] = 0; out_len[i] = 0; }
+        for (u64 i = 0; i <= npairs; i++) out_p[i] = 0;
+        *nedges = 0;
+        return GrB_SUCCESS;
+    }
+    info = device_ready();                       // no device: fail before any host work
+    if (info) return info;
+    return guarded([&]() {
+        GpuLock g;
+        MultiLock lk = lock_all(types, ntypes);
+        ensure_init();
+        const u64 fl = all_shortest_paths((const u64 *)src, (const u64 *)dst, npairs, edge_types_dev(types, ntypes, B200_DIR_BOTH), dir,
+                                          nv, max_hops, (u64)std::max<i64>(0, ctx().opt_shortest_path_budget), first, out_count,
+                                          out_len, out_p, path_edge, path_node, edge_capacity, nedges);
+        Context &cx = ctx();
+        cx.last_flops = fl; cx.total_flops += fl;
+        return GrB_SUCCESS;
+    });
+}
+
 // ---- shortestPath((a)-[:R*min..max]->(b)) for a batch of bound pairs (ExprEval::eval_shortest_path, eval.rs:1296-1513) ----
 // The reference runs a bidirectional BFS per row over versioned row iterators.  Here the pairs other than src == dst run together
 // (shortest_path.cu): each side's neighbours are the union of its operands' effective rows, read from the layers as they stand.

@@ -6,6 +6,7 @@
 #include "algo_bfs.hpp"
 #include "algo_procs.hpp"
 #include "shortest_path.hpp"
+#include "all_shortest_paths.hpp"
 #include <functional>
 #include <map>
 #include <set>
@@ -1491,6 +1492,33 @@ int fdbh_shortest_path(void *adj, void **all_types, uint64_t nall, void **named,
             memcpy(*dst, v.data(), sizeof(uint64_t) * v.size());
         };
         out(out_p, r.p); out(out_nodes, r.nodes); out(out_ep, r.ep); out(out_ids, r.ids);
+        return 0;
+    } catch (const std::exception &e) { g_msg = e.what(); return 1; }
+}
+
+// allShortestPaths (all_shortest_paths.hpp).  all_types / named: Tensor pointers (nnamed = 0: no type named; a null entry: a named
+// type the graph lacks); max_hops UINT64_MAX unbounded.  route 0: all_shortest_paths (B200_all_shortest_paths, count then windows
+// of at most `window` edges); 1: all_shortest_paths_by_iter (expand_row over TypesAdjacency).  Outputs (malloc'ed; free with
+// fdbh_free): pp[npairs + 1] over paths, count[npairs], len[npairs], the edges and the nodes (AllShortestPathsResult's layout).
+int fdbh_all_shortest_paths(void **all_types, uint64_t nall, void **named, uint64_t nnamed, int directed, uint64_t max_hops,
+                            const uint64_t *srcs, const uint64_t *dsts, uint64_t npairs, int route, uint64_t window, uint64_t **out_pp,
+                            uint64_t **out_count, uint64_t **out_len, uint64_t **out_edges, uint64_t **out_nodes) {
+    try {
+        AllShortestPathsQuery q;
+        for (uint64_t k = 0; k < nall; k++) q.all_types.push_back((const Tensor *)all_types[k]);
+        for (uint64_t k = 0; k < nnamed; k++) q.named.push_back((const Tensor *)named[k]);
+        q.directed = directed != 0; q.max_hops = max_hops;
+        if (npairs) { q.srcs.assign(srcs, srcs + npairs); q.dsts.assign(dsts, dsts + npairs); }
+        AllShortestPathsResult r;
+        if (route == 0) r = all_shortest_paths(q, window);
+        else if (route == 1) r = all_shortest_paths_by_iter(q);
+        else throw std::invalid_argument("all_shortest_paths: unknown route");
+        auto out = [](uint64_t **dst, const std::vector<uint64_t> &v) {
+            *dst = (uint64_t *)malloc(sizeof(uint64_t) * (v.size() + 1));
+            if (!*dst) throw std::bad_alloc();
+            memcpy(*dst, v.data(), sizeof(uint64_t) * v.size());
+        };
+        out(out_pp, r.pp); out(out_count, r.count); out(out_len, r.len); out(out_edges, r.edges); out(out_nodes, r.nodes);
         return 0;
     } catch (const std::exception &e) { g_msg = e.what(); return 1; }
 }

@@ -200,6 +200,15 @@ struct SpOperand { const DevCSR *m, *dp, *dm; };
 u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<SpOperand> &fwd, const std::vector<SpOperand> &bwd,
                   u64 n, u64 max_hops, u64 budget, std::vector<u64> &len, std::vector<u32> &nodes);
 
+// all_shortest_paths.cu : allShortestPaths' every shortest path (B200_all_shortest_paths) for np >= 1 pairs (< n and max_hops >= 1,
+// checked by the caller) over relationship types' live layers (every type with its transpose), dir 0 out / 2 both.  Per pair:
+// count (saturating), len (edges per path, 0 when none), out_p (np + 1, paths written, a prefix); path_edge null: count only,
+// else from rank h_first[i] (null: 0) on, pair after pair, until a path no longer fits edge_capacity.  budget: candidates per
+// piece of a forward level (0: from free memory).  Returns the adjacency entries scanned.
+u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<EdgeTypeDev> &types, int dir, u64 n,
+                       u64 max_hops, u64 budget, const u64 *h_first, u64 *count, u32 *len, u64 *out_p, u64 *path_edge,
+                       u32 *path_node, u64 edge_capacity, u64 *nedges);
+
 // adj.cu : the induced effective layer (B200_adjacency_delta).  out = L \ dm restricted to kept rows and columns, both indices
 // replaced by their rank: d_keep null, rank(v) = v below n_out (out is n_out x n_out); else d_keep[0 .. nkeep) strictly ascending
 // and rank_tab from adj_rank_table (out is nkeep x nkeep).  dm may be null.  Pattern only.

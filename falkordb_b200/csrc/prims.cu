@@ -154,7 +154,8 @@ const char *timed_name(int id) {
     static const char *names[] = {"bits_pull", "bits_push", "heavy_accumulate", "small_rows", "bits_fill",
                                   "bits_count", "bitmap_expand", "bfs_expand", "union", "filter", "mxv_fp64", "spgemm_masked", "transpose",
                                   "bits_delta", "bits_repair", "bits_pull_acc", "bits_push_acc", "edge_expand", "bfs_delta", "adj_build",
-                                  "tensor_write", "var_len_trails", "var_len_reach_both", "shortest_path"};
+                                  "tensor_write", "var_len_trails", "var_len_reach_both", "shortest_path",
+                                  "all_shortest_paths"};
     return (id >= 0 && id < TK_COUNT_) ? names[id] : "?";
 }
 static cudaEvent_t get_event() {

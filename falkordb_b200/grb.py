@@ -715,3 +715,36 @@ def shortest_path(src, dst, fwd, bwd, min_hops=1, max_hops=None, fwd_deltas=None
         cap = nn.value
     check(info)
     return [nodes[out_p[i]:out_p[i + 1]].copy() if out_p[i + 1] > out_p[i] else None for i in range(n)]
+
+
+def all_shortest_paths(src, dst, types, dir=DIR_OUT, max_hops=None, first=None, edge_capacity=None):
+    """B200_all_shortest_paths: allShortestPaths((a)-[*..max_hops]->(b)) for the pairs (src[i], dst[i]) over relationship types
+    (`types` as expand_edges takes them; mt required), dir DIR_OUT or DIR_BOTH; max_hops None: unbounded.  edge_capacity 0: count
+    only; None: room for every path; else pairs fill from rank first[i] (None: 0) on until a path no longer fits.  Returns a dict
+    of numpy arrays: count and len per pair, p (paths written, a prefix over pairs), edges and nodes (path k's edges are
+    edges[E_k : E_k + len], E_k the edges of the paths before it; its nodes nodes[E_k + k : E_k + k + len + 1])."""
+    src, dst = _u64arr(src), _u64arr(dst)
+    assert len(src) == len(dst), "one dst per src"
+    n = len(src)
+    fs = None if first is None else _u64arr(first)
+    ls = _layers(types)
+    count, ln, p = np.zeros(max(1, n), np.uint64), np.zeros(max(1, n), np.uint32), np.zeros(n + 1, np.uint64)
+    ne = U64(0)
+    mh = (1 << 64) - 1 if max_hops is None else int(max_hops)
+
+    def call(pe, pn, cap):
+        check(lib().B200_all_shortest_paths(src.ctypes.data if n else None, dst.ctypes.data if n else None, n, ls, len(types), int(dir),
+                                            mh, None if fs is None else fs.ctypes.data, count.ctypes.data, ln.ctypes.data, p.ctypes.data,
+                                            None if pe is None else pe.ctypes.data, None if pn is None else pn.ctypes.data, cap,
+                                            C.byref(ne)))
+    if edge_capacity is None:
+        call(None, None, 0)
+        f = np.zeros(n, np.uint64) if fs is None else fs
+        edge_capacity = int(sum(int(c - min(c, x)) * int(l) for c, x, l in zip(count[:n], f, ln[:n])))
+    edges, nodes = np.zeros(max(1, edge_capacity), np.uint64), np.zeros(max(1, 2 * edge_capacity), np.uint32)
+    if edge_capacity:
+        call(edges, nodes, edge_capacity)
+    else:
+        call(None, None, 0)
+    return {"count": count[:n].copy(), "len": ln[:n].copy(), "p": p, "edges": edges[:ne.value].copy(),
+            "nodes": nodes[:ne.value + int(p[n])].copy()}

@@ -3,7 +3,8 @@ Tensor built by GRAPH.BULK's device-side load and changed by batched writes that
 or the device plans, B200_Tensor_insert_plan / B200_Tensor_remove_plan), and the routes that read its
 relationship ids (B200_expand_edges, Tensor::get per pair, bind_edge's traversal-then-get), CondVarLenTraverse's trails
 (B200_var_len_trails, or the reference's DFS) and its bidirectional DISTINCT endpoints (B200_var_len_reach_both), the shortestPath
-expression (B200_shortest_path, or the reference's NeighborIter BFS), and the algo.BFS, algo.pageRank, algo.WCC
+expression (B200_shortest_path, or the reference's NeighborIter BFS), allShortestPaths (B200_all_shortest_paths, or
+the reference's expand_row), and the algo.BFS, algo.pageRank, algo.WCC
 and algo.labelPropagation procedures over them."""
 import ctypes as C
 import os
@@ -18,6 +19,7 @@ _L = None
 ROUTE_DEVICE, ROUTE_BY_GET, ROUTE_TRAVERSE_GET = 0, 1, 2
 BFS_DEVICE, BFS_BY_EXTRACT = 0, 1
 SP_DEVICE, SP_BY_ITER = 0, 1
+ASP_DEVICE, ASP_BY_ITER = 0, 1
 ALGO_DEVICE, ALGO_BY_EXTRACT = 0, 1
 WRITE_REFERENCE, WRITE_DEVICE = 0, 1
 
@@ -53,6 +55,7 @@ def host():
     L.fdbh_var_len_trails_dfs.argtypes = vl + [P] * 5 + [C.POINTER(U64)] * 2
     L.fdbh_var_len_reach_both.argtypes = [P, U64, P, U64, U64, U64, C.POINTER(P), C.POINTER(P), C.POINTER(U64)]
     L.fdbh_shortest_path.argtypes = [P, P, U64, P, U64, C.c_int, U64, U64, P, P, U64, C.c_int] + [C.POINTER(P)] * 4
+    L.fdbh_all_shortest_paths.argtypes = [P, U64, P, U64, C.c_int, U64, P, P, U64, C.c_int, U64] + [C.POINTER(P)] * 5
     L.fdbh_algo_bfs.argtypes = [P, P, U64, P, U64, P, U64, U64, C.c_int64, C.c_int, C.c_int, P, C.POINTER(U64), P, C.POINTER(U64)]
     algo = [P, P, U64, P, U64, P, U64, U64, P, U64]
     L.fdbh_algo_pagerank.argtypes = algo + [C.c_int, P, P, C.POINTER(U64)]
@@ -325,6 +328,39 @@ def shortest_path(adj, all_types, named, srcs, dsts, directed=True, min_hops=1, 
     for x in ptrs:
         L.fdbh_free(x)
     return [(nodes[p[i]:p[i + 1]], ids[ep[i]:ep[i + 1]]) if p[i + 1] > p[i] else None for i in range(n)]
+
+
+def all_shortest_paths(all_types, named, srcs, dsts, directed=True, max_hops=None, route=ASP_DEVICE, window=1 << 22):
+    """fdbh_all_shortest_paths: allShortestPaths((a)-[:named*..max_hops]->(b)) per pair (srcs[i], dsts[i]) over `named` Tensors (None
+    entries: types the graph lacks), or over `all_types` when none is named; directed False: both directions.  route ASP_DEVICE
+    drains B200_all_shortest_paths in windows of at most `window` edges.  Returns one list per pair of its paths, in the
+    reference's emission order, each (edges, nodes) as lists."""
+    L = host()
+    s, d = _u64(srcs, dsts)
+    arr = lambda xs: (C.c_void_p * max(1, len(xs)))(*[None if x is None else x.h for x in xs])
+    named = list(named or ())
+    ptrs = [C.c_void_p() for _ in range(5)]
+    rc = L.fdbh_all_shortest_paths(arr(all_types), len(all_types), arr(named), len(named), 1 if directed else 0,
+                                   (1 << 64) - 1 if max_hops is None else int(max_hops), s.ctypes.data, d.ctypes.data, len(s), route,
+                                   int(window), *[C.byref(x) for x in ptrs])
+    if rc:
+        raise RuntimeError(L.fdbh_last_message().decode())
+    n = len(s)
+    get = lambda k, m: np.frombuffer((C.c_char * (8 * m)).from_address(ptrs[k].value), np.uint64).tolist() if m else []
+    pp, count, ln = get(0, n + 1), get(1, n), get(2, n)
+    ne = sum(c * l for c, l in zip(count, ln))
+    edges, nodes = get(3, ne), get(4, ne + pp[-1])
+    for x in ptrs:
+        L.fdbh_free(x)
+    out, e = [], 0
+    for i in range(n):
+        paths = []
+        for _ in range(count[i]):
+            k = len(paths) + pp[i]
+            paths.append((edges[e:e + ln[i]], nodes[e + k:e + k + ln[i] + 1]))
+            e += ln[i]
+        out.append(paths)
+    return out
 
 
 def _algo(fn, dt, adj, all_types, named, labels, node_count, deleted, route, *extra):

@@ -453,6 +453,30 @@ GrB_Info B200_var_len_trails(const GrB_Index *starts, const int64_t *dests, GrB_
  * empty rows, no device work.  No layer changes, apart from finishing pending tuples; no base is downloaded. */
 GrB_Info B200_var_len_reach_both(GrB_Matrix *reached, const GrB_Index *starts, GrB_Index nstarts, const B200_TensorLayers *types,
                                  int ntypes, uint64_t min_hops, uint64_t max_hops);
+/* allShortestPaths((a)-[:R1|R2*..max_hops]->(b)) for npairs bound pairs (AllShortestPathsOp::expand_row,
+ * all_shortest_paths.rs:82-302): every shortest path from src[i] to dst[i] over ntypes tensors' live layers, in the reference's
+ * emission order.  Adjacency is Graph::get_node_relationships_by_type's (see B200_var_len_trails); dir B200_DIR_OUT walks outgoing
+ * edges (a right-to-left pattern still walks them from the arrow's source), B200_DIR_BOTH both halves.  min_hops is 1 (the
+ * reference's planner rejects anything else); max_hops = UINT64_MAX: unbounded.  src[i] == dst[i] asks for the shortest cycles.
+ * The order: a BFS from src in adjacency order records every entry into a node from the level before it (its predecessors, in
+ * visit order); the paths are a DFS from dst that pushes a node's predecessors in list order, so the last one pops first.
+ * Outputs, always written: out_count[i] (the number of shortest paths, saturating at UINT64_MAX; 0 = none), out_len[i] (edges
+ * per path, 0 when none), out_p[npairs + 1] (paths written, a prefix over pairs) and *nedges (edges written).  path_edge NULL:
+ * count only.  Otherwise pairs are filled in order, pair i from rank first[i] on (first NULL: 0), and filling stops at the first
+ * path whose edges no longer fit edge_capacity; a caller drains a pair across calls with first[i] += paths written.  Path k's
+ * edges are path_edge[E_k .. E_k + len), E_k = the edges of the paths before it, in src -> dst walk order, except for
+ * src == dst, whose list starts with the closing edge (the reference keeps a cycle's predecessor-chain order); its nodes are
+ * path_node[E_k + k .. E_k + k + len] following the edge list from src (at most 2 * edge_capacity entries).  A caller reverses
+ * both lists for a right-to-left pattern.  Every type needs mt (the paths are recovered from dst over incoming edges).
+ * Errors: NULL pointers or a NULL m / mt GrB_NULL_POINTER; ntypes outside 1 .. 65536 or dir not OUT / BOTH GrB_INVALID_VALUE;
+ * m / dp not UINT64 GrB_DOMAIN_MISMATCH; layers not square of one size GrB_DIMENSION_MISMATCH; an endpoint >= n
+ * GrB_INVALID_INDEX; host-resident layers GrB_NOT_IMPLEMENTED; with no device GxB_GPU_ERROR before any host work.  npairs == 0
+ * or max_hops == 0: success with empty rows and no device work.  last_flops = the adjacency entries scanned.  No layer changes,
+ * apart from finishing pending tuples; no base is downloaded.  Option "shortest_path_budget": candidates per piece of a forward
+ * level (0: sized from free device memory). */
+GrB_Info B200_all_shortest_paths(const GrB_Index *src, const GrB_Index *dst, GrB_Index npairs, const B200_TensorLayers *types,
+                                 int ntypes, int dir, uint64_t max_hops, const uint64_t *first, uint64_t *out_count, uint32_t *out_len,
+                                 uint64_t *out_p, uint64_t *path_edge, uint32_t *path_node, uint64_t edge_capacity, uint64_t *nedges);
 /* Flags of the write plans below. */
 #define B200_PLAN_COMMITTED 0x01 /* insert: m holds the pair, its value is to be reconciled (dm.erase) */
 #define B200_PLAN_CANCEL 0x02    /* insert: COMMITTED and m's value equals the new inline value (dp.erase instead of dp.insert) */
@@ -500,7 +524,8 @@ void B200_reset_stats(void);
  * products of union hops, "bits_pull_acc" and "bits_push_acc", "transpose", "bfs_expand", B200_bfs_delta's kernels over
  * dirty operands, "bfs_delta", B200_adjacency_delta's induced-layer kernels, "adj_build", B200_var_len_trails' kernels,
  * "var_len_trails", B200_var_len_reach_both's own kernels (its reach and closure levels count under the hop families),
- * "var_len_reach_both", and B200_shortest_path's, "shortest_path".  0 on success. */
+ * "var_len_reach_both", B200_shortest_path's, "shortest_path", and B200_all_shortest_paths' (its adjacency fetches included),
+ * "all_shortest_paths".  0 on success. */
 int B200_kernel_stats(const char *name, double *ms, uint64_t *launches, uint64_t *bytes);
 /* options: "bits_mode" (-1 auto,0 off,1 on), "pull_mode" (-1 auto,0 push,1 pull), "small_cap",
  * "bitmap_budget", "bits_min_flops", "timing" (0/1), "sync_after_op" (0/1) */
