@@ -23,21 +23,6 @@
 
 namespace b200 {
 
-static const u64 AS_NONE = ~0ULL;
-static const int AS_KEY_BITS = 43;        // slot (< 1024) << 32 | v, and AS_NONE above every key in the low 43 bits
-static const u32 AS_T = 256;
-
-static int as_bits(u64 x) { int b = 1; while (b < 64 && (x >> b)) b++; return b; }   // bits that hold every value <= x
-
-__device__ __forceinline__ bool as_seen(const u64 *__restrict__ vis, u64 nw, u64 slot, u32 v) {
-    return (vis[slot * nw + (v >> 6)] >> (v & 63)) & 1;
-}
-__device__ __forceinline__ u64 as_lb(const u64 *__restrict__ k, u64 n, u64 key) {
-    u64 a = 0, b = n;
-    while (a < b) { u64 mid = (a + b) >> 1; if (k[mid] < key) a = mid + 1; else b = mid; }
-    return a;
-}
-
 // one ancestor level of the backward phase: keys ascending; predecessors of key a at ps[a] .. ps[a+1], each with its ancestor
 // index pu in the level below, its relationship id and its suffix count; cnt[a] = suf[ps[a]] (level 0: 1)
 struct AsBack { const u64 *key; u64 n; const u64 *ps; const u32 *pu; const u64 *pedge; const u64 *suf; const u64 *cnt; };
@@ -52,43 +37,8 @@ __global__ void k_as_seed(const u64 *__restrict__ src, u64 S, u64 nw, u64 *__res
 __global__ void k_as_iota(u64 *__restrict__ x, u64 n) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) x[i] = i;
 }
-__global__ void k_as_low(const u64 *__restrict__ key, u64 n, u64 *__restrict__ out) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) out[i] = (u32)key[i];
-}
-// sorted keys -> run heads (head[n] = 0), and the heads compacted
-__global__ void k_as_heads(const u64 *__restrict__ k, u64 n, u32 *__restrict__ head) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e <= n; e += (u64)gridDim.x * blockDim.x)
-        head[e] = e < n && (e == 0 || k[e] != k[e - 1]) ? 1 : 0;
-}
-__global__ void k_as_compact(const u64 *__restrict__ k, u64 n, const u32 *__restrict__ head, const u64 *__restrict__ hpos,
-                             u64 *__restrict__ out) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x)
-        if (head[e]) out[hpos[e]] = k[e];
-}
-
-// per (slot << 32 | v) entry: its node's row among the distinct nodes u (ascending) and its adjacency length; deg[n] = 0
-__global__ void k_as_rows(const u64 *__restrict__ key, u64 n, const u64 *__restrict__ u, u64 nu, const u64 *__restrict__ adj_p,
-                          u32 *__restrict__ row, u64 *__restrict__ deg) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (u64)gridDim.x * blockDim.x) {
-        u64 d = 0;
-        if (i < n) {
-            const u64 a = as_lb(u, nu, (u32)key[i]);
-            row[i] = (u32)a;
-            d = adj_p[a + 1] - adj_p[a];
-        }
-        deg[i] = d;
-    }
-}
-
-// the end of the piece starting at front entry i0: the last i1 with cum[i1] - cum[i0] <= budget, at least i0 + 1
-__global__ void k_as_cut(const u64 *__restrict__ cum, u64 i0, u64 nf, u64 budget, u64 *__restrict__ out) {
-    u64 a = i0 + 1, b = nf;
-    while (a < b) { u64 mid = (a + b + 1) >> 1; if (cum[mid] - cum[i0] <= budget) a = mid; else b = mid - 1; }
-    *out = a;
-}
-
 // candidate q of the piece (global position g = q0 + q, in (rank, adjacency position) order): kept with key (slot << 32 | v) when
-// the slot has not seen v, else AS_NONE; an entry into the slot's dst marks the slot found
+// the slot has not seen v, else SLOT_NONE; an entry into the slot's dst marks the slot found
 __global__ void k_as_emit(const u64 *__restrict__ front, const u64 *__restrict__ cum, u64 i0, u64 i1, u64 q0, u64 R,
                           const u32 *__restrict__ row, const u64 *__restrict__ adj_p, const u32 *__restrict__ adj_node,
                           const u64 *__restrict__ dst, const u64 *__restrict__ vis, u64 nw, u32 *__restrict__ found,
@@ -96,13 +46,12 @@ __global__ void k_as_emit(const u64 *__restrict__ front, const u64 *__restrict__
     u64 kept = 0;
     for (u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x; q < R; q += (u64)gridDim.x * blockDim.x) {
         const u64 g = q0 + q;
-        u64 a = i0, b = i1 - 1;                              // the last front entry with cum <= g
-        while (a < b) { u64 mid = (a + b + 1) >> 1; if (cum[mid] <= g) a = mid; else b = mid - 1; }
+        const u64 a = i0 + list_at(cum + i0, i1 - i0, g);     // the last front entry with cum <= g
         const u64 s = front[a] >> 32;
         const u32 v = adj_node[adj_p[row[a]] + (g - cum[a])];
         if (v == (u32)dst[s]) found[s] = 1;
-        const bool live = !as_seen(vis, nw, s, v);
-        key[q] = live ? (s << 32 | v) : AS_NONE;
+        const bool live = !slot_seen(vis, nw, s, v);
+        key[q] = live ? (s << 32 | v) : SLOT_NONE;
         val[q] = g;
         kept += live;
     }
@@ -132,11 +81,6 @@ __global__ void k_as_live(const u64 *__restrict__ front, u64 n, const u32 *__res
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (u64)gridDim.x * blockDim.x)
         flag[i] = i < n && !sdep[front[i] >> 32] ? 1 : 0;
 }
-__global__ void k_as_keep(const u64 *__restrict__ in, u64 n, const u32 *__restrict__ flag, const u64 *__restrict__ pos,
-                          u64 *__restrict__ out) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x)
-        if (flag[i]) out[pos[i]] = in[i];
-}
 
 // backward candidate q (ancestor a, its reverse-adjacency entry): kept when the far end u is in forward level l - 1 of the slot,
 // with sort key (rank(u), type, half as u sees it).  A reverse entry of v's outgoing half is in u's incoming half, except a
@@ -149,7 +93,7 @@ __global__ void k_as_back(const u64 *__restrict__ akey, const u64 *__restrict__ 
         const u64 a = list_at(cum, na, q), k = akey[a], s = k >> 32;
         const u64 pos = adj_p[row[a]] + (q - cum[a]);
         const u32 x = adj_node[pos], tb = adj_tb[pos];
-        const u64 uk = s << 32 | x, f = as_lb(fkey, fn, uk);
+        const u64 uk = s << 32 | x, f = lb64(fkey, 0, fn, uk);
         const bool in = f < fn && fkey[f] == uk;
         keep[q] = in;
         if (in) k1[q] = frank[f] << 18 | (u64)(tb >> 1) << 1 | (!(tb & 1) && x != (u32)k ? 1 : 0);
@@ -175,11 +119,11 @@ __global__ void k_as_preds(const u64 *__restrict__ q, const u64 *__restrict__ an
     }
 }
 __global__ void k_as_ps(const u64 *__restrict__ anc, u64 E, u64 na, u64 *__restrict__ ps) {
-    for (u64 a = (u64)blockIdx.x * blockDim.x + threadIdx.x; a <= na; a += (u64)gridDim.x * blockDim.x) ps[a] = as_lb(anc, E, a);
+    for (u64 a = (u64)blockIdx.x * blockDim.x + threadIdx.x; a <= na; a += (u64)gridDim.x * blockDim.x) ps[a] = lb64(anc, 0, E, a);
 }
 // pu[j] = the position of predecessor j's far end in the ancestor level below
 __global__ void k_as_pu(const u64 *__restrict__ pkey, u64 E, const u64 *__restrict__ key, u64 n, u32 *__restrict__ pu) {
-    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < E; j += (u64)gridDim.x * blockDim.x) pu[j] = (u32)as_lb(key, n, pkey[j]);
+    for (u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x; j < E; j += (u64)gridDim.x * blockDim.x) pu[j] = (u32)lb64(key, 0, n, pkey[j]);
 }
 
 // counts, top-down: per ancestor of level l >= 1 the saturating suffix sums of its predecessors' counts
@@ -189,7 +133,7 @@ __global__ void k_as_count(u64 n, const u64 *__restrict__ ps, const u32 *__restr
         u64 c = 0;
         for (u64 j = ps[a + 1]; j-- > ps[a];) {
             const u64 x = below[pu[j]];
-            c = c + x < c ? AS_NONE : c + x;
+            c = c + x < c ? SLOT_NONE : c + x;
             suf[j] = c;
         }
         cnt[a] = c;
@@ -201,7 +145,7 @@ __global__ void k_as_total(u64 S, const u32 *__restrict__ sdep, const u64 *__res
         u64 c = 0, p = 0;
         if (sdep[s]) {
             const AsBack &L = B[sdep[s]];
-            p = as_lb(L.key, L.n, s << 32 | (u32)dst[s]);
+            p = lb64(L.key, 0, L.n, s << 32 | (u32)dst[s]);
             c = L.cnt[p];
         }
         count[s] = c; dpos[s] = p;
@@ -242,41 +186,6 @@ __global__ void k_as_fill(u64 W, u64 S, const u64 *__restrict__ woff, const u64 
 
 // ---- host side ----
 
-// keys[0 .. n) sorted and deduplicated in place; returns the distinct count
-static u64 as_unique(DevBuf<u64> &keys, u64 n, int bits) {
-    if (!n) return 0;
-    sort_keys_u64(keys.ptr, n, bits);
-    DevBuf<u32> head(n + 1);
-    DevBuf<u64> hpos(n + 1), out;
-    LAUNCH(k_as_heads, grid_for(n + 1, AS_T), AS_T, 0, keys.ptr, n, head.ptr);
-    exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, n + 1);
-    const u64 m = read_scalar(hpos.ptr + n);
-    out.alloc(m);
-    LAUNCH(k_as_compact, grid_for(n, AS_T), AS_T, 0, keys.ptr, n, head.ptr, hpos.ptr, out.ptr);
-    keys = std::move(out);
-    return m;
-}
-
-// the adjacency (direction dir) of the distinct nodes of keys[0 .. n) (slot << 32 | v), and per key its row and the scan of
-// the rows' lengths (cum[n] = the total)
-struct AsAdj {
-    DevBuf<u64> u, p, edge, cum;
-    DevBuf<u32> node, tb, row;
-    u64 total = 0;
-    void fetch(const EType *dt, u32 T, const u64 *keys, u64 n, int dir, bool want_tb, u64 *bytes) {
-        u.alloc(n);
-        LAUNCH(k_as_low, grid_for(n, AS_T), AS_T, 0, keys, n, u.ptr);
-        const u64 nu = as_unique(u, n, 32);
-        edge_adjacency(dt, T, u.ptr, nu, dir, p, node, edge, bytes, want_tb ? &tb : nullptr);
-        row.alloc(n);
-        cum.alloc(n + 1);
-        LAUNCH(k_as_rows, grid_for(n + 1, AS_T), AS_T, 0, keys, n, u.ptr, nu, p.ptr, row.ptr, cum.ptr);
-        exclusive_scan_u64(cum.ptr, cum.ptr, n + 1);
-        total = read_scalar(cum.ptr + n);
-        *bytes += 24 * n;
-    }
-};
-
 struct AsLevel { DevBuf<u64> key, rank; u64 n = 0; };       // a forward level: its keys ascending, each with its rank
 struct AsAnc {                                              // a backward ancestor level (AsBack's arrays)
     DevBuf<u64> key, ps, pedge, pkey, suf, cnt;
@@ -287,21 +196,12 @@ struct AsAnc {                                              // a backward ancest
 u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<EdgeTypeDev> &types, int dir, u64 n,
                        u64 max_hops, u64 budget, const u64 *h_first, u64 *count, u32 *len, u64 *out_p, u64 *path_edge,
                        u32 *path_node, u64 edge_capacity, u64 *nedges) {
-    const u32 T = (u32)types.size();
-    std::vector<EType> ht(T);
-    for (u32 t = 0; t < T; t++) {
-        const EdgeTypeDev &x = types[t];
-        ht[t] = EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
-                      estore(x.me_dm)};
-    }
-    DevBuf<EType> dt(T);
-    h2d(dt.ptr, ht.data(), T);
+    const ETypes ty(types);
     const int rdir = dir == 0 ? 1 : 2;                      // the reverse adjacency: incoming edges, or both halves
     const u64 nw = (n + 63) / 64;
     size_t fr = 0, tot = 0;
     CUDA_TRY(cudaMemGetInfo(&fr, &tot));
-    // as B200_shortest_path: a piece of a forward level holds about 80 bytes per candidate; a sixteenth of free memory by default
-    if (!budget) budget = std::min<u64>((u64)1 << 30, std::max<u64>((u64)1 << 16, fr / 16 / 80));
+    budget = piece_budget(budget, fr);
     const u64 S_max = std::max<u64>(1, std::min<u64>(1024, fr / 4 / (nw * 8)));
     // Compulsory bytes ("all_shortest_paths"): the adjacency fetches (edge_expand's formula plus 12 per entry written, 16 with the
     // type and half) and 24 per fetched key (its node, row and length); per forward candidate 28 (its neighbour, the visited word,
@@ -320,7 +220,7 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
         h2d(ddst.ptr, h_dst + p0, S);
         DevBuf<u64> vis(S * nw), front(S);
         vis.zero();
-        LAUNCH(k_as_seed, grid_for(S, AS_T), AS_T, 0, dsrc.ptr, S, nw, front.ptr, vis.ptr);
+        LAUNCH(k_as_seed, grid_for(S, PAIR_T), PAIR_T, 0, dsrc.ptr, S, nw, front.ptr, vis.ptr);
         DevBuf<u32> found(S), sdep(S);
         found.zero(); sdep.zero();
         std::vector<AsLevel> lev;
@@ -333,61 +233,45 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             F.n = nf;
             F.key.alloc(nf); F.rank.alloc(nf);
             d2d(F.key.ptr, front.ptr, nf);
-            LAUNCH(k_as_iota, grid_for(nf, AS_T), AS_T, 0, F.rank.ptr, nf);
-            sort_pairs_u64(F.key.ptr, F.rank.ptr, nf, AS_KEY_BITS);
+            LAUNCH(k_as_iota, grid_for(nf, PAIR_T), PAIR_T, 0, F.rank.ptr, nf);
+            sort_pairs_u64(F.key.ptr, F.rank.ptr, nf, SLOT_KEY_BITS);
             bytes += 16 * nf;
-            AsAdj A;
-            A.fetch(dt.ptr, T, front.ptr, nf, dir, false, &bytes);
+            NodeAdj A;
+            A.fetch(ty, front.ptr, nf, dir, false, &bytes);
             const u64 total = A.total;
             flops += total;
+            bytes += 24 * nf;
             DevBuf<u64> next(1), scal(1);
             u64 nnext = 0;
-            const int gbits = as_bits(total);
-            for (u64 i0 = 0, q0 = 0; q0 < total;) {
-                u64 i1 = nf;
-                if (total - q0 > budget) {
-                    LAUNCH(k_as_cut, 1, 1, 0, A.cum.ptr, i0, nf, budget, scal.ptr);
-                    i1 = read_scalar(scal.ptr);
-                }
-                const u64 q1 = i1 < nf ? read_scalar(A.cum.ptr + i1) : total, R = q1 - q0;
-                if (R) {
-                    DevBuf<u64> key(R), val(R);
-                    CUDA_TRY(cudaMemsetAsync(scal.ptr, 0, sizeof(u64), stream()));
-                    LAUNCH(k_as_emit, grid_for(R, AS_T, 8 * (u64)ctx().num_sms), AS_T, 0, front.ptr, A.cum.ptr, i0, i1, q0, R, A.row.ptr,
-                           A.p.ptr, A.node.ptr, ddst.ptr, vis.ptr, nw, found.ptr, key.ptr, val.ptr, scal.ptr);
-                    const u64 E = read_scalar(scal.ptr);
-                    bytes += 28 * R;
-                    if (E) {
-                        sort_pairs_u64(key.ptr, val.ptr, R, AS_KEY_BITS);       // stable: the first to reach v leads its run
-                        DevBuf<u32> head(E + 1);
-                        DevBuf<u64> hpos(E + 1);
-                        LAUNCH(k_as_heads, grid_for(E + 1, AS_T), AS_T, 0, key.ptr, E, head.ptr);
-                        exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, E + 1);
-                        const u64 nh = read_scalar(hpos.ptr + E);
-                        DevBuf<u64> rk(nh), nk(nh);
-                        LAUNCH(k_as_first, grid_for(E, AS_T), AS_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, vis.ptr, nw, rk.ptr,
-                               nk.ptr);
-                        sort_pairs_u64(rk.ptr, nk.ptr, nh, gbits);              // by (rank, adjacency position)
-                        if (next.n < nnext + nh) {
-                            DevBuf<u64> g(std::max<u64>(nnext + nh, 2 * next.n));
-                            d2d(g.ptr, next.ptr, nnext);
-                            next = std::move(g);
-                        }
-                        d2d(next.ptr + nnext, nk.ptr, nh);
-                        nnext += nh;
-                        bytes += 40 * nh;
-                    }
-                }
-                i0 = i1; q0 = q1;
-            }
-            LAUNCH(k_as_stop, grid_for(S, AS_T), AS_T, 0, S, found.ptr, (u32)(L + 1), sdep.ptr);
+            for_each_piece(A.cum.ptr, nf, total, budget, [&](u64 i0, u64 i1, u64 q0, u64 q1) {
+                const u64 R = q1 - q0;
+                DevBuf<u64> key(R), val(R);
+                CUDA_TRY(cudaMemsetAsync(scal.ptr, 0, sizeof(u64), stream()));
+                LAUNCH(k_as_emit, grid_for(R, PAIR_T, 8 * (u64)ctx().num_sms), PAIR_T, 0, front.ptr, A.cum.ptr, i0, i1, q0, R, A.row.ptr,
+                       A.p.ptr, A.node.ptr, ddst.ptr, vis.ptr, nw, found.ptr, key.ptr, val.ptr, scal.ptr);
+                const u64 E = read_scalar(scal.ptr);
+                bytes += 28 * R;
+                if (!E) return;
+                sort_pairs_u64(key.ptr, val.ptr, R, SLOT_KEY_BITS);            // stable: the first to reach v leads its run
+                DevBuf<u32> head(E + 1);
+                DevBuf<u64> hpos(E + 1);
+                const u64 nh = run_heads(key.ptr, E, head.ptr, hpos.ptr);
+                DevBuf<u64> rk(nh), nk(nh);
+                LAUNCH(k_as_first, grid_for(E, PAIR_T), PAIR_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, vis.ptr, nw, rk.ptr, nk.ptr);
+                sort_pairs_u64(rk.ptr, nk.ptr, nh, bit_length(total));         // by (rank, adjacency position)
+                grow(next, nnext, nnext + nh);
+                d2d(next.ptr + nnext, nk.ptr, nh);
+                nnext += nh;
+                bytes += 40 * nh;
+            });
+            LAUNCH(k_as_stop, grid_for(S, PAIR_T), PAIR_T, 0, S, found.ptr, (u32)(L + 1), sdep.ptr);
             DevBuf<u32> flag(nnext + 1);
             DevBuf<u64> fpos(nnext + 1);
-            LAUNCH(k_as_live, grid_for(nnext + 1, AS_T), AS_T, 0, next.ptr, nnext, sdep.ptr, flag.ptr);
+            LAUNCH(k_as_live, grid_for(nnext + 1, PAIR_T), PAIR_T, 0, next.ptr, nnext, sdep.ptr, flag.ptr);
             exclusive_scan_u32_to_u64(flag.ptr, fpos.ptr, nnext + 1);
             nf = read_scalar(fpos.ptr + nnext);
             front.alloc(std::max<u64>(nf, 1));
-            if (nf) LAUNCH(k_as_keep, grid_for(nnext, AS_T), AS_T, 0, next.ptr, nnext, flag.ptr, fpos.ptr, front.ptr);
+            if (nf) scatter_flagged(next.ptr, nnext, flag.ptr, fpos.ptr, front.ptr);
         }
         front.release(); vis.release();
         std::vector<u32> hdep(S);
@@ -406,22 +290,23 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             Y.key.alloc(ncarry + seeds.size());
             d2d(Y.key.ptr, carry.ptr, ncarry);
             h2d(Y.key.ptr + ncarry, seeds.data(), seeds.size());
-            Y.n = as_unique(Y.key, ncarry + seeds.size(), AS_KEY_BITS);
+            Y.n = unique_sorted(Y.key, ncarry + seeds.size(), SLOT_KEY_BITS);
             carry.release(); ncarry = 0;
             if (l + 1 <= Lmax && anc[l + 1].np)             // the level above's predecessors, as positions in this level
-                LAUNCH(k_as_pu, grid_for(anc[l + 1].np, AS_T), AS_T, 0, anc[l + 1].pkey.ptr, anc[l + 1].np, Y.key.ptr, Y.n,
+                LAUNCH(k_as_pu, grid_for(anc[l + 1].np, PAIR_T), PAIR_T, 0, anc[l + 1].pkey.ptr, anc[l + 1].np, Y.key.ptr, Y.n,
                        anc[l + 1].pu.ptr);
             if (l + 1 <= Lmax) anc[l + 1].pkey.release();
             if (l == 0 || !Y.n) continue;
-            AsAdj A;
-            A.fetch(dt.ptr, T, Y.key.ptr, Y.n, rdir, true, &bytes);
+            NodeAdj A;
+            A.fetch(ty, Y.key.ptr, Y.n, rdir, true, &bytes);
             const u64 C = A.total;
+            bytes += 24 * Y.n;
             flops += C;
             DevBuf<u32> keep(C + 1);
             DevBuf<u64> k1(std::max<u64>(C, 1)), kpos(C + 1);
             CUDA_TRY(cudaMemsetAsync(keep.ptr + C, 0, sizeof(u32), stream()));
             const AsLevel &F = lev[l - 1];
-            if (C) LAUNCH(k_as_back, grid_for(C, AS_T), AS_T, 0, Y.key.ptr, A.cum.ptr, Y.n, C, A.row.ptr, A.p.ptr, A.node.ptr, A.tb.ptr,
+            if (C) LAUNCH(k_as_back, grid_for(C, PAIR_T), PAIR_T, 0, Y.key.ptr, A.cum.ptr, Y.n, C, A.row.ptr, A.p.ptr, A.node.ptr, A.tb.ptr,
                           F.key.ptr, F.rank.ptr, F.n, keep.ptr, k1.ptr);
             exclusive_scan_u32_to_u64(keep.ptr, kpos.ptr, C + 1);
             const u64 E = read_scalar(kpos.ptr + C);
@@ -430,15 +315,15 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             Y.ps.alloc(Y.n + 1); Y.pedge.alloc(E); Y.pkey.alloc(E); Y.pu.alloc(E); Y.suf.alloc(E);
             DevBuf<u64> sk(E), sq(E);
             if (E) {
-                LAUNCH(k_as_pack, grid_for(C, AS_T), AS_T, 0, keep.ptr, kpos.ptr, k1.ptr, C, sk.ptr, sq.ptr);
+                LAUNCH(k_as_pack, grid_for(C, PAIR_T), PAIR_T, 0, keep.ptr, kpos.ptr, k1.ptr, C, sk.ptr, sq.ptr);
                 keep.release(); k1.release(); kpos.release();
-                sort_pairs_u64(sk.ptr, sq.ptr, E, as_bits(F.n) + 18);           // (rank(u), type, half), stable on position
-                LAUNCH(k_as_anc, grid_for(E, AS_T), AS_T, 0, sq.ptr, E, A.cum.ptr, Y.n, sk.ptr);
-                sort_pairs_u64(sk.ptr, sq.ptr, E, as_bits(Y.n));                // then by ancestor, stable
-                LAUNCH(k_as_preds, grid_for(E, AS_T), AS_T, 0, sq.ptr, sk.ptr, E, Y.key.ptr, A.cum.ptr, A.row.ptr, A.p.ptr, A.node.ptr,
+                sort_pairs_u64(sk.ptr, sq.ptr, E, bit_length(F.n) + 18);           // (rank(u), type, half), stable on position
+                LAUNCH(k_as_anc, grid_for(E, PAIR_T), PAIR_T, 0, sq.ptr, E, A.cum.ptr, Y.n, sk.ptr);
+                sort_pairs_u64(sk.ptr, sq.ptr, E, bit_length(Y.n));               // then by ancestor, stable
+                LAUNCH(k_as_preds, grid_for(E, PAIR_T), PAIR_T, 0, sq.ptr, sk.ptr, E, Y.key.ptr, A.cum.ptr, A.row.ptr, A.p.ptr, A.node.ptr,
                        A.edge.ptr, Y.pedge.ptr, Y.pkey.ptr);
             }
-            LAUNCH(k_as_ps, grid_for(Y.n + 1, AS_T), AS_T, 0, sk.ptr, E, Y.n, Y.ps.ptr);
+            LAUNCH(k_as_ps, grid_for(Y.n + 1, PAIR_T), PAIR_T, 0, sk.ptr, E, Y.n, Y.ps.ptr);
             carry.alloc(E);
             d2d(carry.ptr, Y.pkey.ptr, E);
             ncarry = E;
@@ -449,13 +334,13 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             AsAnc &Y = anc[l];
             Y.cnt.alloc(std::max<u64>(Y.n, 1));
             if (l == 0) { if (Y.n) fill_u64(Y.cnt.ptr, 1, Y.n); }
-            else if (Y.n) LAUNCH(k_as_count, grid_for(Y.n, AS_T), AS_T, 0, Y.n, Y.ps.ptr, Y.pu.ptr, anc[l - 1].cnt.ptr, Y.suf.ptr, Y.cnt.ptr);
+            else if (Y.n) LAUNCH(k_as_count, grid_for(Y.n, PAIR_T), PAIR_T, 0, Y.n, Y.ps.ptr, Y.pu.ptr, anc[l - 1].cnt.ptr, Y.suf.ptr, Y.cnt.ptr);
             hb[l] = AsBack{Y.key.ptr, Y.n, Y.ps.ptr, Y.pu.ptr, Y.pedge.ptr, Y.suf.ptr, Y.cnt.ptr};
         }
         DevBuf<AsBack> db(Lmax + 1);
         h2d(db.ptr, hb.data(), Lmax + 1);
         DevBuf<u64> dcount(S), dpos(S);
-        LAUNCH(k_as_total, grid_for(S, AS_T), AS_T, 0, S, sdep.ptr, ddst.ptr, db.ptr, dcount.ptr, dpos.ptr);
+        LAUNCH(k_as_total, grid_for(S, PAIR_T), PAIR_T, 0, S, sdep.ptr, ddst.ptr, db.ptr, dcount.ptr, dpos.ptr);
         std::vector<u64> hcount(S);
         d2h(hcount.data(), dcount.ptr, S);
         sync_stream();
@@ -478,7 +363,7 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             DevBuf<u64> dwoff(S + 1), dfirst(S), deoff(S), oedge(ne);
             DevBuf<u32> onode(ne + W);
             h2d(dwoff.ptr, woff.data(), S + 1); h2d(dfirst.ptr, hfirst.data(), S); h2d(deoff.ptr, eoff.data(), S);
-            LAUNCH(k_as_fill, grid_for(W, AS_T), AS_T, 0, W, S, dwoff.ptr, dfirst.ptr, deoff.ptr, sdep.ptr, dsrc.ptr, ddst.ptr, dpos.ptr,
+            LAUNCH(k_as_fill, grid_for(W, PAIR_T), PAIR_T, 0, W, S, dwoff.ptr, dfirst.ptr, deoff.ptr, sdep.ptr, dsrc.ptr, ddst.ptr, dpos.ptr,
                    db.ptr, oedge.ptr, onode.ptr);
             d2h(path_edge + e_used, oedge.ptr, ne);
             d2h(path_node + e_used + w_used, onode.ptr, ne + W);
@@ -493,21 +378,7 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
         }
         e_used += ne; w_used += W; full = stop;
     };
-    // as B200_shortest_path: a slice that runs out of device memory is run again as two halves, down to one pair
-    u64 S_cur = S_max;
-    for (u64 p0 = 0; p0 < np;) {
-        const u64 S = std::min<u64>(S_cur, np - p0);
-        try {
-            run_slice(p0, S);
-        } catch (const CudaError &e) {
-            if (e.code != cudaErrorMemoryAllocation || S == 1) throw;
-            cudaGetLastError();
-            pool_trim();
-            S_cur = S / 2;
-            continue;
-        }
-        p0 += S;
-    }
+    for_each_slice(np, S_max, run_slice);
     out_p[np] = w_used;
     *nedges = e_used;
     ts.bytes = bytes;

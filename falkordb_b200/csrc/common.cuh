@@ -261,4 +261,14 @@ void sort_pairs_u64(u64 *keys_in_out, u64 *vals_in_out, size_t n, int end_bit); 
 u64 reduce_sum_u64(const u64 *in, size_t n);
 void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz);  // every CSR row's entries ascending, in place (uses temp)
 
+// ---- sorted u64 keys (prims.cu) ----
+// head[e] = 1 where a run of equal keys of keys[0 .. n) starts (head[n] = 0), hpos its exclusive scan; returns the runs
+u64 run_heads(const u64 *keys, u64 n, u32 *head, u64 *hpos);
+// out[pos[i]] = in[i] for every i < n with flag[i]
+void scatter_flagged(const u64 *in, u64 n, const u32 *flag, const u64 *pos, u64 *out);
+// keys[0 .. n) sorted over end_bit bits and deduplicated (keys is replaced by the distinct keys); returns their count
+u64 unique_sorted(DevBuf<u64> &keys, u64 n, int end_bit);
+// the bits of x (0 for 0): a sort key holding every value <= x needs this end_bit
+inline int bit_length(u64 x) { int b = 0; while (b < 64 && (x >> b)) b++; return b; }
+
 } // namespace b200

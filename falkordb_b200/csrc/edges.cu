@@ -242,10 +242,16 @@ struct EeBatch {
     u64 bytes() const { return 16 * A.G + 12 * h[0] + 28 * h[1] + 4 * h[2]; }
 };
 
-u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
+ETypes::ETypes(const std::vector<EdgeTypeDev> &types) : d(types.size()), T((u32)types.size()) {
+    std::vector<EType> h(T);
+    for (u32 t = 0; t < T; t++) h[t] = etype(types[t]);
+    h2d(d.ptr, h.data(), T);
+}
+
+u64 edge_adjacency(const ETypes &types, const u64 *d_src, u64 n, int dir, DevBuf<u64> &p, DevBuf<u32> &node, DevBuf<u64> &edge,
                    u64 *bytes, DevBuf<u32> *tb) {
-    const u32 nb = dir == 2 ? 2 : 1, grid = (u32)ctx().num_sms * 8;
-    EeBatch B(EArgs{d_src, nullptr, dt, n, n * nb * T * 2, 0, T, nb, dir});
+    const u32 T = types.T, nb = dir == 2 ? 2 : 1, grid = (u32)ctx().num_sms * 8;
+    EeBatch B(EArgs{d_src, nullptr, types.d.ptr, n, n * nb * T * 2, 0, T, nb, dir});
     B.prepare(0, grid);
     p.alloc(n + 1);
     LAUNCH(k_ee_rowptr, grid_for(n + 1, 256, grid), 256, 0, B.A, B.lstart.ptr, B.pos.ptr, p.ptr);
@@ -261,6 +267,80 @@ u64 edge_adjacency(const EType *dt, u32 T, const u64 *d_src, u64 n, int dir, Dev
     return total;
 }
 
+template <class K>
+__global__ void k_adj_low(const K *__restrict__ key, u64 n, u64 *__restrict__ out) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) out[i] = (u32)key[i];
+}
+template <class K>
+__global__ void k_adj_rows(const K *__restrict__ key, u64 n, const u64 *__restrict__ u, u64 nu, const u64 *__restrict__ adj_p,
+                           u32 *__restrict__ row, u64 *__restrict__ deg) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (u64)gridDim.x * blockDim.x) {
+        u64 d = 0;
+        if (i < n) {
+            const u64 a = lb64(u, 0, nu, (u32)key[i]);
+            row[i] = (u32)a;
+            if (deg) d = adj_p[a + 1] - adj_p[a];
+        }
+        if (deg) deg[i] = d;
+    }
+}
+template <class K>
+void node_rows(const K *keys, u64 n, const u64 *u, u64 nu, const u64 *adj_p, u32 *row, u64 *deg) {
+    LAUNCH(k_adj_rows<K>, grid_for(n + 1, 256), 256, 0, keys, n, u, nu, adj_p, row, deg);
+}
+template <class K>
+void NodeAdj::fetch(const ETypes &types, const K *keys, u64 n, int dir, bool want_tb, u64 *bytes) {
+    u.alloc(n);
+    LAUNCH(k_adj_low<K>, grid_for(n, 256), 256, 0, keys, n, u.ptr);
+    const u64 nu = unique_sorted(u, n, 32);
+    edge_adjacency(types, u.ptr, nu, dir, p, node, edge, bytes, want_tb ? &tb : nullptr);
+    row.alloc(n);
+    cum.alloc(n + 1);
+    node_rows(keys, n, u.ptr, nu, p.ptr, row.ptr, cum.ptr);
+    exclusive_scan_u64(cum.ptr, cum.ptr, n + 1);
+    total = read_scalar(cum.ptr + n);
+}
+template void node_rows<u64>(const u64 *, u64, const u64 *, u64, const u64 *, u32 *, u64 *);
+template void NodeAdj::fetch<u32>(const ETypes &, const u32 *, u64, int, bool, u64 *);
+template void NodeAdj::fetch<u64>(const ETypes &, const u64 *, u64, int, bool, u64 *);
+
+// the end of the piece starting at front entry i0: the last i1 with cum[i1] - cum[i0] <= budget, at least i0 + 1
+__global__ void k_piece_cut(const u64 *__restrict__ cum, u64 i0, u64 nf, u64 budget, u64 *__restrict__ out) {
+    u64 a = i0 + 1, b = nf;
+    while (a < b) { u64 mid = (a + b + 1) >> 1; if (cum[mid] - cum[i0] <= budget) a = mid; else b = mid - 1; }
+    *out = a;
+}
+void for_each_piece(const u64 *cum, u64 nf, u64 total, u64 budget, const std::function<void(u64, u64, u64, u64)> &f) {
+    DevBuf<u64> end(1);
+    for (u64 i0 = 0, q0 = 0; q0 < total;) {
+        u64 i1 = nf;
+        if (total - q0 > budget) {
+            LAUNCH(k_piece_cut, 1, 1, 0, cum, i0, nf, budget, end.ptr);
+            i1 = read_scalar(end.ptr);
+        }
+        const u64 q1 = i1 < nf ? read_scalar(cum + i1) : total;
+        if (q1 > q0) f(i0, i1, q0, q1);
+        i0 = i1; q0 = q1;
+    }
+}
+
+void for_each_slice(u64 np, u64 S_max, const std::function<void(u64, u64)> &run_slice) {
+    u64 S_cur = S_max;
+    for (u64 p0 = 0; p0 < np;) {
+        const u64 S = std::min<u64>(S_cur, np - p0);
+        try {
+            run_slice(p0, S);
+        } catch (const CudaError &e) {
+            if (e.code != cudaErrorMemoryAllocation || S == 1) throw;
+            cudaGetLastError();
+            pool_trim();
+            S_cur = S / 2;
+            continue;
+        }
+        p0 += S;
+    }
+}
+
 void DevIdStore::upload(const u64 *hkey, const u64 *hptr, const u64 *hid, u64 nk) {
     clear();
     nkey = nk;
@@ -274,16 +354,9 @@ void DevIdStore::upload(const u64 *hkey, const u64 *hptr, const u64 *hid, u64 nk
 
 u64 edge_expand(const u64 *d_src, const u64 *d_tgt, u64 n, const std::vector<EdgeTypeDev> &types, int dir, int mode, u64 *out_p,
                 u32 *out_node, u64 *out_edge, uint16_t *out_type, uint8_t *out_rev, u64 capacity) {
-    const u32 T = (u32)types.size(), nb = dir == 2 ? 2 : 1;
-    std::vector<EType> ht(T);
-    for (u32 t = 0; t < T; t++) {
-        const EdgeTypeDev &x = types[t];
-        ht[t] = EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
-                      estore(x.me_dm)};
-    }
-    DevBuf<EType> dt(T);
-    h2d(dt.ptr, ht.data(), T);
-    EArgs A{d_src, d_tgt, dt.ptr, n, n * nb * T * 2, 0, T, nb, dir};
+    const ETypes ty(types);
+    const u32 T = ty.T, nb = dir == 2 ? 2 : 1;
+    EArgs A{d_src, d_tgt, ty.d.ptr, n, n * nb * T * 2, 0, T, nb, dir};
     const u32 grid = (u32)ctx().num_sms * 8;
     DevBuf<u64> out(n + 1);
     if (n == 0) {

@@ -286,6 +286,35 @@ void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz) {
     LAUNCH(k_keys_low, grid_for(nnz, 256, (u64)ctx().num_sms * 32), 256, 0, keys.ptr, nnz, cols);
 }
 
+__global__ void k_run_heads(const u64 *__restrict__ k, u64 n, u32 *__restrict__ head) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e <= n; e += (u64)gridDim.x * blockDim.x)
+        head[e] = e < n && (e == 0 || k[e] != k[e - 1]) ? 1 : 0;
+}
+__global__ void k_scatter_flagged(const u64 *__restrict__ in, u64 n, const u32 *__restrict__ flag, const u64 *__restrict__ pos,
+                                  u64 *__restrict__ out) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x)
+        if (flag[i]) out[pos[i]] = in[i];
+}
+u64 run_heads(const u64 *keys, u64 n, u32 *head, u64 *hpos) {
+    LAUNCH(k_run_heads, grid_for(n + 1, 256), 256, 0, keys, n, head);
+    exclusive_scan_u32_to_u64(head, hpos, n + 1);
+    return read_scalar(hpos + n);
+}
+void scatter_flagged(const u64 *in, u64 n, const u32 *flag, const u64 *pos, u64 *out) {
+    LAUNCH(k_scatter_flagged, grid_for(n, 256), 256, 0, in, n, flag, pos, out);
+}
+u64 unique_sorted(DevBuf<u64> &keys, u64 n, int end_bit) {
+    if (!n) return 0;
+    sort_keys_u64(keys.ptr, n, end_bit);
+    DevBuf<u32> head(n + 1);
+    DevBuf<u64> hpos(n + 1), out;
+    const u64 m = run_heads(keys.ptr, n, head.ptr, hpos.ptr);
+    out.alloc(m);
+    scatter_flagged(keys.ptr, n, head.ptr, hpos.ptr, out.ptr);
+    keys = std::move(out);
+    return m;
+}
+
 u64 reduce_sum_u64(const u64 *in, size_t n) {
     if (n == 0) return 0;
     DevBuf<u64> out(1);

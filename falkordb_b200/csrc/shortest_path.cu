@@ -23,20 +23,14 @@
 namespace b200 {
 
 enum { SP_ACTIVE = 0, SP_FOUND = 1, SP_NULL = 2 };
-static const u64 SP_NONE = ~0ULL;
-static const int SP_KEY_BITS = 43;           // slot (< 1024) << 32 | v, and the sentinel SP_NONE above every key in the low 43 bits
 
 struct SpOp { ECsr m, dp, dm; };
 struct SpChunk { u64 off, n; };
 
-__device__ __forceinline__ bool sp_seen(const u64 *__restrict__ vis, u64 nw, u64 slot, u32 v) {
-    return (vis[slot * nw + (v >> 6)] >> (v & 63)) & 1;
-}
 // (slot, v)'s entry among a side's chunks: its position in lkey (and lval)
 __device__ __forceinline__ bool sp_find(const SpChunk *__restrict__ ch, u32 nch, const u64 *__restrict__ lkey, u64 key, u64 *pos) {
     for (u32 c = 0; c < nch; c++) {
-        u64 a = ch[c].off, b = ch[c].off + ch[c].n;
-        while (a < b) { u64 mid = (a + b) >> 1; if (lkey[mid] < key) a = mid + 1; else b = mid; }
+        const u64 a = lb64(lkey, ch[c].off, ch[c].off + ch[c].n, key);
         if (a < ch[c].off + ch[c].n && lkey[a] == key) { *pos = a; return true; }
     }
     return false;
@@ -70,23 +64,15 @@ __global__ void k_sp_deg(const u64 *__restrict__ front, u64 nf, u32 sd, const u3
     }
 }
 
-// the end of the piece starting at front entry i0: the last i1 with cum[i1] - cum[i0] <= budget, at least i0 + 1
-__global__ void k_sp_cut(const u64 *__restrict__ cum, u64 i0, u64 nf, u64 budget, u64 *__restrict__ out) {
-    u64 a = i0 + 1, b = nf;
-    while (a < b) { u64 mid = (a + b + 1) >> 1; if (cum[mid] - cum[i0] <= budget) a = mid; else b = mid - 1; }
-    *out = a;
-}
-
 // raw neighbour entry q of the piece (global position q0 + q): its front entry and neighbour, kept when the entry is effective (an
-// m entry its own dm does not delete, or a dp entry) and the side has not seen the neighbour; key SP_NONE otherwise
+// m entry its own dm does not delete, or a dp entry) and the side has not seen the neighbour; key SLOT_NONE otherwise
 __global__ void k_sp_emit(const u64 *__restrict__ front, const u64 *__restrict__ cum, u64 i0, u64 i1, u64 q0, u64 R,
                           const SpOp *__restrict__ ops, u32 nops, const u64 *__restrict__ vis, u64 nw, u64 *__restrict__ key,
                           u64 *__restrict__ val, u64 *__restrict__ nkept) {
     u64 kept = 0;
     for (u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x; q < R; q += (u64)gridDim.x * blockDim.x) {
         const u64 g = q0 + q;
-        u64 a = i0, b = i1 - 1;                              // the last front entry with cum <= g
-        while (a < b) { u64 mid = (a + b + 1) >> 1; if (cum[mid] <= g) a = mid; else b = mid - 1; }
+        const u64 a = i0 + list_at(cum + i0, i1 - i0, g);     // the last front entry with cum <= g
         const u64 s = front[a] >> 32, u = (u32)front[a];
         u64 o = g - cum[a];
         u32 v = 0;
@@ -100,21 +86,16 @@ __global__ void k_sp_emit(const u64 *__restrict__ front, const u64 *__restrict__
             if (o < ld) { v = op.dp.j[op.dp.p[u] + o]; live = true; break; }
             o -= ld;
         }
-        live = live && !sp_seen(vis, nw, s, v);
-        key[q] = live ? (s << 32 | v) : SP_NONE;
+        live = live && !slot_seen(vis, nw, s, v);
+        key[q] = live ? (s << 32 | v) : SLOT_NONE;
         val[q] = a;
         kept += live;
     }
     if (kept) atomicAdd((unsigned long long *)nkept, (unsigned long long)kept);
 }
 
-__global__ void k_sp_heads(const u64 *__restrict__ key, u64 E, u32 *__restrict__ head) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e <= E; e += (u64)gridDim.x * blockDim.x)
-        head[e] = e < E && (e == 0 || key[e] != key[e - 1]) ? 1 : 0;
-}
-
 // per distinct (slot, v) h: recorded in the side's new chunk with its parent, marked seen, and either a meet candidate (code = od,
-// the piece's least od per slot in pod) or a survivor (code = SP_NONE, surv = 1)
+// the piece's least od per slot in pod) or a survivor (code = SLOT_NONE, surv = 1)
 __global__ void k_sp_classify(const u64 *__restrict__ key, const u64 *__restrict__ val, u64 E, const u32 *__restrict__ head,
                               const u64 *__restrict__ hpos, const u64 *__restrict__ front, u64 *__restrict__ vis_own,
                               const u64 *__restrict__ vis_oth, u64 nw, const SpChunk *__restrict__ och, u32 noch,
@@ -128,8 +109,8 @@ __global__ void k_sp_classify(const u64 *__restrict__ key, const u64 *__restrict
         lkey[h] = k;
         lval[h] = (u64)(u32)front[val[e]] << 32 | (u32)(sdepth[s] + 1);
         atomicOr((unsigned long long *)&vis_own[s * nw + (v >> 6)], 1ULL << (v & 63));
-        u64 pos, od = SP_NONE;
-        if (sp_seen(vis_oth, nw, s, v) && sp_find(och, noch, olkey, k, &pos)) {
+        u64 pos, od = SLOT_NONE;
+        if (slot_seen(vis_oth, nw, s, v) && sp_find(och, noch, olkey, k, &pos)) {
             od = (u32)olval[pos];
             atomicMin((unsigned long long *)&pod[s], (unsigned long long)od);
             surv[h] = 0;
@@ -147,7 +128,7 @@ __global__ void k_sp_tie(const u64 *__restrict__ lkey, const u64 *__restrict__ k
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < E; e += (u64)gridDim.x * blockDim.x) {
         if (!head[e]) continue;
         const u64 h = hpos[e], s = key[e] >> 32;
-        if (code[h] != SP_NONE && code[h] == pod[s]) atomicMin((unsigned long long *)&prv[s], (unsigned long long)(val[e] << 32 | (u32)lkey[h]));
+        if (code[h] != SLOT_NONE && code[h] == pod[s]) atomicMin((unsigned long long *)&prv[s], (unsigned long long)(val[e] << 32 | (u32)lkey[h]));
     }
 }
 
@@ -155,7 +136,7 @@ __global__ void k_sp_tie(const u64 *__restrict__ lkey, const u64 *__restrict__ k
 __global__ void k_sp_merge(u64 S, u64 *__restrict__ pod, u64 *__restrict__ prv, u64 *__restrict__ bod, u64 *__restrict__ brv) {
     for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s < S; s += (u64)gridDim.x * blockDim.x) {
         if (pod[s] < bod[s]) { bod[s] = pod[s]; brv[s] = prv[s]; }
-        pod[s] = SP_NONE; prv[s] = SP_NONE;
+        pod[s] = SLOT_NONE; prv[s] = SLOT_NONE;
     }
 }
 
@@ -181,11 +162,6 @@ __global__ void k_sp_keep_flag(const u64 *__restrict__ front, u64 nf, u32 sd, co
         flag[i] = f;
     }
 }
-__global__ void k_sp_keep(const u64 *__restrict__ front, u64 nf, const u32 *__restrict__ flag, const u64 *__restrict__ pos,
-                          u64 *__restrict__ out) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < nf; i += (u64)gridDim.x * blockDim.x)
-        if (flag[i]) out[pos[i]] = front[i];
-}
 
 // the end of a round: the expanded side one level deeper; a slot with a meet is found
 __global__ void k_sp_end(u64 S, u32 *__restrict__ state, const u32 *__restrict__ side, u64 *__restrict__ depth,
@@ -193,14 +169,14 @@ __global__ void k_sp_end(u64 S, u32 *__restrict__ state, const u32 *__restrict__
     for (u64 s = (u64)blockIdx.x * blockDim.x + threadIdx.x; s < S; s += (u64)gridDim.x * blockDim.x) {
         if (state[s] != SP_ACTIVE) continue;
         depth[side[s] * S + s]++;
-        if (brv[s] != SP_NONE) state[s] = SP_FOUND;
+        if (brv[s] != SLOT_NONE) state[s] = SP_FOUND;
     }
 }
 
 // per slot its front entries; one atomic per run of equal slots in a warp (a front is mostly grouped by slot)
 __global__ void k_sp_count(const u64 *__restrict__ front, u64 nf, u64 *__restrict__ cnt) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    const u64 s = i < nf ? front[i] >> 32 : SP_NONE;
+    const u64 s = i < nf ? front[i] >> 32 : SLOT_NONE;
     const unsigned peers = __match_any_sync(0xffffffffu, s);
     if (i < nf && (u32)(__ffs(peers) - 1) == (threadIdx.x & 31)) atomicAdd((unsigned long long *)&cnt[s], (unsigned long long)__popc(peers));
 }
@@ -261,16 +237,6 @@ __global__ void k_sp_seed(const u64 *__restrict__ ends, u64 S, u64 nw, u64 *__re
 
 // ---- host side ----
 
-template <class T>
-static void sp_grow(DevBuf<T> &b, u64 used, u64 need) {     // capacity for `need` entries, keeping the first `used`
-    if (b.n >= need) return;
-    DevBuf<T> nb(std::max<u64>(need, 2 * b.n));
-    d2d(nb.ptr, b.ptr, used);
-    b = std::move(nb);
-}
-
-static const u32 SP_T = 256;
-
 struct SpSideState {
     DevBuf<u64> vis, front, lkey, lval;
     u64 nf = 0, nl = 0;
@@ -291,7 +257,7 @@ struct SpSideState {
             SpChunk &a = chunks[chunks.size() - 2];
             const SpChunk b = chunks.back();
             if (a.n > 2 * b.n) break;
-            sort_pairs_u64(lkey.ptr + a.off, lval.ptr + a.off, a.n + b.n, SP_KEY_BITS);
+            sort_pairs_u64(lkey.ptr + a.off, lval.ptr + a.off, a.n + b.n, SLOT_KEY_BITS);
             a.n += b.n;
             chunks.pop_back();
         }
@@ -305,72 +271,57 @@ static u64 sp_expand(SpSideState &own, SpSideState &oth, u32 sd, u64 S, u64 nw, 
     // the front entries that carry over
     DevBuf<u32> kf(nf + 1);
     DevBuf<u64> kpos(nf + 1);
-    LAUNCH(k_sp_keep_flag, grid_for(nf + 1, SP_T), SP_T, 0, own.front.ptr, nf, sd, state.ptr, side.ptr, kf.ptr);
+    LAUNCH(k_sp_keep_flag, grid_for(nf + 1, PAIR_T), PAIR_T, 0, own.front.ptr, nf, sd, state.ptr, side.ptr, kf.ptr);
     exclusive_scan_u32_to_u64(kf.ptr, kpos.ptr, nf + 1);
     const u64 nkeep = read_scalar(kpos.ptr + nf);
     DevBuf<u64> next(std::max<u64>(nkeep, 1));
-    if (nkeep) LAUNCH(k_sp_keep, grid_for(nf, SP_T), SP_T, 0, own.front.ptr, nf, kf.ptr, kpos.ptr, next.ptr);
+    if (nkeep) scatter_flagged(own.front.ptr, nf, kf.ptr, kpos.ptr, next.ptr);
     u64 nnext = nkeep;
     kf.release(); kpos.release();
 
     DevBuf<u64> cum(nf + 1);
-    LAUNCH(k_sp_deg, grid_for(nf + 1, SP_T), SP_T, 0, own.front.ptr, nf, sd, state.ptr, side.ptr, own.ops.ptr, own.nops, cum.ptr);
+    LAUNCH(k_sp_deg, grid_for(nf + 1, PAIR_T), PAIR_T, 0, own.front.ptr, nf, sd, state.ptr, side.ptr, own.ops.ptr, own.nops, cum.ptr);
     exclusive_scan_u64(cum.ptr, cum.ptr, nf + 1);
     const u64 total = nf ? read_scalar(cum.ptr + nf) : 0;
-    DevBuf<u64> scal(2);
+    DevBuf<u64> scal(1);
     oth.upload();
-    for (u64 i0 = 0, q0 = 0; q0 < total;) {
-        u64 i1 = nf;
-        if (total - q0 > budget) {
-            LAUNCH(k_sp_cut, 1, 1, 0, cum.ptr, i0, nf, budget, scal.ptr);
-            i1 = read_scalar(scal.ptr);
-        }
-        const u64 q1 = i1 < nf ? read_scalar(cum.ptr + i1) : total;
+    for_each_piece(cum.ptr, nf, total, budget, [&](u64 i0, u64 i1, u64 q0, u64 q1) {
         const u64 R = q1 - q0;
-        if (R) {
-            DevBuf<u64> key(R), val(R);
-            CUDA_TRY(cudaMemsetAsync(scal.ptr, 0, sizeof(u64), stream()));
-            LAUNCH(k_sp_emit, grid_for(R, SP_T, 8 * (u64)ctx().num_sms), SP_T, 0, own.front.ptr, cum.ptr, i0, i1, q0, R, own.ops.ptr,
-                   own.nops, own.vis.ptr, nw, key.ptr, val.ptr, scal.ptr);
-            const u64 E = read_scalar(scal.ptr);
-            if (E) {
-                sort_pairs_u64(key.ptr, val.ptr, R, SP_KEY_BITS);            // stable: the least rank leads each (slot, v)
-                DevBuf<u32> head(E + 1);
-                DevBuf<u64> hpos(E + 1);
-                LAUNCH(k_sp_heads, grid_for(E + 1, SP_T), SP_T, 0, key.ptr, E, head.ptr);
-                exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, E + 1);
-                const u64 nh = read_scalar(hpos.ptr + E);
-                sp_grow(own.lkey, own.nl, own.nl + nh);
-                sp_grow(own.lval, own.nl, own.nl + nh);
-                DevBuf<u64> code(nh), spos(nh + 1);
-                DevBuf<u32> surv(nh + 1);
-                CUDA_TRY(cudaMemsetAsync(surv.ptr + nh, 0, sizeof(u32), stream()));
-                LAUNCH(k_sp_classify, grid_for(E, SP_T), SP_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, own.front.ptr, own.vis.ptr,
-                       oth.vis.ptr, nw, oth.dch.ptr, (u32)oth.chunks.size(), oth.lkey.ptr, oth.lval.ptr, depth.ptr + sd * S,
-                       own.lkey.ptr + own.nl, own.lval.ptr + own.nl, code.ptr, surv.ptr, pod.ptr);
-                own.chunks.push_back(SpChunk{own.nl, nh});
-                own.nl += nh;
-                LAUNCH(k_sp_tie, grid_for(E, SP_T), SP_T, 0, own.lkey.ptr + own.nl - nh, key.ptr, val.ptr, E, head.ptr, hpos.ptr, code.ptr,
-                       pod.ptr, prv.ptr);
-                LAUNCH(k_sp_merge, grid_for(S, SP_T), SP_T, 0, S, pod.ptr, prv.ptr, bod.ptr, brv.ptr);
-                own.merge_tail();                                       // after k_sp_tie, which reads the new chunk in place
-                exclusive_scan_u32_to_u64(surv.ptr, spos.ptr, nh + 1);
-                const u64 ns = read_scalar(spos.ptr + nh);
-                if (ns) {
-                    DevBuf<u64> rk(ns), nk(ns);
-                    LAUNCH(k_sp_survivors, grid_for(E, SP_T), SP_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, surv.ptr, spos.ptr, rk.ptr,
-                           nk.ptr);
-                    int bits = 1;
-                    while (bits < 64 && (nf >> bits)) bits++;
-                    sort_pairs_u64(rk.ptr, nk.ptr, ns, bits);               // stable: (rank, v)
-                    sp_grow(next, nnext, nnext + ns);
-                    d2d(next.ptr + nnext, nk.ptr, ns);
-                    nnext += ns;
-                }
-            }
-        }
-        i0 = i1; q0 = q1;
-    }
+        DevBuf<u64> key(R), val(R);
+        CUDA_TRY(cudaMemsetAsync(scal.ptr, 0, sizeof(u64), stream()));
+        LAUNCH(k_sp_emit, grid_for(R, PAIR_T, 8 * (u64)ctx().num_sms), PAIR_T, 0, own.front.ptr, cum.ptr, i0, i1, q0, R, own.ops.ptr,
+               own.nops, own.vis.ptr, nw, key.ptr, val.ptr, scal.ptr);
+        const u64 E = read_scalar(scal.ptr);
+        if (!E) return;
+        sort_pairs_u64(key.ptr, val.ptr, R, SLOT_KEY_BITS);            // stable: the least rank leads each (slot, v)
+        DevBuf<u32> head(E + 1);
+        DevBuf<u64> hpos(E + 1);
+        const u64 nh = run_heads(key.ptr, E, head.ptr, hpos.ptr);
+        grow(own.lkey, own.nl, own.nl + nh);
+        grow(own.lval, own.nl, own.nl + nh);
+        DevBuf<u64> code(nh), spos(nh + 1);
+        DevBuf<u32> surv(nh + 1);
+        CUDA_TRY(cudaMemsetAsync(surv.ptr + nh, 0, sizeof(u32), stream()));
+        LAUNCH(k_sp_classify, grid_for(E, PAIR_T), PAIR_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, own.front.ptr, own.vis.ptr,
+               oth.vis.ptr, nw, oth.dch.ptr, (u32)oth.chunks.size(), oth.lkey.ptr, oth.lval.ptr, depth.ptr + sd * S,
+               own.lkey.ptr + own.nl, own.lval.ptr + own.nl, code.ptr, surv.ptr, pod.ptr);
+        own.chunks.push_back(SpChunk{own.nl, nh});
+        own.nl += nh;
+        LAUNCH(k_sp_tie, grid_for(E, PAIR_T), PAIR_T, 0, own.lkey.ptr + own.nl - nh, key.ptr, val.ptr, E, head.ptr, hpos.ptr, code.ptr,
+               pod.ptr, prv.ptr);
+        LAUNCH(k_sp_merge, grid_for(S, PAIR_T), PAIR_T, 0, S, pod.ptr, prv.ptr, bod.ptr, brv.ptr);
+        own.merge_tail();                                       // after k_sp_tie, which reads the new chunk in place
+        exclusive_scan_u32_to_u64(surv.ptr, spos.ptr, nh + 1);
+        const u64 ns = read_scalar(spos.ptr + nh);
+        if (!ns) return;
+        DevBuf<u64> rk(ns), nk(ns);
+        LAUNCH(k_sp_survivors, grid_for(E, PAIR_T), PAIR_T, 0, key.ptr, val.ptr, E, head.ptr, hpos.ptr, surv.ptr, spos.ptr, rk.ptr,
+               nk.ptr);
+        sort_pairs_u64(rk.ptr, nk.ptr, ns, bit_length(nf));          // stable: (rank, v)
+        grow(next, nnext, nnext + ns);
+        d2d(next.ptr + nnext, nk.ptr, ns);
+        nnext += ns;
+    });
     own.front = std::move(next);
     own.nf = nnext;
     return total;
@@ -382,9 +333,7 @@ u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<
     const u64 nw = (n + 63) / 64;
     size_t fr = 0, tot = 0;
     CUDA_TRY(cudaMemGetInfo(&fr, &tot));
-    // a piece holds about 80 bytes per neighbour entry (keys, ranks, the sort's second buffers, run heads and their scans): by
-    // default a sixteenth of the free memory, and below the sort's 2^31 keys
-    if (!budget) budget = std::min<u64>((u64)1 << 30, std::max<u64>((u64)1 << 16, fr / 16 / 80));
+    budget = piece_budget(budget, fr);
     // the two visited bitmaps of a slice take at most a quarter of the free memory
     const u64 per_slot = 2 * nw * 8;
     const u64 S_max = std::max<u64>(1, std::min<u64>(1024, fr / 4 / per_slot));
@@ -409,7 +358,7 @@ u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<
             st.vis.alloc(S * nw);
             st.vis.zero();
             st.front.alloc(S); st.lkey.alloc(S); st.lval.alloc(S);
-            LAUNCH(k_sp_seed, grid_for(S, SP_T), SP_T, 0, ends.ptr, S, nw, st.front.ptr, st.lkey.ptr, st.lval.ptr, st.vis.ptr);
+            LAUNCH(k_sp_seed, grid_for(S, PAIR_T), PAIR_T, 0, ends.ptr, S, nw, st.front.ptr, st.lkey.ptr, st.lval.ptr, st.vis.ptr);
             st.nf = st.nl = S;
             st.chunks = {SpChunk{0, S}};
         }
@@ -423,22 +372,22 @@ u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<
         while (true) {
             cnt.zero();
             for (int sd = 0; sd < 2; sd++)
-                if (side_st[sd].nf) LAUNCH(k_sp_count, grid_for(side_st[sd].nf, SP_T), SP_T, 0, side_st[sd].front.ptr, side_st[sd].nf,
+                if (side_st[sd].nf) LAUNCH(k_sp_count, grid_for(side_st[sd].nf, PAIR_T), PAIR_T, 0, side_st[sd].front.ptr, side_st[sd].nf,
                                            cnt.ptr + sd * S);
             CUDA_TRY(cudaMemsetAsync(scal.ptr, 0, 8, stream()));
-            LAUNCH(k_sp_begin, grid_for(S, SP_T), SP_T, 0, S, state.ptr, cnt.ptr, depth.ptr, max_hops, side.ptr, scal.ptr);
+            LAUNCH(k_sp_begin, grid_for(S, PAIR_T), PAIR_T, 0, S, state.ptr, cnt.ptr, depth.ptr, max_hops, side.ptr, scal.ptr);
             if (!read_scalar(scal.ptr)) break;
             for (int sd = 0; sd < 2; sd++) {
                 SpSideState &own = side_st[sd];
                 if (own.nf >= ((u64)1 << 32)) throw GrbError(-8, "shortest_path: a front of 2^32 entries");   // ranks are 32 bits
                 flops += sp_expand(own, side_st[1 - sd], (u32)sd, S, nw, state, side, depth, pod, prv, bod, brv, budget);
             }
-            LAUNCH(k_sp_end, grid_for(S, SP_T), SP_T, 0, S, state.ptr, side.ptr, depth.ptr, brv.ptr);
+            LAUNCH(k_sp_end, grid_for(S, PAIR_T), PAIR_T, 0, S, state.ptr, side.ptr, depth.ptr, brv.ptr);
         }
         // paths
         for (int sd = 0; sd < 2; sd++) side_st[sd].upload();
         DevBuf<u64> dl(S + 1), off(S + 1);
-        LAUNCH(k_sp_len, grid_for(S, SP_T), SP_T, 0, S, state.ptr, brv.ptr, side_st[0].view(), side_st[1].view(), dl.ptr);
+        LAUNCH(k_sp_len, grid_for(S, PAIR_T), PAIR_T, 0, S, state.ptr, brv.ptr, side_st[0].view(), side_st[1].view(), dl.ptr);
         d2h(len.data() + p0, dl.ptr, S);
         sync_stream();
         std::vector<u64> hoff(S + 1, 0);
@@ -446,29 +395,15 @@ u64 shortest_path(const u64 *h_src, const u64 *h_dst, u64 np, const std::vector<
         if (hoff[S]) {
             h2d(off.ptr, hoff.data(), S + 1);
             DevBuf<u32> out(hoff[S]);
-            LAUNCH(k_sp_write, grid_for(S, SP_T), SP_T, 0, S, state.ptr, brv.ptr, side_st[0].view(), side_st[1].view(), off.ptr, out.ptr);
+            LAUNCH(k_sp_write, grid_for(S, PAIR_T), PAIR_T, 0, S, state.ptr, brv.ptr, side_st[0].view(), side_st[1].view(), off.ptr, out.ptr);
             const size_t base = nodes.size();                   // no allocation after this: a retried slice appends nothing
             nodes.resize(base + hoff[S]);
             d2h(nodes.data() + base, out.ptr, hoff[S]);
             sync_stream();
         }
     };
-    // The bitmaps size a slice up front; the fronts and level entries grow with what each pair visits.  A slice that runs out of
-    // device memory is run again as two halves (down to one pair), so a large batch on a large graph slices instead of failing.
-    u64 S_cur = S_max;
-    for (u64 p0 = 0; p0 < np;) {
-        const u64 S = std::min<u64>(S_cur, np - p0);
-        try {
-            run_slice(p0, S);
-        } catch (const CudaError &e) {
-            if (e.code != cudaErrorMemoryAllocation || S == 1) throw;
-            cudaGetLastError();
-            pool_trim();
-            S_cur = S / 2;
-            continue;
-        }
-        p0 += S;
-    }
+    // the bitmaps size a slice up front; the fronts and level entries grow with what each pair visits
+    for_each_slice(np, S_max, run_slice);
     return flops;
 }
 

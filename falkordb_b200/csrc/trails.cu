@@ -60,29 +60,6 @@ __global__ void k_tr_zero(TArgs T, u64 n, u32 *__restrict__ z) {
         z[i] = T.min_hops == 0 && can_end(T, i, T.lev[0].node[i]) ? 1 : 0;
 }
 
-// per level entry: its node's slot among the distinct nodes u (ascending) and its adjacency length; clen[n] = 0 is set by the caller
-__global__ void k_tr_len(const u32 *__restrict__ node, u64 n, const u64 *__restrict__ u, u64 nu, const u64 *__restrict__ adj_p,
-                         u32 *__restrict__ slot, u64 *__restrict__ clen) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x) {
-        const u64 x = node[e];
-        u64 a = 0, b = nu;
-        while (a < b) { u64 mid = (a + b) >> 1; if (u[mid] < x) a = mid + 1; else b = mid; }
-        slot[e] = (u32)a;
-        clen[e] = adj_p[a + 1] - adj_p[a];
-    }
-}
-
-// sorted keys -> run heads
-__global__ void k_tr_heads(const u64 *__restrict__ k, u64 n, u32 *__restrict__ head) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x)
-        head[e] = e == 0 || k[e] != k[e - 1] ? 1 : 0;
-}
-__global__ void k_tr_compact(const u64 *__restrict__ k, u64 n, const u32 *__restrict__ head, const u64 *__restrict__ hpos,
-                             u64 *__restrict__ u) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x)
-        if (head[e]) u[hpos[e]] = k[e];
-}
-
 // per candidate of level h (hop = h + 1): kept (stored, or on the last level emitted) and will_emit
 __global__ void k_tr_cand(TArgs T, u32 h, const u64 *__restrict__ cstart, u64 n, const u32 *__restrict__ slot,
                           const u64 *__restrict__ adj_p, const u32 *__restrict__ adj_node, const u64 *__restrict__ adj_edge, u64 C,
@@ -201,24 +178,17 @@ struct Level {                  // level h of the trail tree
     bool last_children = false; // cb indexes the last level's kept candidates
 };
 struct LastLevel {              // the expansion of level h into the emit-only hop max_hops (kept for the output passes)
-    u32 h = 0; u64 n = 0, C = 0;
-    DevBuf<u64> cstart, adj_p, adj_edge, kpos;
-    DevBuf<u32> slot, adj_node, kept;
+    u32 h = 0; u64 n = 0;
+    NodeAdj adj;
+    DevBuf<u64> kpos;
+    DevBuf<u32> kept;
 };
-u64 d2h_word(const u64 *p) { u64 v = 0; d2h(&v, p, 1); sync_stream(); return v; }
 }
 
 int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const std::vector<EdgeTypeDev> &types, int dir, u64 min_hops,
                    u64 max_hops, const std::vector<LabelDev> &labels, u64 nv, u64 tree_capacity, TrailsOut &o) {
-    const u32 grid = (u32)ctx().num_sms * 8, T = (u32)types.size();
-    std::vector<EType> ht(T);
-    for (u32 t = 0; t < T; t++) {
-        const EdgeTypeDev &x = types[t];
-        ht[t] = EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
-                      estore(x.me_dm)};
-    }
-    DevBuf<EType> dt(T);
-    h2d(dt.ptr, ht.data(), T);
+    const u32 grid = (u32)ctx().num_sms * 8;
+    const ETypes ty(types);
     std::vector<std::unique_ptr<Level>> lv;
     lv.emplace_back(new Level());
     Level &L0 = *lv[0];
@@ -267,52 +237,27 @@ int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const s
         Level &X = *lv[h];
         const u64 n = X.n;
         const bool to_last = (u64)h + 1 == max_hops;
-        // the level's distinct nodes
-        DevBuf<u64> keys(n), u;
-        widen_u32(X.node.ptr, keys.ptr, n);
-        sort_keys_u64(keys.ptr, n, 32);
-        u64 nu;
-        {
-            DevBuf<u32> head(n + 1);
-            DevBuf<u64> hpos(n + 1);
-            CUDA_TRY(cudaMemsetAsync(head.ptr + n, 0, sizeof(u32), stream()));
-            LAUNCH(k_tr_heads, grid_for(n, 256, grid), 256, 0, keys.ptr, n, head.ptr);
-            exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, n + 1);
-            nu = d2h_word(hpos.ptr + n);
-            u.alloc(nu);
-            LAUNCH(k_tr_compact, grid_for(n, 256, grid), 256, 0, keys.ptr, n, head.ptr, hpos.ptr, u.ptr);
-        }
-        keys.release();
-        DevBuf<u64> adj_p, adj_edge;
-        DevBuf<u32> adj_node;
-        edge_adjacency(dt.ptr, T, u.ptr, nu, dir, adj_p, adj_node, adj_edge, &bytes);
-        // candidates: one per (entry, adjacency position)
-        DevBuf<u32> slot(n);
-        DevBuf<u64> clen(n + 1), cstart(n + 1);
-        CUDA_TRY(cudaMemsetAsync(clen.ptr + n, 0, sizeof(u64), stream()));
-        LAUNCH(k_tr_len, grid_for(n, 256, grid), 256, 0, X.node.ptr, n, u.ptr, nu, adj_p.ptr, slot.ptr, clen.ptr);
-        exclusive_scan_u64(clen.ptr, cstart.ptr, n + 1);
-        clen.release();
-        const u64 C = d2h_word(cstart.ptr + n);
+        // candidates: one per (entry, adjacency position of its node)
+        NodeAdj adj;
+        adj.fetch(ty, X.node.ptr, n, dir, false, &bytes);
+        const u64 C = adj.total;
         DevBuf<u32> kept(C + 1), emit;
         DevBuf<u64> kpos(C + 1);
         if (!to_last) emit.alloc(C);
         CUDA_TRY(cudaMemsetAsync(kept.ptr + C, 0, sizeof(u32), stream()));
-        if (C) LAUNCH(k_tr_cand, grid_for(C, 256, grid), 256, 0, A, h, cstart.ptr, n, slot.ptr, adj_p.ptr, adj_node.ptr, adj_edge.ptr, C,
-                      kept.ptr, emit.ptr);
+        if (C) LAUNCH(k_tr_cand, grid_for(C, 256, grid), 256, 0, A, h, adj.cum.ptr, n, adj.row.ptr, adj.p.ptr, adj.node.ptr,
+                      adj.edge.ptr, C, kept.ptr, emit.ptr);
         exclusive_scan_u32_to_u64(kept.ptr, kpos.ptr, C + 1);
         X.cb.alloc(n + 1);
-        LAUNCH(k_tr_cb, grid_for(n + 1, 256, grid), 256, 0, cstart.ptr, kpos.ptr, n, X.cb.ptr);
-        const u64 K = d2h_word(kpos.ptr + C);
+        LAUNCH(k_tr_cb, grid_for(n + 1, 256, grid), 256, 0, adj.cum.ptr, kpos.ptr, n, X.cb.ptr);
+        const u64 K = read_scalar(kpos.ptr + C);
         bytes += 16 * n + C * (24 + 16 * (u64)h);
         if (to_last) {
             X.last_children = true;
             npath += K * max_hops;
             if (o.out_end) {                        // the output passes re-read this level's candidates
-                last.h = h; last.n = n; last.C = C;
-                last.cstart = std::move(cstart); last.adj_p = std::move(adj_p); last.adj_edge = std::move(adj_edge);
-                last.kpos = std::move(kpos); last.slot = std::move(slot); last.adj_node = std::move(adj_node);
-                last.kept = std::move(kept);
+                last.h = h; last.n = n;
+                last.adj = std::move(adj); last.kpos = std::move(kpos); last.kept = std::move(kept);
                 has_last = true;
             }
             break;
@@ -324,10 +269,10 @@ int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const s
         Y.n = K;
         Y.par.alloc(K); Y.node.alloc(K); Y.edge.alloc(K); Y.emit.alloc(K + 1); Y.emp.alloc(K + 1);
         CUDA_TRY(cudaMemsetAsync(Y.emit.ptr + K, 0, sizeof(u32), stream()));
-        if (K) LAUNCH(k_tr_fill, grid_for(C, 256, grid), 256, 0, cstart.ptr, n, slot.ptr, adj_p.ptr, adj_node.ptr, adj_edge.ptr, C,
-                      kept.ptr, emit.ptr, kpos.ptr, Y.par.ptr, Y.node.ptr, Y.edge.ptr, Y.emit.ptr);
+        if (K) LAUNCH(k_tr_fill, grid_for(C, 256, grid), 256, 0, adj.cum.ptr, n, adj.row.ptr, adj.p.ptr, adj.node.ptr, adj.edge.ptr,
+                      C, kept.ptr, emit.ptr, kpos.ptr, Y.par.ptr, Y.node.ptr, Y.edge.ptr, Y.emit.ptr);
         exclusive_scan_u32_to_u64(Y.emit.ptr, Y.emp.ptr, K + 1);
-        npath += d2h_word(Y.emp.ptr + K) * (h + 1);
+        npath += read_scalar(Y.emp.ptr + K) * (h + 1);
         bytes += 28 * K;
         upload_levels();
         A.lev = dlev.ptr;
@@ -380,10 +325,11 @@ int var_len_trails(const u64 *h_starts, const i64 *h_dests, u64 nstarts, const s
                 LAUNCH(k_tr_out, grid_for(Y.n, 256, grid), 256, 0, A, (u32)h, Y.n, Y.emit.ptr, Y.emp.ptr, lv[h - 1]->cb.ptr,
                        lv[h - 1]->P.ptr, dend.ptr, dhops.ptr, e, dpedge.ptr, dpnode.ptr);
         }
-        if (has_last && last.C)
-            LAUNCH(k_tr_out_last, grid_for(last.C, 256, grid), 256, 0, A, last.h, last.cstart.ptr, last.n, last.slot.ptr,
-                   last.adj_p.ptr, last.adj_node.ptr, last.adj_edge.ptr, last.C, last.kept.ptr, last.kpos.ptr, lv[last.h]->cb.ptr,
-                   lv[last.h]->P.ptr, dend.ptr, dhops.ptr, e, dpedge.ptr, dpnode.ptr);
+        const NodeAdj &LA = last.adj;
+        if (has_last && LA.total)
+            LAUNCH(k_tr_out_last, grid_for(LA.total, 256, grid), 256, 0, A, last.h, LA.cum.ptr, last.n, LA.row.ptr, LA.p.ptr,
+                   LA.node.ptr, LA.edge.ptr, LA.total, last.kept.ptr, last.kpos.ptr, lv[last.h]->cb.ptr, lv[last.h]->P.ptr, dend.ptr,
+                   dhops.ptr, e, dpedge.ptr, dpnode.ptr);
     }
     d2h(o.out_end, dend.ptr, N);
     if (o.out_hops) d2h(o.out_hops, dhops.ptr, N);

@@ -18,24 +18,6 @@ namespace b200 {
 
 static const u32 NO_ROW = ~0u;
 
-// distinct starts: sorted keys -> run heads
-__global__ void k_vb_heads(const u64 *__restrict__ k, u64 n, u32 *__restrict__ head) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x)
-        head[e] = e == 0 || k[e] != k[e - 1] ? 1 : 0;
-}
-__global__ void k_vb_compact(const u64 *__restrict__ k, u64 n, const u32 *__restrict__ head, const u64 *__restrict__ hpos,
-                             u64 *__restrict__ u) {
-    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (u64)gridDim.x * blockDim.x)
-        if (head[e]) u[hpos[e]] = k[e];
-}
-// per start: its slot among the distinct starts u (ascending)
-__global__ void k_vb_slot(const u64 *__restrict__ s, u64 n, const u64 *__restrict__ u, u64 nu, u32 *__restrict__ slot) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
-        u64 a = 0, b = nu;
-        while (a < b) { u64 mid = (a + b) >> 1; if (u[mid] < s[i]) a = mid + 1; else b = mid; }
-        slot[i] = (u32)a;
-    }
-}
 // per adjacency entry: (slot << 32) | neighbour
 __global__ void k_vb_keys(const u64 *__restrict__ adj_p, u64 nu, const u32 *__restrict__ node, u64 E, u64 *__restrict__ key) {
     for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < E; e += (u64)gridDim.x * blockDim.x)
@@ -180,18 +162,9 @@ __global__ void k_vb_fix_copy(const u64 *__restrict__ s, u64 n, const u32 *__res
     }
 }
 
-static u32 key_bits(u64 v) { u32 b = 0; while (b < 64 && (v >> b)) b++; return b; }
-
 void vlb_plan(const u64 *h_starts, u64 nstarts, const std::vector<EdgeTypeDev> &types, u64 max_hops, VlbPlan &P) {
-    const u32 grid = (u32)ctx().num_sms * 8, T = (u32)types.size();
-    std::vector<EType> ht(T);
-    for (u32 t = 0; t < T; t++) {
-        const EdgeTypeDev &x = types[t];
-        ht[t] = EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
-                      estore(x.me_dm)};
-    }
-    DevBuf<EType> dt(T);
-    h2d(dt.ptr, ht.data(), T);
+    const u32 grid = (u32)ctx().num_sms * 8;
+    const ETypes ty(types);
     // Compulsory bytes ("var_len_reach_both"), this pass: 24 per start (its id, twice for the sort, and its slot), the adjacency
     // fetch (edge_expand's formula), 28 per adjacency entry (the key written, read by the sort and the run pass, its head flag and
     // scan), 8 per distinct neighbour (vertex and slot), 40 per distinct start (flags, bases, decision)
@@ -200,24 +173,14 @@ void vlb_plan(const u64 *h_starts, u64 nstarts, const std::vector<EdgeTypeDev> &
     P.n = nstarts;
     P.ds.alloc(nstarts);
     h2d(P.ds.ptr, h_starts, nstarts);
-    {
-        DevBuf<u64> keys(nstarts), hpos(nstarts + 1);
-        DevBuf<u32> head(nstarts + 1);
-        d2d(keys.ptr, P.ds.ptr, nstarts);
-        sort_keys_u64(keys.ptr, nstarts, 32);
-        CUDA_TRY(cudaMemsetAsync(head.ptr + nstarts, 0, sizeof(u32), stream()));
-        LAUNCH(k_vb_heads, grid_for(nstarts, 256, grid), 256, 0, keys.ptr, nstarts, head.ptr);
-        exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, nstarts + 1);
-        P.nu = read_scalar(hpos.ptr + nstarts);
-        P.u.alloc(P.nu);
-        LAUNCH(k_vb_compact, grid_for(nstarts, 256, grid), 256, 0, keys.ptr, nstarts, head.ptr, hpos.ptr, P.u.ptr);
-    }
-    const u64 nu = P.nu;
+    P.u.alloc(nstarts);
+    d2d(P.u.ptr, P.ds.ptr, nstarts);
+    const u64 nu = P.nu = unique_sorted(P.u, nstarts, 32);
     P.slot.alloc(nstarts);
-    LAUNCH(k_vb_slot, grid_for(nstarts, 256, grid), 256, 0, P.ds.ptr, nstarts, P.u.ptr, nu, P.slot.ptr);
+    node_rows(P.ds.ptr, nstarts, P.u.ptr, nu, nullptr, P.slot.ptr, nullptr);
     DevBuf<u64> adj_p, adj_edge;
     DevBuf<u32> adj_node;
-    const u64 E = edge_adjacency(dt.ptr, T, P.u.ptr, nu, 2, adj_p, adj_node, adj_edge, &bytes);
+    const u64 E = edge_adjacency(ty, P.u.ptr, nu, 2, adj_p, adj_node, adj_edge, &bytes);
     adj_edge.release();
     DevBuf<u64> key(E), npos(E + 1);
     DevBuf<u32> flag(nu), nh(E + 1);
@@ -226,7 +189,7 @@ void vlb_plan(const u64 *h_starts, u64 nstarts, const std::vector<EdgeTypeDev> &
     if (E) {
         LAUNCH(k_vb_keys, grid_for(E, 256, grid), 256, 0, adj_p.ptr, nu, adj_node.ptr, E, key.ptr);
         adj_node.release();
-        sort_keys_u64(key.ptr, E, 32 + key_bits(nu));
+        sort_keys_u64(key.ptr, E, 32 + bit_length(nu));
         LAUNCH(k_vb_runs, grid_for(E, 256, grid), 256, 0, key.ptr, E, P.u.ptr, flag.ptr, nh.ptr);
     }
     exclusive_scan_u32_to_u64(nh.ptr, npos.ptr, E + 1);

@@ -25,11 +25,6 @@ __global__ void k_wp_keys(const u64 *__restrict__ src, const u64 *__restrict__ d
         val[k] = id ? id[k] : k;
     }
 }
-// head[k] = 1 where a run of equal keys starts
-__global__ void k_wp_heads(const u64 *__restrict__ key, u64 n, u32 *__restrict__ head) {
-    for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (u64)gridDim.x * blockDim.x)
-        head[k] = k == 0 || key[k] != key[k - 1];
-}
 // rstart[r] = the first position of run r; rstart[R] = n
 __global__ void k_wp_starts(const u32 *__restrict__ head, const u64 *__restrict__ hpos, u64 n, u64 *__restrict__ rstart) {
     for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k <= n; k += (u64)gridDim.x * blockDim.x)
@@ -38,9 +33,8 @@ __global__ void k_wp_starts(const u32 *__restrict__ head, const u64 *__restrict_
 
 // is v among ids[lo, hi) (ascending)
 __device__ __forceinline__ bool ids_has(const u64 *__restrict__ ids, u64 lo, u64 hi, u64 v) {
-    const u64 e = hi;
-    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (ids[mid] < v) lo = mid + 1; else hi = mid; }
-    return lo < e && ids[lo] == v;
+    const u64 q = lb64(ids, lo, hi, v);
+    return q < hi && ids[q] == v;
 }
 
 // ---- insert plan ----
@@ -160,10 +154,6 @@ __global__ void k_rm_fill(EType t, const u64 *__restrict__ key, const u64 *__res
     }
 }
 
-static EType etype(const EdgeTypeDev &x) {
-    return EType{ecsr(x.m), ecsr(x.dp), ecsr(x.dm), ecsr(x.mt), ecsr(x.mt_dp), ecsr(x.mt_dm), estore(x.me), estore(x.me_dp),
-                 estore(x.me_dm)};
-}
 // sort bits of the keys: src < nv <= 2^32
 static int key_bits(u64 nv) { int b = 0; while (b < 32 && ((u64)1 << b) < nv) b++; return 32 + b; }
 
@@ -171,14 +161,9 @@ static int key_bits(u64 nv) { int b = 0; while (b < 32 && ((u64)1 << b) < nv) b+
 static u64 mark_runs(const u64 *key, u64 n, u32 grid, DevBuf<u64> &rstart) {
     DevBuf<u32> head(n + 1);
     DevBuf<u64> hpos(n + 1);
-    CUDA_TRY(cudaMemsetAsync(head.ptr + n, 0, sizeof(u32), stream()));
-    LAUNCH(k_wp_heads, grid_for(n, 256, grid), 256, 0, key, n, head.ptr);
-    exclusive_scan_u32_to_u64(head.ptr, hpos.ptr, n + 1);
+    const u64 R = run_heads(key, n, head.ptr, hpos.ptr);
     rstart.alloc(n + 1);
     LAUNCH(k_wp_starts, grid_for(n + 1, 256, grid), 256, 0, head.ptr, hpos.ptr, n, rstart.ptr);
-    u64 R = 0;
-    d2h(&R, hpos.ptr + n, 1);
-    sync_stream();
     return R;
 }
 

@@ -42,7 +42,7 @@ WANT = [
     ("insert plan, fill", r"k_ins_fill"),
     ("remove plan, count", r"k_rm_count"),
     ("remove plan, fill", r"k_rm_fill"),
-    ("write plans, run heads", r"k_wp_heads"),
+    ("sorted keys, run heads", r"k_run_heads"),
     ("relationship ids, reference order fill", r"k_ee_ref_fill"),
     ("trails, candidates", r"k_tr_cand"),
     ("trails, stored level fill", r"k_tr_fill"),
