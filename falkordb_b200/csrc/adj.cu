@@ -25,15 +25,6 @@ struct RankTable {                // keep[r] = the r-th kept vertex, tab[v] = v'
     __device__ __forceinline__ u32 rank(u32 c) const { return tab[c]; }
 };
 
-// smallest q in [lo, hi) with j[q] >= c
-__device__ __forceinline__ u64 adj_lower_bound(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
-    while (lo < hi) {
-        u64 mid = (lo + hi) >> 1;
-        if (j[mid] < c) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
 // One warp walks row v of L in 32-entry strides; lane keeps its own cursor into v's dm row.  FILL: write the surviving entries'
 // ranks from Cp[r] on (ballot prefix keeps them in order), else store the row's count.  in_rows (timing only): the L and dm
 // entries of the kept rows.
@@ -63,7 +54,7 @@ k_adj_layer(const u64 *__restrict__ Lp, const u32 *__restrict__ Lj, const u64 *_
                 const u32 col = Lj[q];
                 out = rk.rank(col);
                 if (out != ADJ_DROP && dq < de) {
-                    dq = adj_lower_bound(Dj, dq, de, col);
+                    dq = lb32(Dj, dq, de, col);
                     if (dq < de && Dj[dq] == col) out = ADJ_DROP;
                 }
             }
@@ -83,10 +74,6 @@ k_adj_layer(const u64 *__restrict__ Lp, const u32 *__restrict__ Lj, const u64 *_
     }
 }
 
-__global__ void k_adj_rank_drop(u64 n, u32 *__restrict__ tab) {
-    const u64 stride = (u64)gridDim.x * blockDim.x;
-    for (u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) tab[t] = ADJ_DROP;
-}
 __global__ void k_adj_rank_scatter(const u64 *__restrict__ keep, u64 nkeep, u32 *__restrict__ tab) {
     const u64 stride = (u64)gridDim.x * blockDim.x;
     for (u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x; t < nkeep; t += stride) tab[keep[t]] = (u32)t;
@@ -94,31 +81,25 @@ __global__ void k_adj_rank_scatter(const u64 *__restrict__ keep, u64 nkeep, u32 
 
 void adj_rank_table(const u64 *d_keep, u64 nkeep, u64 n, DevBuf<u32> &tab) {
     tab.alloc(n ? n : 1);
-    if (n) LAUNCH(k_adj_rank_drop, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, n, tab.ptr);
+    fill_u32(tab.ptr, ADJ_DROP, n);
     if (nkeep) LAUNCH(k_adj_rank_scatter, grid_for(nkeep, 256, (u64)ctx().num_sms * 16), 256, 0, d_keep, nkeep, tab.ptr);
 }
 
 template <class Rank>
 static void adj_layer_run(const DevCSR &L, const DevCSR *dm, u64 rows, Rank rk, bool gather, DevCSR &out) {
-    out.clear();
-    out.nrows = out.ncols = rows;
-    out.p.alloc(rows + 1);
-    if (rows == 0 || L.nnz == 0) { out.p.zero(); out.nnz = 0; return; }
+    csr_shape(out, rows, rows);
+    if (rows == 0 || L.nnz == 0) { out.p.zero(); return; }
     const u64 *Dp = dm && dm->nnz ? dm->p.ptr : nullptr;
     const u32 *Dj = Dp ? dm->j.ptr : nullptr;
     const bool timing = ctx().opt_timing != 0;
     DevBuf<unsigned long long> seen;
     if (timing) { seen.alloc(2); seen.zero(); }
     DevBuf<u32> cnt(rows + 1);
-    CUDA_TRY(cudaMemsetAsync(cnt.ptr + rows, 0, sizeof(u32), stream()));
     const u32 grid = grid_for(rows * 32, 256, (u64)ctx().num_sms * 32);
     timed_begin(TK_ADJ_BUILD);
     LAUNCH((k_adj_layer<Rank, false>), grid, 256, 0, L.p.ptr, L.j.ptr, Dp, Dj, L.nrows, rows, rk, cnt.ptr, (const u64 *)nullptr,
            (u32 *)nullptr, timing ? seen.ptr : nullptr);
-    exclusive_scan_u32_to_u64(cnt.ptr, out.p.ptr, rows + 1);
-    const u64 nnz = read_scalar(out.p.ptr + rows);
-    out.nnz = nnz;
-    out.j.alloc(nnz);
+    const u64 nnz = csr_rows_from_counts(cnt.ptr, rows, out, false);
     if (nnz)
         LAUNCH((k_adj_layer<Rank, true>), grid, 256, 0, L.p.ptr, L.j.ptr, Dp, Dj, L.nrows, rows, rk, (u32 *)nullptr, out.p.ptr, out.j.ptr,
                (unsigned long long *)nullptr);

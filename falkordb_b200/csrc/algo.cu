@@ -129,11 +129,6 @@ int pagerank(const DevCSR &A, const DevCSR &AT, double damping, double tol, int 
 // of the component, which is what this gives (deterministic).  A must have a symmetric pattern (the reference builds
 // build_symmetric_adjacency_matrix and sets is_symmetric_structure).  Rounds of: hook every edge's larger root under the smaller
 // (atomicMin), then full pointer jumping; O(log n) rounds, each one streaming pass over the CSR (4 B per entry + 8 B gathers).
-__global__ void k_cc_init(u64 *__restrict__ parent, u64 n) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) parent[i] = i;
-}
 __global__ void __launch_bounds__(256)
 k_cc_hook(const u64 *__restrict__ p, const u32 *__restrict__ j, u64 n, u64 *__restrict__ parent, u32 *__restrict__ changed) {
     const u32 lane8 = threadIdx.x & 7;
@@ -167,7 +162,7 @@ int connected_components(const DevCSR &A, u64 *d_comp) {
     const u64 n = A.nrows;
     if (!n) return 0;
     const u32 g = grid_for(n, 256, (u64)ctx().num_sms * 16);
-    LAUNCH(k_cc_init, g, 256, 0, d_comp, n);
+    iota_u64(d_comp, n);
     DevBuf<u32> changed(1);
     int rounds = 0;
     while (true) {
@@ -227,7 +222,7 @@ int cdlp(const DevCSR &A, int itermax, u64 *d_label) {
     if (!n) return 0;
     if (n > (1ull << 32)) throw GrbError(-8, "cdlp: more than 2^32 vertices not supported");
     const u32 g = grid_for(n, 256, (u64)ctx().num_sms * 16);
-    LAUNCH(k_cc_init, g, 256, 0, d_label, n);                 // L0(v) = v
+    iota_u64(d_label, n);                                     // L0(v) = v
     if (!A.nnz) return 0;
     int bits_n = 1;
     while ((1ull << bits_n) < n) ++bits_n;

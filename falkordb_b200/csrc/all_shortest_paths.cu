@@ -34,9 +34,6 @@ __global__ void k_as_seed(const u64 *__restrict__ src, u64 S, u64 nw, u64 *__res
         vis[s * nw + (v >> 6)] |= 1ULL << (v & 63);
     }
 }
-__global__ void k_as_iota(u64 *__restrict__ x, u64 n) {
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) x[i] = i;
-}
 // candidate q of the piece (global position g = q0 + q, in (rank, adjacency position) order): kept with key (slot << 32 | v) when
 // the slot has not seen v, else SLOT_NONE; an entry into the slot's dst marks the slot found
 __global__ void k_as_emit(const u64 *__restrict__ front, const u64 *__restrict__ cum, u64 i0, u64 i1, u64 q0, u64 R,
@@ -233,7 +230,7 @@ u64 all_shortest_paths(const u64 *h_src, const u64 *h_dst, u64 np, const std::ve
             F.n = nf;
             F.key.alloc(nf); F.rank.alloc(nf);
             d2d(F.key.ptr, front.ptr, nf);
-            LAUNCH(k_as_iota, grid_for(nf, PAIR_T), PAIR_T, 0, F.rank.ptr, nf);
+            iota_u64(F.rank.ptr, nf);
             sort_pairs_u64(F.key.ptr, F.rank.ptr, nf, SLOT_KEY_BITS);
             bytes += 16 * nf;
             NodeAdj A;

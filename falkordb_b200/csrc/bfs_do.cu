@@ -104,13 +104,6 @@ void comm_allgather(BfsComm *c, const void *send, void *recv, size_t bytes_per_r
 }
 
 // ---------------------------------------------------------------------------------------------- kernels
-__device__ __forceinline__ u64 do_find_le(const u64 *__restrict__ a, u64 lo, u64 hi, u64 target) {
-    while (lo < hi) {
-        u64 mid = (lo + hi + 1) >> 1;
-        if (a[mid] <= target) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
 __device__ __forceinline__ bool bit_of(const u64 *__restrict__ b, u64 v) { return (b[v >> 6] >> (v & 63)) & 1ULL; }
 
 // one operand of the dirty BFS on the device: the base m and its transpose mirror, dp and dm and their transposes (p null: empty)
@@ -141,7 +134,7 @@ __device__ __forceinline__ i64 do_first_parent(const BfsOpDev *__restrict__ ops,
                 if (q < e) {
                     u = Tj[q];
                     hit = u < best && bit_of(frontier, u);
-                    if (hit && d < de) {
+                    if (hit && d < de) {       // lb32 here reorders the code of k_do_pull<true> / k_do_assign<true>
                         u64 lo = d, hi = de;
                         while (lo < hi) { const u64 mid = (lo + hi) >> 1; if (Dj[mid] < u) lo = mid + 1; else hi = mid; }
                         d = lo;
@@ -233,40 +226,30 @@ __global__ void __launch_bounds__(256)
 k_do_expand(const u64 *__restrict__ cum, const u64 *__restrict__ start, u64 nf, u64 total, const u32 *__restrict__ Aj,
             const u64 *__restrict__ visited, u32 *__restrict__ disc, const u32 *__restrict__ fr, const BfsOpDev *__restrict__ ops,
             u32 nops2) {
-    __shared__ u64 s_e0, s_e1;
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (u64 chunk = blockIdx.x; chunk * DO_CHUNK < total; chunk += gridDim.x) {
         u64 lo = chunk * DO_CHUNK, hi = lo + DO_CHUNK;
         if (hi > total) hi = total;
         __syncthreads();
-        if (tid == 0) { s_e0 = do_find_le(cum, 0, nf - 1, lo); s_e1 = do_find_le(cum, 0, nf - 1, hi - 1); }
-        __syncthreads();
-        const u64 e0 = s_e0, e1 = s_e1;
-        for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
-            u64 e = do_find_le(cum, e0, e1, t0);
-            const u64 t = t0 + lane;
-            if (t < hi) {
-                while (e < e1 && cum[e + 1] <= t) e++;
-                if constexpr (DIRTY) {
-                    const u32 r = (u32)(e % nops2);
-                    const BfsOpDev &o = ops[r >> 1];
-                    const u32 v = ((r & 1) ? o.dpj : o.mj)[start[e] + (t - cum[e])];
-                    if (bit_of(visited, v)) continue;
-                    if (!(r & 1) && o.dmp) {
-                        const u64 u = fr[e / nops2];
-                        u64 lo = o.dmp[u], hi = o.dmp[u + 1];
-                        if (lo < hi) {
-                            while (lo < hi) { const u64 mid = (lo + hi) >> 1; if (o.dmj[mid] < v) lo = mid + 1; else hi = mid; }
-                            if (lo < o.dmp[u + 1] && o.dmj[lo] == v) continue;   // a deleted edge
-                        }
+        for_each_flop(cum, 0, nf, lo, hi, [&](u64 e, u64 t) {
+            if constexpr (DIRTY) {
+                const u32 r = (u32)(e % nops2);
+                const BfsOpDev &o = ops[r >> 1];
+                const u32 v = ((r & 1) ? o.dpj : o.mj)[start[e] + (t - cum[e])];
+                if (bit_of(visited, v)) return;
+                if (!(r & 1) && o.dmp) {
+                    const u64 u = fr[e / nops2];
+                    const u64 s = o.dmp[u], de = o.dmp[u + 1];
+                    if (s < de) {
+                        const u64 d = lb32(o.dmj, s, de, v);
+                        if (d < de && o.dmj[d] == v) return;   // a deleted edge
                     }
-                    atomicOr(&disc[v >> 5], 1u << (v & 31));
-                } else {
-                    const u32 v = Aj[start[e] + (t - cum[e])];
-                    if (!bit_of(visited, v)) atomicOr(&disc[v >> 5], 1u << (v & 31));
                 }
+                atomicOr(&disc[v >> 5], 1u << (v & 31));
+            } else {
+                const u32 v = Aj[start[e] + (t - cum[e])];
+                if (!bit_of(visited, v)) atomicOr(&disc[v >> 5], 1u << (v & 31));
             }
-        }
+        });
     }
 }
 // new = (OR of the P gathered bitmaps) & ~visited
@@ -400,35 +383,22 @@ __global__ void __launch_bounds__(256)
 k_bfs_expand(const u32 *__restrict__ fr, const u64 *__restrict__ cum, const u64 *__restrict__ start, u64 nf, u64 total,
              const u32 *__restrict__ Aj, i64 *__restrict__ level, i64 *__restrict__ parent, u64 *__restrict__ cand,
              i64 next_level, u32 *__restrict__ next, u32 *__restrict__ next_count) {
-    __shared__ u64 s_e0, s_e1;
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     u64 lo = (u64)blockIdx.x * DO_CHUNK, hi = lo + DO_CHUNK;
     if (hi > total) hi = total;
-    if (tid == 0) {
-        s_e0 = do_find_le(cum, 0, nf - 1, lo);
-        s_e1 = do_find_le(cum, 0, nf - 1, hi - 1);
-    }
-    __syncthreads();
-    u64 e0 = s_e0, e1 = s_e1;
-    for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
-        u64 e = do_find_le(cum, e0, e1, t0);
-        u64 t = t0 + lane;
-        if (t < hi) {
-            while (e < e1 && cum[e + 1] <= t) e++;
-            u32 u = fr[e];
-            u32 v = Aj[start[e] + (t - cum[e])];
-            if (PHASE == 0) {
-                if (level[v] < 0) atomicMin((unsigned long long *)&cand[v], (unsigned long long)u);
-            } else {
-                // level[v] is only ever written here, by the unique (u,v) with u == cand[v]
-                if (cand[v] == (u64)u && level[v] < 0) {
-                    level[v] = next_level;
-                    if (parent) parent[v] = (i64)u;
-                    next[atomicAdd(next_count, 1u)] = v;
-                }
+    for_each_flop(cum, 0, nf, lo, hi, [&](u64 e, u64 t) {
+        u32 u = fr[e];
+        u32 v = Aj[start[e] + (t - cum[e])];
+        if (PHASE == 0) {
+            if (level[v] < 0) atomicMin((unsigned long long *)&cand[v], (unsigned long long)u);
+        } else {
+            // level[v] is only ever written here, by the unique (u,v) with u == cand[v]
+            if (cand[v] == (u64)u && level[v] < 0) {
+                level[v] = next_level;
+                if (parent) parent[v] = (i64)u;
+                next[atomicAdd(next_count, 1u)] = v;
             }
         }
-    }
+    });
 }
 
 // ---------------------------------------------------------------------------------------------- driver

@@ -19,14 +19,9 @@ __global__ void k_bits_scatter(const u64 *__restrict__ Ap, const u32 *__restrict
     u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
     for (; q < nnz; q += stride) {
-        // row = largest r with Ap[r] <= q
-        u64 lo = 0, hi = nrows - 1;
-        while (lo < hi) {
-            u64 mid = (lo + hi + 1) >> 1;
-            if (Ap[mid] <= q) lo = mid; else hi = mid - 1;
-        }
+        const u64 r = last_le(Ap, 0, nrows - 1, q);   // the row of entry q
         u32 col = Aj[q];
-        atomicOr((unsigned long long *)&X[(u64)col * W + (lo >> 6)], 1ULL << (lo & 63));
+        atomicOr((unsigned long long *)&X[(u64)col * W + (r >> 6)], 1ULL << (r & 63));
     }
 }
 
@@ -271,10 +266,8 @@ void bits_to_csr(const DevBits &X, DevCSR &C) {
     require_natural(X, "bits_to_csr");
     u64 n = X.ncols;
     u32 W = X.W;
-    C.clear();
-    C.nrows = X.nrows; C.ncols = n;
-    C.p.alloc(X.nrows + 1);
-    if (n == 0) { C.p.zero(); C.nnz = 0; return; }
+    csr_shape(C, X.nrows, n);
+    if (n == 0) { C.p.zero(); return; }
     u64 ntiles = (n + TILE_V - 1) / TILE_V;
     u64 ncnt = (u64)64 * W * ntiles;
     DevBuf<u32> tc(ncnt + 1);

@@ -50,30 +50,17 @@ template <int W>
 __global__ void __launch_bounds__(256)
 k_bits_push(const u32 *__restrict__ act, const u64 *__restrict__ cum, const u64 *__restrict__ astart, u64 nact,
             u64 total, const u32 *__restrict__ Aj, const u64 *__restrict__ X, u64 *__restrict__ Y) {
-    __shared__ u64 s_e0, s_e1;
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     u64 lo = (u64)blockIdx.x * PUSH_CHUNK, hi = lo + PUSH_CHUNK;
     if (hi > total) hi = total;
-    if (tid == 0) {
-        s_e0 = find_le64(cum, 0, nact - 1, lo);
-        s_e1 = find_le64(cum, 0, nact - 1, hi - 1);
-    }
-    __syncthreads();
-    u64 e0 = s_e0, e1 = s_e1;
-    for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
-        u64 e = find_le64(cum, e0, e1, t0);
-        u64 t = t0 + lane;
-        if (t < hi) {
-            while (e < e1 && cum[e + 1] <= t) e++;
-            u32 k = act[e];
-            u32 col = Aj[astart[e] + (t - cum[e])];
+    for_each_flop(cum, 0, nact, lo, hi, [&](u64 e, u64 t) {
+        u32 k = act[e];
+        u32 col = Aj[astart[e] + (t - cum[e])];
 #pragma unroll
-            for (int w = 0; w < W; w++) {
-                u64 xw = X[(u64)k * W + w];
-                if (xw) atomicOr((unsigned long long *)&Y[(u64)col * W + w], xw);
-            }
+        for (int w = 0; w < W; w++) {
+            u64 xw = X[(u64)k * W + w];
+            if (xw) atomicOr((unsigned long long *)&Y[(u64)col * W + w], xw);
         }
-    }
+    });
 }
 
 // ---------------------------------------------------------------------------- pull

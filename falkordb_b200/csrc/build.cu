@@ -23,12 +23,6 @@ __global__ void k_pack_keys(const u64 *__restrict__ I, const u64 *__restrict__ J
     }
 }
 
-__global__ void k_iota_u64(u64 *__restrict__ v, u64 n) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; t < n; t += stride) v[t] = t;
-}
-
 __global__ void k_mark_heads(const u64 *__restrict__ keys, u64 n, u32 *__restrict__ head) {
     u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
@@ -60,13 +54,8 @@ __global__ void k_rowptr_from_keys(const u64 *__restrict__ keys, const u64 *__re
     u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
     for (; r <= nrows; r += stride) {
-        u64 target = r << 32;
-        u64 lo = 0, hi = n;
-        if (r >= ((u64)1 << 32)) lo = n; // cannot happen for device matrices (nrows < 2^32)
-        while (lo < hi) {
-            u64 mid = (lo + hi) >> 1;
-            if (keys[mid] < target) lo = mid + 1; else hi = mid;
-        }
+        // r >= 2^32 cannot happen for device matrices (nrows < 2^32)
+        const u64 lo = lb64(keys, r >= ((u64)1 << 32) ? n : 0, n, r << 32);
         u64 v;
         if (lo == n) v = n ? pos[n - 1] + head[n - 1] : 0;
         else v = pos[lo];
@@ -77,10 +66,8 @@ __global__ void k_rowptr_from_keys(const u64 *__restrict__ keys, const u64 *__re
 // sorted keys (ascending; INVALID_KEY entries at the end are dropped; duplicates collapse)
 static void csr_from_sorted_keys(const u64 *keys, u64 n, u64 nrows, u64 ncols, const u64 *perm,
                                  const u64 *vals_src, DevCSR &out) {
-    out.clear();
-    out.nrows = nrows; out.ncols = ncols;
-    out.p.alloc(nrows + 1);
-    if (n == 0) { out.p.zero(); out.nnz = 0; return; }
+    csr_shape(out, nrows, ncols);
+    if (n == 0) { out.p.zero(); return; }
     DevBuf<u32> head(n);
     DevBuf<u64> pos(n);
     LAUNCH(k_mark_heads, grid_for(n, 256, 1 << 20), 256, 0, keys, n, head.ptr);
@@ -117,7 +104,7 @@ void build_from_device_coo(const u64 *dI, const u64 *dJ, const u64 *dX, u64 n, u
     if (dX) {
         // stable radix sort => within a run of duplicates the first tuple in input order leads
         DevBuf<u64> perm(n);
-        LAUNCH(k_iota_u64, grid_for(n, 256, 1 << 20), 256, 0, perm.ptr, n);
+        iota_u64(perm.ptr, n);
         sort_pairs_u64(keys.ptr, perm.ptr, n, 64);
         csr_from_sorted_keys(keys.ptr, n, nrows, ncols, perm.ptr, dX, out);
     } else {
@@ -169,7 +156,7 @@ void tensor_bulk_build(const u64 *dI, const u64 *dJ, const u64 *dID, u64 n, u64 
     DevBuf<u64> xval(n), iota(n), pos(n);
     DevBuf<u32> multi(n);
     LAUNCH(k_bulk_mark, grid_for(n, 256, 1 << 20), 256, 0, keys.ptr, ids.ptr, n, xval.ptr, multi.ptr);
-    LAUNCH(k_iota_u64, grid_for(n, 256, 1 << 20), 256, 0, iota.ptr, n);
+    iota_u64(iota.ptr, n);
     csr_from_sorted_keys(keys.ptr, n, nrows, ncols, iota.ptr, xval.ptr, fwd);
     exclusive_scan_u32_to_u64(multi.ptr, pos.ptr, n);
     const u64 nm = read_scalar(pos.ptr + (n - 1)) + read_scalar(multi.ptr + (n - 1));
@@ -204,7 +191,7 @@ void transpose_csr(const DevCSR &A, DevCSR &out, bool keep_values) {
     int eb = key_bits(A.ncols);
     if (keep_values && A.has_values()) {
         DevBuf<u64> perm(n);
-        LAUNCH(k_iota_u64, grid_for(n, 256, 1 << 20), 256, 0, perm.ptr, n);
+        iota_u64(perm.ptr, n);
         sort_pairs_u64(keys.ptr, perm.ptr, n, eb);
         csr_from_sorted_keys(keys.ptr, n, A.ncols, A.nrows, perm.ptr, A.x.ptr, out);
     } else {
@@ -228,26 +215,6 @@ __device__ inline u64 scramble(u64 v, int scale, u64 k1, u64 k2) {
     v = (v * k2) & mask;
     v ^= v >> sh;
     return v & mask;
-}
-
-__global__ void k_rmat_keys(int scale, u64 nedges, u64 seed, u64 k1, u64 k2, u64 *__restrict__ keys) {
-    const u32 TA = (u32)(0.57 * 4294967296.0), TB = (u32)((0.57 + 0.19) * 4294967296.0),
-              TC = (u32)((0.57 + 0.19 + 0.19) * 4294967296.0);
-    u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; e < nedges; e += stride) {
-        u64 r = 0, c = 0, h = 0;
-        for (int l = 0; l < scale; l++) {
-            if ((l & 1) == 0) h = splitmix64(seed * 0xD1342543DE82EF95ULL + e * 64 + (u64)(l >> 1));
-            u32 u = (l & 1) ? (u32)(h >> 32) : (u32)h;
-            u32 rb, cb;
-            if (u < TA) { rb = 0; cb = 0; } else if (u < TB) { rb = 0; cb = 1; }
-            else if (u < TC) { rb = 1; cb = 0; } else { rb = 1; cb = 1; }
-            r = (r << 1) | rb; c = (c << 1) | cb;
-        }
-        u64 i = scramble(r, scale, k1, k2), j = scramble(c, scale, k1, k2);
-        keys[e] = (i == j) ? INVALID_KEY : ((i << 32) | j);
-    }
 }
 
 // Row block [lo,hi) of the same RMAT matrix (by_col: row block of its transpose).  Every rank regenerates the global
@@ -288,12 +255,7 @@ void rmat_block_csr(int scale, u64 edge_factor, u64 seed, u64 lo, u64 hi, int by
 
 void rmat_csr(int scale, u64 edge_factor, u64 seed, DevCSR &out) {
     if (scale < 1 || scale > 31) throw GrbError(-3, "rmat scale must be in [1,31]");
-    u64 n = (u64)1 << scale, ne = n * edge_factor;
-    u64 k1 = splitmix64(seed ^ 0xA5A5A5A5ULL) | 1ULL, k2 = splitmix64(seed ^ 0x5A5A5A5AULL) | 1ULL;
-    DevBuf<u64> keys(ne);
-    LAUNCH(k_rmat_keys, grid_for(ne, 256, 1 << 20), 256, 0, scale, ne, seed, k1, k2, keys.ptr);
-    sort_keys_u64(keys.ptr, ne, 64);
-    csr_from_sorted_keys(keys.ptr, ne, n, n, nullptr, nullptr, out);
+    rmat_block_csr(scale, edge_factor, seed, 0, (u64)1 << scale, 0, out);
 }
 
 } // namespace b200

@@ -251,6 +251,52 @@ __device__ __forceinline__ void st_u64_stream(u64 *p, u64 v, u64 pol) {
 __device__ __forceinline__ void st_u32_stream(u32 *p, u32 v, u64 pol) {
     asm volatile("st.global.L2::cache_hint.u32 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
 }
+
+// ---- searches over ascending arrays ----
+// the first position in j[lo, hi) whose value is not below c
+__device__ __forceinline__ u64 lb32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
+    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] < c) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+__device__ __forceinline__ u64 lb64(const u64 *__restrict__ k, u64 lo, u64 hi, u64 key) {
+    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (k[mid] < key) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+// the first position in j[lo, hi) whose value is above c
+__device__ __forceinline__ u64 ub32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
+    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] <= c) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+// the largest i in [lo, hi] with a[i] <= x (a[lo] <= x)
+__device__ __forceinline__ u64 last_le(const u64 *__restrict__ a, u64 lo, u64 hi, u64 x) {
+    while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (a[mid] <= x) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
+// The flop-balanced walk of a CTA over flops [lo, hi) (lo < hi) of the flat expansion behind cum, the scan of the lengths of
+// entries [e_first, e_end): f(e, t) for every flop t, e the last of those entries with cum[e] <= t (t - cum[e] is the flop's
+// place in entry e).  Thread 0 finds the CTA's first and last entry, then each warp takes 32 consecutive flops at a time and
+// advances its lanes from one search.  Assumes 256-thread CTAs (8 warps); every thread of the CTA must call it.  f computes
+// t - cum[e] itself: computed here, ahead of f's own loads, it changes the callers' code and register counts.
+template <class F>
+__device__ __forceinline__ void for_each_flop(const u64 *cum, u64 e_first, u64 e_end, u64 lo, u64 hi, F &&f) {
+    __shared__ u64 s_e0, s_e1;
+    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        s_e0 = last_le(cum, e_first, e_end - 1, lo);
+        s_e1 = last_le(cum, e_first, e_end - 1, hi - 1);
+    }
+    __syncthreads();
+    const u64 e0 = s_e0, e1 = s_e1;
+    for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
+        u64 e = last_le(cum, e0, e1, t0);
+        const u64 t = t0 + lane;
+        if (t < hi) {
+            while (e < e1 && cum[e + 1] <= t) e++;
+            f(e, t);
+        }
+    }
+}
 #endif
 
 // ---- primitive wrappers implemented in prims.cu (CUB scan / sort) ----------------------------
@@ -260,6 +306,20 @@ void sort_keys_u64(u64 *keys_in_out, size_t n, int end_bit);            // ascen
 void sort_pairs_u64(u64 *keys_in_out, u64 *vals_in_out, size_t n, int end_bit); // stable
 u64 reduce_sum_u64(const u64 *in, size_t n);
 void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz);  // every CSR row's entries ascending, in place (uses temp)
+
+// ---- element-wise one-liners (prims.cu) ----
+void iota_u64(u64 *p, u64 n);                     // p[i] = i
+void fill_u64(u64 *p, u64 v, u64 n);
+void fill_u32(u32 *p, u32 v, u64 n);
+void widen_u32(const u32 *in, u64 *out, u64 n);
+void narrow_u64(const u64 *in, u32 *out, u64 n);  // the low 32 bits
+
+// ---- CSR results built from per-row counts (prims.cu) ----
+// out emptied and shaped nrows x ncols, with room for its row pointers
+void csr_shape(DevCSR &out, u64 nrows, u64 ncols);
+// out's row pointers from the counts of its first `counted` rows (cnt holds out.nrows + 1 slots; the rest are zeroed here), then
+// out.nnz and room for its column ids, and for its values when asked; returns out.nnz
+u64 csr_rows_from_counts(u32 *cnt, u64 counted, DevCSR &out, bool values);
 
 // ---- sorted u64 keys (prims.cu) ----
 // head[e] = 1 where a run of equal keys of keys[0 .. n) starts (head[n] = 0), hpos its exclusive scan; returns the runs

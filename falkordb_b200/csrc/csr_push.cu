@@ -59,31 +59,18 @@ template <int W, bool ANDNOT, bool SLICED = false, u64 CHUNK = PUSH_CHUNK>
 __global__ void __launch_bounds__(256)
 k_csr_push(const u32 *__restrict__ erow, const u32 *__restrict__ Fj, const u64 *__restrict__ cum, u64 nent, u64 total,
            const u64 *__restrict__ Ap, const u32 *__restrict__ Aj, u64 *__restrict__ Y, const u32 *__restrict__ perm) {
-    __shared__ u64 s_e0, s_e1;
-    const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     u64 lo = (u64)blockIdx.x * CHUNK, hi = lo + CHUNK;
     if (hi > total) hi = total;
-    if (tid == 0) {
-        s_e0 = find_le64(cum, 0, nent - 1, lo);
-        s_e1 = find_le64(cum, 0, nent - 1, hi - 1);
-    }
-    __syncthreads();
-    u64 e0 = s_e0, e1 = s_e1;
-    for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
-        u64 e = find_le64(cum, e0, e1, t0);
-        u64 t = t0 + lane;
-        if (t < hi) {
-            while (e < e1 && cum[e + 1] <= t) e++;
-            const u32 i = erow[e];
-            u32 col = Aj[(SLICED ? Ap[e] : Ap[Fj[e]]) + (t - cum[e])];
-            // hot-set order through the table (the deltas, which have no relabelled copy); a prepared operand passes its
-            // relabelled col_idx (PullTables::ap) as Aj instead, with perm null
-            if (perm) col = __ldg(perm + col);
-            unsigned long long *dst = (unsigned long long *)&Y[(u64)col * W + (i >> 6)];
-            if (ANDNOT) atomicAnd(dst, ~(1ULL << (i & 63)));
-            else atomicOr(dst, 1ULL << (i & 63));
-        }
-    }
+    for_each_flop(cum, 0, nent, lo, hi, [&](u64 e, u64 t) {
+        const u32 i = erow[e];
+        u32 col = Aj[(SLICED ? Ap[e] : Ap[Fj[e]]) + (t - cum[e])];
+        // hot-set order through the table (the deltas, which have no relabelled copy); a prepared operand passes its
+        // relabelled col_idx (PullTables::ap) as Aj instead, with perm null
+        if (perm) col = __ldg(perm + col);
+        unsigned long long *dst = (unsigned long long *)&Y[(u64)col * W + (i >> 6)];
+        if (ANDNOT) atomicAnd(dst, ~(1ULL << (i & 63)));
+        else atomicOr(dst, 1ULL << (i & 63));
+    });
 }
 template <int W>
 static void csr_push_impl(const DevCSR &F, const DevCSR &A, const u32 *Aj, DevBits &Y, u64 flops, const u32 *erow, const u64 *cum,
@@ -247,15 +234,15 @@ k_bits_delta(const u64 *__restrict__ Dp, const u32 *__restrict__ Dj, u64 nrows, 
     __shared__ u64 s_r0, s_r1;
     const u64 lo = (u64)blockIdx.x * DELTA_CHUNK;
     const u64 hi = lo + DELTA_CHUNK < nnz ? lo + DELTA_CHUNK : nnz;
-    if (threadIdx.x == 0) s_r0 = find_le64(Dp, 0, nrows - 1, lo);          // the two bounds are independent searches
-    if (threadIdx.x == 32) s_r1 = find_le64(Dp, 0, nrows - 1, hi - 1);
+    if (threadIdx.x == 0) s_r0 = last_le(Dp, 0, nrows - 1, lo);            // the two bounds are independent searches
+    if (threadIdx.x == 32) s_r1 = last_le(Dp, 0, nrows - 1, hi - 1);
     __syncthreads();
     const u64 r1 = s_r1;
     u64 k = s_r0;
     const u32 h = threadIdx.x % SPLIT;
     u64 fl = 0;
     for (u64 q = lo + threadIdx.x / SPLIT; q < hi; q += EPS) {
-        k = find_le64(Dp, k, r1, q);                 // entries only move forward: the previous row bounds the search
+        k = last_le(Dp, k, r1, q);                   // entries only move forward: the previous row bounds the search
         const u64 j = __ldg(Dj + q);
         const u64 px = xperm ? __ldg(xperm + k) : k, py = yperm ? __ldg(yperm + j) : j;
         u64 x[WL];

@@ -35,25 +35,8 @@ struct ETypes {
     explicit ETypes(const std::vector<EdgeTypeDev> &types);   // edges.cu
 };
 
-__device__ __forceinline__ u64 lb32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
-    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] < c) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-// the first position in k[lo, hi) (ascending) whose key is not below key
-__device__ __forceinline__ u64 lb64(const u64 *__restrict__ k, u64 lo, u64 hi, u64 key) {
-    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (k[mid] < key) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-__device__ __forceinline__ u64 ub32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
-    while (lo < hi) { u64 mid = (lo + hi) >> 1; if (j[mid] <= c) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 // largest g with lstart[g] <= e (lstart ascending, lstart[0] = 0): the segment of flat position e behind a scan of lengths
-__device__ __forceinline__ u64 list_at(const u64 *__restrict__ lstart, u64 G, u64 e) {
-    u64 lo = 0, hi = G - 1;
-    while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (lstart[mid] <= e) lo = mid; else hi = mid - 1; }
-    return lo;
-}
+__device__ __forceinline__ u64 list_at(const u64 *__restrict__ lstart, u64 G, u64 e) { return last_le(lstart, 0, G - 1, e); }
 // position of (r, c) in A, or ~0
 __device__ __forceinline__ u64 find_rc(const ECsr &A, u64 r, u32 c) {
     if (!A.p) return ~0ULL;

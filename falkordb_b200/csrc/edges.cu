@@ -18,6 +18,7 @@
 // rows, and places the entries in Graph::get_node_relationships_by_type's order instead (k_ee_ref_fill): type, block, neighbour.
 // The me layers are host-resident (2^60 x 2^60); their sorted (key, ids) stores are uploaded once and cached on the handle.
 #include "edge_layers.cuh"
+#include <type_traits>
 
 namespace b200 {
 
@@ -267,8 +268,7 @@ u64 edge_adjacency(const ETypes &types, const u64 *d_src, u64 n, int dir, DevBuf
     return total;
 }
 
-template <class K>
-__global__ void k_adj_low(const K *__restrict__ key, u64 n, u64 *__restrict__ out) {
+__global__ void k_adj_low(const u64 *__restrict__ key, u64 n, u64 *__restrict__ out) {
     for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) out[i] = (u32)key[i];
 }
 template <class K>
@@ -291,7 +291,8 @@ void node_rows(const K *keys, u64 n, const u64 *u, u64 nu, const u64 *adj_p, u32
 template <class K>
 void NodeAdj::fetch(const ETypes &types, const K *keys, u64 n, int dir, bool want_tb, u64 *bytes) {
     u.alloc(n);
-    LAUNCH(k_adj_low<K>, grid_for(n, 256), 256, 0, keys, n, u.ptr);
+    if constexpr (std::is_same<K, u32>::value) widen_u32(keys, u.ptr, n);
+    else LAUNCH(k_adj_low, grid_for(n, 256), 256, 0, keys, n, u.ptr);
     const u64 nu = unique_sorted(u, n, 32);
     edge_adjacency(types, u.ptr, nu, dir, p, node, edge, bytes, want_tb ? &tb : nullptr);
     row.alloc(n);

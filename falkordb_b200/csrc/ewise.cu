@@ -11,29 +11,12 @@
 
 namespace b200 {
 
-__global__ void k_fill_u64(u64 *__restrict__ p, u64 v, u64 n) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; t < n; t += stride) p[t] = v;
-}
-void fill_u64(u64 *p, u64 v, u64 n) { if (n) LAUNCH(k_fill_u64, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, p, v, n); }
-void fill_i64(i64 *p, i64 v, u64 n) { fill_u64((u64 *)p, (u64)v, n); }
-
-// lower bound of c in j[lo,hi); found <=> j[result]==c
-__device__ __forceinline__ u64 lower_bound_u32(const u32 *__restrict__ j, u64 lo, u64 hi, u32 c) {
-    while (lo < hi) {
-        u64 mid = (lo + hi) >> 1;
-        if (j[mid] < c) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
 // ---- predicates -------------------------------------------------------------------------------
 struct MaskPred {
     const u64 *Mp; const u32 *Mj; const u64 *Mx; bool comp, structural;
     __device__ bool operator()(u64 i, u32 c, u64) const {
         u64 s = Mp[i], e = Mp[i + 1];
-        u64 q = lower_bound_u32(Mj, s, e, c);
+        u64 q = lb32(Mj, s, e, c);
         bool in = (q < e && Mj[q] == c);
         if (in && !structural && Mx) in = (Mx[q] != 0);
         return in != comp;
@@ -100,21 +83,14 @@ __global__ void k_rowfilter_fill(const u64 *__restrict__ Tp, const u32 *__restri
 
 template <class Pred>
 static void rowfilter(const DevCSR &T, Pred pred, u64 out_nrows, u64 out_ncols, bool keep_values, DevCSR &out) {
-    out.clear();
-    out.nrows = out_nrows; out.ncols = out_ncols;
-    out.p.alloc(out_nrows + 1);
+    csr_shape(out, out_nrows, out_ncols);
     u64 rows = T.nrows < out_nrows ? T.nrows : out_nrows;
-    if (T.nnz == 0 || rows == 0) { out.p.zero(); out.nnz = 0; return; }
+    if (T.nnz == 0 || rows == 0) { out.p.zero(); return; }
     DevBuf<u32> cnt(out_nrows + 1);
-    cnt.zero();
     timed_begin(TK_FILTER);
     LAUNCH((k_rowfilter_count<Pred>), grid_for(rows * 32, 256, (u64)ctx().num_sms * 32), 256, 0, T.p.ptr, T.j.ptr, rows, pred, cnt.ptr);
-    exclusive_scan_u32_to_u64(cnt.ptr, out.p.ptr, out_nrows + 1);
-    u64 nnz = read_scalar(out.p.ptr + out_nrows);
-    out.nnz = nnz;
-    out.j.alloc(nnz);
     bool vals = keep_values && T.has_values();
-    if (vals) out.x.alloc(nnz);
+    u64 nnz = csr_rows_from_counts(cnt.ptr, rows, out, vals);
     if (nnz)
         LAUNCH((k_rowfilter_fill<Pred>), grid_for(rows * 32, 256, (u64)ctx().num_sms * 32), 256, 0, T.p.ptr, T.j.ptr,
                vals ? T.x.ptr : (const u64 *)nullptr, rows, pred, out.p.ptr, out.j.ptr, vals ? out.x.ptr : (u64 *)nullptr);
@@ -196,14 +172,14 @@ k_masked_pairs(const u32 *__restrict__ Arid, const u32 *__restrict__ Aj, u64 nnz
         if (be - bs <= me - ms) {                         // B(k,:) drives, probe M(i,:)
             for (u64 q = bs + lane; q < be; q += 32) {
                 u32 j = Bj[q];
-                u64 pos = lower_bound_u32(Mj, ms, me, j);
+                u64 pos = lb32(Mj, ms, me, j);
                 if (pos < me && Mj[pos] == j) atomicOr(&flag[pos >> 5], 1u << (pos & 31));
             }
         } else {                                          // M(i,:) drives, probe B(k,:); skip already-flagged entries
             for (u64 pz = ms + lane; pz < me; pz += 32) {
                 if ((flag[pz >> 5] >> (pz & 31)) & 1u) continue;
                 u32 j = Mj[pz];
-                u64 pos = lower_bound_u32(Bj, bs, be, j);
+                u64 pos = lb32(Bj, bs, be, j);
                 if (pos < be && Bj[pos] == j) atomicOr(&flag[pz >> 5], 1u << (pz & 31));
             }
         }
@@ -250,7 +226,7 @@ __global__ void k_union_count(const u64 *__restrict__ Ap, const u32 *__restrict_
                 bool hit = false;
                 if (q < se) {
                     u32 c = Sj[q];
-                    u64 r = lower_bound_u32(Lj, ls, le, c);
+                    u64 r = lb32(Lj, ls, le, c);
                     hit = (r < le && Lj[r] == c);
                 }
                 common += __popc(__ballot_sync(0xffffffffu, hit));
@@ -280,7 +256,7 @@ __global__ void k_union_fill(const u64 *__restrict__ Ap, const u32 *__restrict__
             u64 r = bs;
             if (valid) {
                 c = Aj[q];
-                r = lower_bound_u32(Bj, bs, be, c);
+                r = lb32(Bj, bs, be, c);
                 hit = (r < be && Bj[r] == c);
             }
             u32 m = __ballot_sync(0xffffffffu, hit);
@@ -299,7 +275,7 @@ __global__ void k_union_fill(const u64 *__restrict__ Ap, const u32 *__restrict__
             u64 r = as;
             if (valid) {
                 c = Bj[q];
-                r = lower_bound_u32(Aj, as, ae, c);
+                r = lb32(Aj, as, ae, c);
                 hit = (r < ae && Aj[r] == c);
             }
             u32 m = __ballot_sync(0xffffffffu, hit);
@@ -316,20 +292,13 @@ __global__ void k_union_fill(const u64 *__restrict__ Ap, const u32 *__restrict__
 void ewise_union(const DevCSR &A, const DevCSR &B, bool keep_values, DevCSR &out) {
     if (A.nrows != B.nrows || A.ncols != B.ncols) throw GrbError(-6, "eWiseAdd dimensions differ");
     u64 nrows = A.nrows;
-    out.clear();
-    out.nrows = nrows; out.ncols = A.ncols;
-    out.p.alloc(nrows + 1);
-    if (nrows == 0 || (A.nnz == 0 && B.nnz == 0)) { out.p.zero(); out.nnz = 0; return; }
+    csr_shape(out, nrows, A.ncols);
+    if (nrows == 0 || (A.nnz == 0 && B.nnz == 0)) { out.p.zero(); return; }
     DevBuf<u32> cnt(nrows + 1);
-    CUDA_TRY(cudaMemsetAsync(cnt.ptr + nrows, 0, sizeof(u32), stream()));
     timed_begin(TK_UNION);
     LAUNCH(k_union_count, grid_for(nrows * 32, 256, (u64)ctx().num_sms * 32), 256, 0, A.p.ptr, A.j.ptr, B.p.ptr, B.j.ptr, nrows, cnt.ptr);
-    exclusive_scan_u32_to_u64(cnt.ptr, out.p.ptr, nrows + 1);
-    u64 nnz = read_scalar(out.p.ptr + nrows);
-    out.nnz = nnz;
-    out.j.alloc(nnz);
     bool vals = keep_values && (A.has_values() || B.has_values());
-    if (vals) out.x.alloc(nnz);
+    u64 nnz = csr_rows_from_counts(cnt.ptr, nrows, out, vals);
     if (nnz)
         LAUNCH(k_union_fill, grid_for(nrows * 32, 256, (u64)ctx().num_sms * 32), 256, 0, A.p.ptr, A.j.ptr,
                A.has_values() ? A.x.ptr : (const u64 *)nullptr, B.p.ptr, B.j.ptr,
@@ -353,7 +322,7 @@ __global__ void k_probe_pairs(const u64 *__restrict__ Ap, const u32 *__restrict_
         u64 v = 0;
         if (i < nrows && j < ncols) {
             u64 s = Ap[i], e = Ap[i + 1];
-            u64 q = lower_bound_u32(Aj, s, e, (u32)j);
+            u64 q = lb32(Aj, s, e, (u32)j);
             if (q < e && Aj[q] == (u32)j) { hit = true; v = Ax ? Ax[q] : 1ULL; }
         }
         found[t] = hit ? 1 : 0;
@@ -371,14 +340,7 @@ __global__ void k_rowptr_from_hyper(const u64 *__restrict__ hrow, const u64 *__r
                                     u64 *__restrict__ p) {
     u64 r = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; r <= nrows; r += stride) {
-        u64 lo = 0, hi = nvec;
-        while (lo < hi) {
-            u64 mid = (lo + hi) >> 1;
-            if (hrow[mid] < r) lo = mid + 1; else hi = mid;
-        }
-        p[r] = hptr[lo];
-    }
+    for (; r <= nrows; r += stride) p[r] = hptr[lb64(hrow, 0, nvec, r)];
 }
 void rowptr_from_hyper(const u64 *d_hrow, const u64 *d_hptr, u64 nvec, u64 nrows, u64 *d_p) {
     LAUNCH(k_rowptr_from_hyper, grid_for(nrows + 1, 256, (u64)ctx().num_sms * 16), 256, 0, d_hrow, d_hptr, nvec, nrows, d_p);
@@ -410,19 +372,6 @@ u64 hyper_from_rowptr(const u64 *d_p, u64 nrows, u64 nnz, DevBuf<u64> &d_hrow, D
     return nvec;
 }
 
-__global__ void k_widen_u32(const u32 *__restrict__ in, u64 *__restrict__ out, u64 n) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; t < n; t += stride) out[t] = in[t];
-}
-__global__ void k_narrow_u64(const u64 *__restrict__ in, u32 *__restrict__ out, u64 n) {
-    u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; t < n; t += stride) out[t] = (u32)in[t];
-}
-void widen_u32(const u32 *in, u64 *out, u64 n) { if (n) LAUNCH(k_widen_u32, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, in, out, n); }
-void narrow_u64(const u64 *in, u32 *out, u64 n) { if (n) LAUNCH(k_narrow_u64, grid_for(n, 256, (u64)ctx().num_sms * 16), 256, 0, in, out, n); }
-
 
 // ---- order-sensitive digest of a CSR pattern (full-size parity checks: a multi-GB result is compared by three numbers) ----
 // key = row << 32 | col, position q = index in CSR order:  d[0] = nnz, d[1] = sum mix(key), d[2] = sum mix(key + GOLD * (q + 1)).
@@ -437,11 +386,7 @@ __global__ void __launch_bounds__(256) k_csr_digest(const u64 *__restrict__ p, c
     u64 s1 = 0, s2 = 0;
     u64 row = 0;                                   // rows only move forward along a thread's ascending positions
     for (; q < nnz; q += stride) {
-        if (p[row + 1] <= q) {                     // largest row with p[row] <= q, searched in (row, nrows)
-            u64 lo = row + 1, hi = nrows - 1;
-            while (lo < hi) { u64 mid = (lo + hi + 1) >> 1; if (p[mid] <= q) lo = mid; else hi = mid - 1; }
-            row = lo;
-        }
+        if (p[row + 1] <= q) row = last_le(p, row + 1, nrows - 1, q);   // largest row with p[row] <= q, searched in (row, nrows)
         const u64 key = (row << 32) | j[q];
         s1 += mix64(key);
         s2 += mix64(key + 0x9E3779B97F4A7C15ULL * (q + 1));

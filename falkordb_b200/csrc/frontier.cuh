@@ -29,13 +29,6 @@ template <int W> struct PullCfg {
 };
 static const u64 PUSH_CHUNK = 8192;
 
-__device__ __forceinline__ u64 find_le64(const u64 *__restrict__ a, u64 lo, u64 hi, u64 target) {
-    while (lo < hi) {
-        u64 mid = (lo + hi + 1) >> 1;
-        if (a[mid] <= target) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
 template <int WL> __device__ __forceinline__ void ld_part(u64 (&x)[WL], const u64 *p) {
     static_assert(WL == 1 || WL == 2, "a record part is one 8- or 16-byte load");
     if constexpr (WL == 1) { x[0] = __ldg(p); }

@@ -218,11 +218,5 @@ void adj_layer(const DevCSR &L, const DevCSR *dm, u64 n_out, const u64 *d_keep, 
 // hypersparse host form <-> dense device rowptr (ewise.cu)
 void rowptr_from_hyper(const u64 *d_hrow, const u64 *d_hptr, u64 nvec, u64 nrows, u64 *d_p);
 u64 hyper_from_rowptr(const u64 *d_p, u64 nrows, u64 nnz, DevBuf<u64> &d_hrow, DevBuf<u64> &d_hptr);
-void widen_u32(const u32 *in, u64 *out, u64 n);
-void narrow_u64(const u64 *in, u32 *out, u64 n);
-
-// generic tiny helpers (ewise.cu)
-void fill_u64(u64 *p, u64 v, u64 n);
-void fill_i64(i64 *p, i64 v, u64 n);
 
 } // namespace b200

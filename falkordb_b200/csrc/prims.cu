@@ -270,11 +270,6 @@ __global__ void k_row_keys(const u64 *__restrict__ rowptr, u64 nrows, const u32 
     for (u64 r = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nrows; r += nwarps)
         for (u64 q = rowptr[r] + lane; q < rowptr[r + 1]; q += 32) keys[q] = (r << 32) | cols[q];
 }
-__global__ void k_keys_low(const u64 *__restrict__ keys, u64 n, u32 *__restrict__ out) {
-    u64 q = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    const u64 stride = (u64)gridDim.x * blockDim.x;
-    for (; q < n; q += stride) out[q] = (u32)keys[q];
-}
 void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz) {
     if (nnz <= 1) return;
     if (nrows > ((u64)1 << 32)) throw GrbError(-8, "sort_rows_u32: more than 2^32 rows not supported");
@@ -283,7 +278,41 @@ void sort_rows_u32(const u64 *rowptr, u64 nrows, u32 *cols, u64 nnz) {
     int row_bits = 1;
     while (row_bits < 32 && ((u64)1 << row_bits) < nrows) row_bits++;
     sort_keys_u64(keys.ptr, nnz, 32 + row_bits);
-    LAUNCH(k_keys_low, grid_for(nnz, 256, (u64)ctx().num_sms * 32), 256, 0, keys.ptr, nnz, cols);
+    narrow_u64(keys.ptr, cols, nnz);
+}
+
+__global__ void k_iota_u64(u64 *__restrict__ v, u64 n) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) v[i] = i;
+}
+template <class T>
+__global__ void k_fill(T *__restrict__ p, T v, u64 n) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) p[i] = v;
+}
+__global__ void k_widen_u32(const u32 *__restrict__ in, u64 *__restrict__ out, u64 n) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) out[i] = in[i];
+}
+__global__ void k_narrow_u64(const u64 *__restrict__ in, u32 *__restrict__ out, u64 n) {
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) out[i] = (u32)in[i];
+}
+static u32 small_grid(u64 n) { return grid_for(n, 256, (u64)ctx().num_sms * 16); }
+void iota_u64(u64 *p, u64 n) { if (n) LAUNCH(k_iota_u64, small_grid(n), 256, 0, p, n); }
+void fill_u64(u64 *p, u64 v, u64 n) { if (n) LAUNCH(k_fill<u64>, small_grid(n), 256, 0, p, v, n); }
+void fill_u32(u32 *p, u32 v, u64 n) { if (n) LAUNCH(k_fill<u32>, small_grid(n), 256, 0, p, v, n); }
+void widen_u32(const u32 *in, u64 *out, u64 n) { if (n) LAUNCH(k_widen_u32, small_grid(n), 256, 0, in, out, n); }
+void narrow_u64(const u64 *in, u32 *out, u64 n) { if (n) LAUNCH(k_narrow_u64, small_grid(n), 256, 0, in, out, n); }
+
+void csr_shape(DevCSR &out, u64 nrows, u64 ncols) {
+    out.clear();
+    out.nrows = nrows; out.ncols = ncols;
+    out.p.alloc(nrows + 1);
+}
+u64 csr_rows_from_counts(u32 *cnt, u64 counted, DevCSR &out, bool values) {
+    CUDA_TRY(cudaMemsetAsync(cnt + counted, 0, (out.nrows + 1 - counted) * sizeof(u32), stream()));
+    exclusive_scan_u32_to_u64(cnt, out.p.ptr, out.nrows + 1);
+    out.nnz = read_scalar(out.p.ptr + out.nrows);
+    out.j.alloc(out.nnz);
+    if (values) out.x.alloc(out.nnz);
+    return out.nnz;
 }
 
 __global__ void k_run_heads(const u64 *__restrict__ k, u64 n, u32 *__restrict__ head) {

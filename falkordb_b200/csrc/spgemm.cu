@@ -107,15 +107,6 @@ k_small_rows(const u32 *__restrict__ list, u32 nlist, const u64 *__restrict__ Ap
     }
 }
 
-__device__ __forceinline__ u64 find_le(const u64 *__restrict__ a, u64 lo, u64 hi, u64 target) {
-    // largest e in [lo,hi] with a[e] <= target (a ascending, a[lo] <= target)
-    while (lo < hi) {
-        u64 mid = (lo + hi + 1) >> 1;
-        if (a[mid] <= target) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-
 __global__ void k_chunk_counts(const u32 *__restrict__ hrows, u32 nh, const u64 *__restrict__ Ap,
                                const u64 *__restrict__ cum, u64 CH, u64 *__restrict__ nch) {
     u32 h = blockIdx.x * blockDim.x + threadIdx.x;
@@ -126,6 +117,8 @@ __global__ void k_chunk_counts(const u32 *__restrict__ hrows, u32 nh, const u64 
     nch[h] = (f + CH - 1) / CH;
 }
 
+// Walks its chunk as common.cuh's for_each_flop does, but in flops counted from the row's first (cum[a0]).  Handing
+// for_each_flop the global positions instead changes this kernel's code and takes 4 fewer registers than were measured.
 __global__ void __launch_bounds__(256)
 k_heavy_accumulate(const u32 *__restrict__ hrows, const u64 *__restrict__ choff, u32 nh, u64 CH,
                    const u64 *__restrict__ Ap, const u64 *__restrict__ cum, const u64 *__restrict__ bstart,
@@ -134,7 +127,7 @@ k_heavy_accumulate(const u32 *__restrict__ hrows, const u64 *__restrict__ choff,
     __shared__ u64 s_e0, s_e1;
     const u32 tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     u64 c = blockIdx.x;
-    if (tid == 0) s_h = (u32)find_le(choff, 0, nh - 1, c);
+    if (tid == 0) s_h = (u32)last_le(choff, 0, nh - 1, c);
     __syncthreads();
     u32 h = s_h;
     u32 row = hrows[h];
@@ -143,14 +136,14 @@ k_heavy_accumulate(const u32 *__restrict__ hrows, const u64 *__restrict__ choff,
     u64 lo = lc * CH, hi = lo + CH;
     if (hi > f) hi = f;
     if (tid == 0) {
-        s_e0 = find_le(cum, a0, a1 - 1, base + lo);
-        s_e1 = find_le(cum, a0, a1 - 1, base + hi - 1);
+        s_e0 = last_le(cum, a0, a1 - 1, base + lo);
+        s_e1 = last_le(cum, a0, a1 - 1, base + hi - 1);
     }
     __syncthreads();
     u64 e0 = s_e0, e1 = s_e1;
     u32 *bm = bitmap + (u64)h * wpr;
     for (u64 t0 = lo + (u64)warp * 32; t0 < hi; t0 += 8 * 32) {
-        u64 e = find_le(cum, e0, e1, base + t0);
+        u64 e = last_le(cum, e0, e1, base + t0);
         u64 t = t0 + lane;
         if (t < hi) {
             while (e < e1 && cum[e + 1] <= base + t) e++;
@@ -264,11 +257,9 @@ void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out)
     Context &cx = ctx();
     if (A.ncols != B.nrows) throw GrbError(-6, "mxm: inner dimensions differ");
     u64 nrows = A.nrows, ncols = B.ncols;
-    C.clear();
-    C.nrows = nrows; C.ncols = ncols;
-    C.p.alloc(nrows + 1);
+    csr_shape(C, nrows, ncols);
     if (flops_out) *flops_out = 0;
-    if (A.nnz == 0 || B.nnz == 0) { C.p.zero(); C.nnz = 0; return; }
+    if (A.nnz == 0 || B.nnz == 0) { C.p.zero(); return; }
 
     // 1. per-entry degrees, their prefix, and the B segment starts
     DevBuf<u64> cum(A.nnz + 1), bstart(A.nnz);
@@ -287,7 +278,7 @@ void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out)
     if (maybe_single) d2h(&hm, multi.ptr, 1);
     sync_stream();                                 // the only host round trip of the single-entry path
     if (flops_out) *flops_out = flops;
-    if (flops == 0) { C.p.zero(); C.nnz = 0; return; }
+    if (flops == 0) { C.p.zero(); return; }
     if (maybe_single) {
         if (!hm) {
             C.nnz = flops;
@@ -307,7 +298,6 @@ void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out)
     counts.zero();
     LAUNCH(k_classify, grid_for(nrows + 1, 256, 1 << 16), 256, 0, A.p.ptr, cum.ptr, nrows, cap, ub.ptr, l0.ptr, l1.ptr,
            l2.ptr, l3.ptr, counts.ptr, cnt.ptr);
-    CUDA_TRY(cudaMemsetAsync(cnt.ptr + nrows, 0, sizeof(u32), stream()));
     u32 hc[4];
     d2h(hc, counts.ptr, 4);
     exclusive_scan_u64(ub.ptr, ub.ptr, nrows + 1); // ub becomes toff
@@ -365,10 +355,7 @@ void spgemm_anypair(const DevCSR &A, const DevCSR &B, DevCSR &C, u64 *flops_out)
     }
 
     // 5. row pointers
-    exclusive_scan_u32_to_u64(cnt.ptr, C.p.ptr, nrows + 1);
-    u64 nnzC = read_scalar(C.p.ptr + nrows);
-    C.nnz = nnzC;
-    C.j.alloc(nnzC);
+    csr_rows_from_counts(cnt.ptr, nrows, C, false);
 
     // 6. fill
     if (hc[0]) LAUNCH(k_gather_small, grid_for((u64)hc[0] * 32, 256, 1 << 16), 256, 0, l0.ptr, hc[0], ub.ptr, tmp.ptr, C.p.ptr, C.j.ptr);

@@ -794,7 +794,7 @@ def test_pagerank_at_n_big(dev):
 
 # ------------------------------------------------------------------------------------------ LAGr_ConnectedComponents
 def wcc_dev(L, S):
-    """(component vector, rounds): the rounds from the launch count -- k_cc_init, then k_cc_hook + k_cc_jump per round"""
+    """(component vector, rounds): the rounds from the launch count -- k_iota_u64, then k_cc_hook + k_cc_jump per round"""
     G = _graph(L, S, 0)
     comp = P()
     l0 = fb.get_stat("launches")
@@ -860,7 +860,7 @@ def test_wcc_hard_graphs_at_n_big(dev):
 
 # ------------------------------------------------------------------------------------------ LAGraph_cdlp
 def cdlp_dev(L, S, itermax):
-    """(labels, rounds): the rounds from the launch count -- k_cc_init, then k_cdlp_keys + k_cdlp_pick per round"""
+    """(labels, rounds): the rounds from the launch count -- k_iota_u64, then k_cdlp_keys + k_cdlp_pick per round"""
     G = _graph(L, S, 0)
     out = P()
     l0 = fb.get_stat("launches")
